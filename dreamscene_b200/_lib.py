@@ -16,7 +16,8 @@ EXPORTS = ["b200gsr_version", "b200gsr_last_error", "b200gsr_saved_layout_query"
            "b200gsr_disparity_backward", "b200gsr_densify_stats", "b200gsr_densify_scratch_bytes",
            "b200gsr_densify_plan", "b200gsr_densify_map", "b200gsr_compact_plan", "b200gsr_gather_rows",
            "b200gsr_split_children", "b200gsr_kth_smallest", "b200gsr_views_geometry", "b200gsr_forward_views",
-           "b200gsr_backward_views", "b200gsr_sh_grad_expand"]
+           "b200gsr_backward_views", "b200gsr_sh_grad_expand", "b200gsr_backward_views_ex",
+           "b200gsr_disparity_backward_ex"]
 
 
 class Params(C.Structure):
@@ -62,7 +63,10 @@ class ScratchLayout(C.Structure):
 _lib = None
 ABI_VERSION = 3
 FWD_NO_BACKWARD = 1
+FWD_DETERMINISTIC = 2
 BWD_COMPOSITE, BWD_PROJECT = 1, 2
+BWD_DETERMINISTIC = 4
+SAVED_DETERMINISTIC = 0x100
 
 
 def load():
@@ -107,7 +111,9 @@ def load():
     lib.b200gsr_assemble_forward.restype = lib.b200gsr_assemble_backward.restype = C.c_int
     lib.b200gsr_disparity_forward.argtypes = [i32, i32, vp, vp, vp, vp, vp]
     lib.b200gsr_disparity_backward.argtypes = [i32, i32, vp, vp, vp, vp, vp, vp, vp]
+    lib.b200gsr_disparity_backward_ex.argtypes = [i32, i32, vp, vp, vp, vp, vp, vp, u32, vp]
     lib.b200gsr_disparity_forward.restype = lib.b200gsr_disparity_backward.restype = C.c_int
+    lib.b200gsr_disparity_backward_ex.restype = C.c_int
     f = C.c_float
     lib.b200gsr_densify_stats.argtypes = [i32, vp, vp, vp, vp, vp, vp]
     lib.b200gsr_densify_scratch_bytes.argtypes = [i32]
@@ -126,7 +132,8 @@ def load():
                                           u64, u32, vp, u32, vp]
     lib.b200gsr_backward_views.argtypes = [i32, C.POINTER(Params), C.POINTER(ViewInputs), vp, vp, vp, vp, vp, sz, u64,
                                            C.POINTER(ViewGrads), vp]
-    for fn in ("b200gsr_views_geometry", "b200gsr_forward_views", "b200gsr_backward_views"):
+    lib.b200gsr_backward_views_ex.argtypes = lib.b200gsr_backward_views.argtypes[:-1] + [u32, vp]
+    for fn in ("b200gsr_views_geometry", "b200gsr_forward_views", "b200gsr_backward_views", "b200gsr_backward_views_ex"):
         getattr(lib, fn).restype = C.c_int
     lib.b200gsr_debug_counters.argtypes = [vp]
     lib.b200gsr_debug_counters.restype = C.c_int
@@ -149,9 +156,13 @@ def last_error() -> str:
     return load().b200gsr_last_error().decode("utf-8", "replace")
 
 
-def saved_layout(P: int, H: int, W: int, max_pairs: int, with_backward: bool = True) -> SavedLayout:
+def saved_layout(P: int, H: int, W: int, max_pairs: int, with_backward: bool = True,
+                 deterministic: bool = False) -> SavedLayout:
+    """deterministic: `total` also covers the fixed-point accumulators of deterministic mode (appended; every
+    offset is the same as without)."""
     out = SavedLayout()
-    rc = load().b200gsr_saved_layout_query(P, H, W, max_pairs, int(bool(with_backward)), C.byref(out))
+    flag = int(bool(with_backward)) | (SAVED_DETERMINISTIC if deterministic else 0)
+    rc = load().b200gsr_saved_layout_query(P, H, W, max_pairs, flag, C.byref(out))
     if rc:
         raise RuntimeError(f"b200gsr_saved_layout_query failed ({rc}): {last_error()}")
     return out

@@ -120,6 +120,28 @@ int validate_inputs(const b200gsr_params* p, const float* means3D, const float* 
     return B200GSR_OK;
 }
 
+// The deterministic accumulators (GsrDetLayout) follow everything b200gsr_saved_layout describes, so that layout's
+// offsets and its total without B200GSR_SAVED_DETERMINISTIC stay what they always were.
+GsrDetLayout det_layout(int32_t P, size_t base, bool with_backward) {
+    GsrDetLayout d{};
+    size_t off = base;
+    if (with_backward) {
+        d.dmax = off; off = align_up(off + (size_t)P * GSR_DET_COMPONENTS * sizeof(uint32_t));
+        d.dfx = off;  off = align_up(off + (size_t)P * GSR_DET_COMPONENTS * sizeof(unsigned long long));
+    }
+    d.score_fx = off; off = align_up(off + (size_t)P * sizeof(unsigned long long));
+    d.total = off;
+    return d;
+}
+
+// Deterministic sums have overflow headroom for GSR_DET_MAX_VIEW_TILES tiles per view (common.cuh).
+int check_det_size(int32_t H, int32_t W) {
+    if ((long long)gsr_grid(H, W).ntiles > GSR_DET_MAX_VIEW_TILES)
+        return fail(B200GSR_ERR_UNSUPPORTED, "deterministic mode supports at most %d 16x16 tiles per view (8192x8192); "
+                    "the image is %dx%d", GSR_DET_MAX_VIEW_TILES, W, H);
+    return B200GSR_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -132,6 +154,8 @@ int b200gsr_saved_layout_query(int32_t P, int32_t H, int32_t W, uint64_t max_pai
                                int32_t with_backward, b200gsr_saved_layout* out) {
     if (!out || P < 0 || H < 0 || W < 0) return fail(B200GSR_ERR_BAD_ARG, "bad layout query");
     if (max_pairs > 0xfffffff0ull) return fail(B200GSR_ERR_UNSUPPORTED, "max_pairs must fit in 32 bits");
+    const bool det = (with_backward & B200GSR_SAVED_DETERMINISTIC) != 0;
+    with_backward &= ~B200GSR_SAVED_DETERMINISTIC;
     const GsrTileGrid g = gsr_grid(H, W);
     size_t off = 0;
     out->header = off;      off = align_up(off + GSR_H_WORDS * sizeof(uint32_t));
@@ -142,7 +166,7 @@ int b200gsr_saved_layout_query(int32_t P, int32_t H, int32_t W, uint64_t max_pai
     out->geom = off;        off = align_up(off + (size_t)P * sizeof(GsrRec));
     out->dgeom = off;       off = align_up(off + (with_backward ? (size_t)P * 12 * sizeof(float) : 0));
     out->bwd_items = off;   off = align_up(off + (with_backward ? (size_t)GSR_BWD_CLASSES * g.ntiles * 8 * sizeof(uint32_t) : 0));
-    out->total = off;
+    out->total = det ? det_layout(P, off, with_backward != 0).total : off;
     return B200GSR_OK;
 }
 
@@ -181,11 +205,15 @@ int b200gsr_forward(const b200gsr_params* prm, const float* means3D, const float
     GsrFwdArgs a;
     a.prm = *prm;
     const int with_bwd = (flags & B200GSR_FWD_NO_BACKWARD) ? 0 : 1;
+    a.det = (flags & B200GSR_FWD_DETERMINISTIC) != 0;
+    if (a.det && (rc = check_det_size(prm->image_height, prm->image_width))) return rc;
     if ((rc = b200gsr_scratch_layout_query(prm->P, prm->image_height, prm->image_width, max_pairs, &a.sl))) return rc;
     if ((rc = b200gsr_saved_layout_query(prm->P, prm->image_height, prm->image_width, max_pairs, with_bwd, &a.vl))) return rc;
-    if (scratch_bytes < a.sl.total || saved_bytes < a.vl.total)
+    a.dl = det_layout(prm->P, a.vl.total, with_bwd != 0);
+    const size_t saved_need = a.det ? a.dl.total : a.vl.total;
+    if (scratch_bytes < a.sl.total || saved_bytes < saved_need)
         return fail(B200GSR_ERR_WORKSPACE, "workspace too small: scratch %zu < %zu or saved %zu < %zu",
-                    scratch_bytes, a.sl.total, saved_bytes, a.vl.total);
+                    scratch_bytes, a.sl.total, saved_bytes, saved_need);
     a.means3D = means3D; a.shs = shs; a.colors = colors_precomp; a.opac = opacities;
     a.scales = scales; a.rots = rotations; a.cov3d = cov3D_precomp;
     a.out_color = out_color; a.out_depth_alpha = out_depth_alpha; a.score = score; a.radii = radii;
@@ -267,10 +295,14 @@ int b200gsr_backward_ex(const b200gsr_params* prm, const float* means3D, const f
     GsrBwdArgs a;
     a.prm = *prm;
     a.sl = b200gsr_scratch_layout{};
+    a.det = (stages & B200GSR_BWD_DETERMINISTIC) != 0;
+    if (a.det && (rc = check_det_size(prm->image_height, prm->image_width))) return rc;
     if ((rc = b200gsr_saved_layout_query(prm->P, prm->image_height, prm->image_width, max_pairs, 1, &a.vl))) return rc;
-    if (saved_bytes < a.vl.total)
+    a.dl = det_layout(prm->P, a.vl.total, true);
+    if (saved_bytes < (a.det ? a.dl.total : a.vl.total))
         return fail(B200GSR_ERR_WORKSPACE, "saved buffer too small for backward: %zu < %zu (was the forward "
-                    "run with B200GSR_FWD_NO_BACKWARD?)", saved_bytes, a.vl.total);
+                    "run with B200GSR_FWD_NO_BACKWARD, or without B200GSR_FWD_DETERMINISTIC?)", saved_bytes,
+                    a.det ? a.dl.total : a.vl.total);
     a.means3D = means3D; a.shs = shs; a.colors = colors_precomp; a.opac = opacities;
     a.scales = scales; a.rots = rotations; a.cov3d = cov3D_precomp;
     a.radii = radii; a.out_depth_alpha = out_depth_alpha;
@@ -370,11 +402,15 @@ int b200gsr_forward_views(int32_t B, const b200gsr_params* prm, const b200gsr_vi
     const int Hs = B * g1.gy * GSR_TILE;
     GsrFwdArgs a;
     const int with_bwd = (flags & B200GSR_FWD_NO_BACKWARD) ? 0 : 1;
+    a.det = (flags & B200GSR_FWD_DETERMINISTIC) != 0;
+    if (a.det && (rc = check_det_size(H, W))) return rc;
     if ((rc = b200gsr_scratch_layout_query(B * P, Hs, W, max_pairs, &a.sl))) return rc;
     if ((rc = b200gsr_saved_layout_query(B * P, Hs, W, max_pairs, with_bwd, &a.vl))) return rc;
-    if (scratch_bytes < a.sl.total || saved_bytes < a.vl.total)
+    a.dl = det_layout(B * P, a.vl.total, with_bwd != 0);
+    const size_t saved_need = a.det ? a.dl.total : a.vl.total;
+    if (scratch_bytes < a.sl.total || saved_bytes < saved_need)
         return fail(B200GSR_ERR_WORKSPACE, "workspace too small: scratch %zu < %zu or saved %zu < %zu",
-                    scratch_bytes, a.sl.total, saved_bytes, a.vl.total);
+                    scratch_bytes, a.sl.total, saved_bytes, saved_need);
     a.out_color = out_color; a.out_depth_alpha = out_depth_alpha; a.score = score; a.radii = radii;
     a.scratch = static_cast<uint8_t*>(scratch); a.saved = static_cast<uint8_t*>(saved);
     a.max_pairs = (uint32_t)max_pairs;
@@ -407,10 +443,10 @@ int b200gsr_forward_views(int32_t B, const b200gsr_params* prm, const b200gsr_vi
     return rc;
 }
 
-int b200gsr_backward_views(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, const int32_t* radii,
-                           const float* out_depth_alpha, const float* dL_dcolor, const float* dL_ddepth_alpha,
-                           void* saved, size_t saved_bytes, uint64_t max_pairs, const b200gsr_view_grads* out,
-                           void* stream) {
+int b200gsr_backward_views_ex(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, const int32_t* radii,
+                              const float* out_depth_alpha, const float* dL_dcolor, const float* dL_ddepth_alpha,
+                              void* saved, size_t saved_bytes, uint64_t max_pairs, const b200gsr_view_grads* out,
+                              uint32_t flags, void* stream) {
     int rc = check_views(B, prm, in);
     if (rc) return rc;
     const int P = prm[0].P, H = prm[0].image_height, W = prm[0].image_width;
@@ -423,8 +459,12 @@ int b200gsr_backward_views(int32_t B, const b200gsr_params* prm, const b200gsr_v
     const int Hs = B * g1.gy * GSR_TILE;
     GsrBwdArgs a;
     a.sl = b200gsr_scratch_layout{};
+    a.det = (flags & B200GSR_BWD_DETERMINISTIC) != 0;
+    if (a.det && (rc = check_det_size(H, W))) return rc;
     if ((rc = b200gsr_saved_layout_query(B * P, Hs, W, max_pairs, 1, &a.vl))) return rc;
-    if (saved_bytes < a.vl.total) return fail(B200GSR_ERR_WORKSPACE, "saved buffer too small for backward: %zu < %zu", saved_bytes, a.vl.total);
+    a.dl = det_layout(B * P, a.vl.total, true);
+    const size_t saved_need = a.det ? a.dl.total : a.vl.total;
+    if (saved_bytes < saved_need) return fail(B200GSR_ERR_WORKSPACE, "saved buffer too small for backward: %zu < %zu", saved_bytes, saved_need);
     a.radii = radii; a.out_depth_alpha = out_depth_alpha; a.dL_dcolor = dL_dcolor; a.dL_ddepth_alpha = dL_ddepth_alpha;
     a.saved = static_cast<uint8_t*>(saved); a.scratch = nullptr; a.max_pairs = (uint32_t)max_pairs;
     a.num_sms = ds->num_sms; a.stats = g_stats;
@@ -454,6 +494,14 @@ int b200gsr_backward_views(int32_t B, const b200gsr_params* prm, const b200gsr_v
     }
     GSR_RANGE_POP();
     return rc;
+}
+
+int b200gsr_backward_views(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, const int32_t* radii,
+                           const float* out_depth_alpha, const float* dL_dcolor, const float* dL_ddepth_alpha,
+                           void* saved, size_t saved_bytes, uint64_t max_pairs, const b200gsr_view_grads* out,
+                           void* stream) {
+    return b200gsr_backward_views_ex(B, prm, in, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes,
+                                     max_pairs, out, 0u, stream);
 }
 
 int b200gsr_profile_enable(int32_t max_calls) {
@@ -559,14 +607,20 @@ int b200gsr_disparity_forward(int32_t B, int32_t N, const float* depth_alpha, co
                                                static_cast<cudaStream_t>(stream)), "disparity_forward");
 }
 
-int b200gsr_disparity_backward(int32_t B, int32_t N, const float* depth_alpha, const float* focal, const float* g_disp,
-                               const float* g_alpha, void* stats, float* d_depth_alpha, void* stream) {
+int b200gsr_disparity_backward_ex(int32_t B, int32_t N, const float* depth_alpha, const float* focal, const float* g_disp,
+                                  const float* g_alpha, void* stats, float* d_depth_alpha, uint32_t flags, void* stream) {
     if (B < 0 || N < 0 || ((B > 0 && N > 0) && (!depth_alpha || !focal || !g_disp || !stats || !d_depth_alpha)))
         return fail(B200GSR_ERR_BAD_ARG, "bad disparity_backward arguments");
     DeviceState* ds = device_state();
     if (!ds) return fail(B200GSR_ERR_CUDA, "cannot query the current CUDA device");
     return check_cuda(gsr_launch_disparity_bwd(B, N, depth_alpha, focal, g_disp, g_alpha, stats, d_depth_alpha,
-                                               ds->num_sms, static_cast<cudaStream_t>(stream)), "disparity_backward");
+                                               (flags & B200GSR_BWD_DETERMINISTIC) != 0, ds->num_sms,
+                                               static_cast<cudaStream_t>(stream)), "disparity_backward");
+}
+
+int b200gsr_disparity_backward(int32_t B, int32_t N, const float* depth_alpha, const float* focal, const float* g_disp,
+                               const float* g_alpha, void* stats, float* d_depth_alpha, void* stream) {
+    return b200gsr_disparity_backward_ex(B, N, depth_alpha, focal, g_disp, g_alpha, stats, d_depth_alpha, 0u, stream);
 }
 
 #define GSR_ST(x) static_cast<cudaStream_t>(x)

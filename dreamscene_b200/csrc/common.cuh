@@ -52,6 +52,8 @@ enum { GSR_H_NUM_PAIRS = 0, GSR_H_MAX_PAIRS = 1, GSR_H_NUM_TILES = 2, GSR_H_OVER
        GSR_H_BWD_QUEUE = 8,       // [8, 8+GSR_NQUEUE): work-queue counters of composite_bwd; zeroed by the
                                   // forward's scan kernel and restored to zero by project_bwd, so a saved
                                   // buffer can be back-propagated any number of times without a memset
+       GSR_H_BWD_QUEUE_DET = 16,  // [16, 16+GSR_NQUEUE): the same for the second deterministic backward pass; zeroed
+                                  // by the deterministic forward, restored to zero by det_resolve_kernel
        GSR_H_BWD_FILL = 32,       // [32, 64): items per size class of the backward's work lists (written by the
                                   // forward's composite kernel, zeroed by its scan kernel)
        GSR_H_WORDS = 64 };
@@ -96,6 +98,64 @@ __host__ __device__ inline int gsr_ms_blocks(long long P) {
 }
 #define GSR_MS_MAX_TILES 12288   // 4 B x tiles of dynamic smem (48 KB); 12 tiles per thread in the scan kernel
 __host__ __device__ inline bool gsr_use_multisplit(int ntiles) { return ntiles <= GSR_MS_MAX_TILES; }
+
+// ---- deterministic mode (B200GSR_FWD_DETERMINISTIC / B200GSR_BWD_DETERMINISTIC) ------------------------
+// Float atomics sum in whatever order the warps commit.  Deterministic mode commits integer images of the
+// partials instead: integer addition is associative, so the sum no longer depends on that order.
+//   gradients: per (Gaussian, component) the largest |partial| is found first (pass A, atomicMax of the float
+//              bits); pass B adds round(partial * 2^s) with s = GSR_DET_FIX_BITS - exponent(largest) into int64.
+//              A partial is then < 2^(K+1) in magnitude, and a Gaussian receives at most 8 commits per tile of
+//              its view, so with at most GSR_DET_MAX_VIEW_TILES tiles (8192^2 pixels) a sum stays below
+//              2^21 * 2^41 = 2^62: no overflow, with a factor 2 to spare.  Quantisation error <= 2^-(K+1) of the
+//              component's largest partial per commit.
+//   important score: every commit is a warp's summed blend weight; a Gaussian's score is at most its view's
+//              pixel count (2^26), so a fixed scale 2^GSR_DET_SCORE_BITS keeps the sum below 2^62.
+// The constants are fixed (never derived from the image or the view count): a sum depends only on the set
+// of partials, so one view of a multi-view render reproduces the single-view result bit for bit.
+#define GSR_DET_FIX_BITS 40
+#define GSR_DET_MAX_VIEW_TILES (1 << 18)
+#define GSR_DET_SCORE_BITS 36
+#define GSR_DET_COMPONENTS 10     // per-Gaussian gradient accumulators used of the 12 in a dgeom row
+
+// Offsets of the deterministic accumulators, appended to the saved buffer after bwd_items (0 = absent).
+struct GsrDetLayout {
+    size_t dmax;       // uint32[P][10]: float bits of the largest |partial| per (Gaussian, component)
+    size_t dfx;        // int64[P][10]: fixed-point sums
+    size_t score_fx;   // int64[P]: fixed-point important score
+    size_t total;
+};
+
+__host__ __device__ inline double gsr_pow2(int s) {   // exact 2^s for -1022 <= s <= 1023
+    const unsigned long long b = (unsigned long long)(s + 1023) << 52;
+#ifdef __CUDA_ARCH__
+    return __longlong_as_double((long long)b);
+#else
+    double d;
+    __builtin_memcpy(&d, &b, sizeof(d));
+    return d;
+#endif
+}
+// Scale exponent s for a component whose largest |partial| has the float bits `max_bits` (finite, sign clear).
+__host__ __device__ inline int gsr_det_shift(uint32_t max_bits) {
+    int e = (int)(max_bits >> 23);   // biased exponent
+    if (e == 0) e = 1;               // zero or subnormal: bounded by the smallest normal binade
+    return GSR_DET_FIX_BITS - (e - 127);
+}
+__host__ __device__ inline bool gsr_det_finite(uint32_t max_bits) { return max_bits < 0x7f800000u; }
+__host__ __device__ inline long long gsr_det_quantise(float x, int shift) {
+    return llrint((double)x * gsr_pow2(shift));
+}
+// The summed component; NaN when any partial was NaN or infinite (the float atomics give a non-finite sum too).
+__host__ __device__ inline float gsr_det_dequantise(long long sum, uint32_t max_bits) {
+    if (!gsr_det_finite(max_bits)) return nanf("");
+    return (float)((double)sum * gsr_pow2(-gsr_det_shift(max_bits)));
+}
+__host__ __device__ inline long long gsr_det_score_quantise(float w) {
+    return llrint((double)w * gsr_pow2(GSR_DET_SCORE_BITS));
+}
+__host__ __device__ inline float gsr_det_score_dequantise(long long sum) {
+    return (float)((double)sum * gsr_pow2(-GSR_DET_SCORE_BITS));
+}
 
 #ifdef __CUDACC__
 // ---- 128-bit global access helpers -------------------------------------------------------
@@ -165,6 +225,8 @@ struct GsrFwdArgs {
     uint32_t* host_notify;
     uint32_t notify_seq;
     uint32_t flags;        // B200GSR_FWD_*
+    bool det;              // B200GSR_FWD_DETERMINISTIC: `dl` locates the fixed-point accumulators in `saved`
+    GsrDetLayout dl;
     // multi-view (b200gsr_forward_views): the views are stacked vertically into one image of
     // num_views * gy_view tile rows; view v's Gaussians are the virtual Gaussians [v*P_view, (v+1)*P_view).
     // Single-view calls: view = 0, num_views = 1, P_view = prm.P, gy_view = tile rows of the image.
@@ -189,6 +251,8 @@ struct GsrBwdArgs {
     int accumulate;        // project_bwd adds into the gradient outputs instead of overwriting (views sharing a parameter)
     int g_begin, g_end;    // Gaussian range of the project_bwd stage (chunked launches)
     int dsh_coefs;         // coefficients per row of d_shs (0 = M, the reference layout)
+    bool det;              // B200GSR_BWD_DETERMINISTIC: fixed-point accumulation, see GsrDetLayout
+    GsrDetLayout dl;
     int num_sms;
     unsigned long long* stats;   // optional device counters (b200gsr_debug_counters); selects the STATS kernels
     cudaStream_t stream;
@@ -231,7 +295,8 @@ cudaError_t gsr_launch_assemble(bool backward, int num_groups, const b200gsr_gro
 cudaError_t gsr_launch_disparity_fwd(int B, int N, const float* da, const float* focal, float* out, void* stats,
                                      int num_sms, cudaStream_t s);
 cudaError_t gsr_launch_disparity_bwd(int B, int N, const float* da, const float* focal, const float* g_out,
-                                     const float* g_alpha, void* stats, float* d_da, int num_sms, cudaStream_t s);
+                                     const float* g_alpha, void* stats, float* d_da, bool deterministic, int num_sms,
+                                     cudaStream_t s);
 
 // densification / pruning (densify.cu)
 cudaError_t gsr_densify_stats(int P, const float* vs_grad, const int32_t* radii, float* accum, float* denom,

@@ -159,7 +159,9 @@ struct __align__(128) SmemCta {
 
 // PARTS = 1: one CTA of 8 warps per tile.  PARTS = 2 (A/B variant): a tile is rendered by two CTAs of 4 warps,
 // each taking an 16x8 half (both gather the whole list; fewer warps per barrier, twice as many barrier groups).
-template <bool SCORE, int PPL, bool STATS, int PARTS = 1, int ILP = 1>
+// DET (deterministic mode, with SCORE): `score` points to the int64 fixed-point accumulators (GsrDetLayout::score_fx)
+// and each warp's weight sum is committed as an integer (gsr_det_score_quantise).
+template <bool SCORE, int PPL, bool STATS, int PARTS = 1, int ILP = 1, bool DET = false>
 __global__ void __launch_bounds__(256 / PPL / PARTS)
 composite_fwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, const uint32_t* __restrict__ header,
                      const uint32_t* __restrict__ work_order,
@@ -290,7 +292,13 @@ composite_fwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, cons
                     if (SCORE) {
 #pragma unroll
                         for (int o = 16; o > 0; o >>= 1) wsum += __shfl_xor_sync(0xffffffffu, wsum, o);
-                        if (lane == 0 && wsum != 0.f) atomicAdd(score + __float_as_uint(q2.w), wsum);
+                        if (lane == 0 && wsum != 0.f) {
+                            if (DET)
+                                atomicAdd(reinterpret_cast<unsigned long long*>(score) + __float_as_uint(q2.w),
+                                          (unsigned long long)gsr_det_score_quantise(wsum));
+                            else
+                                atomicAdd(score + __float_as_uint(q2.w), wsum);
+                        }
                     }
                 };
                 while (mask) {
@@ -739,6 +747,23 @@ composite_bwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, cons
 }
 
 
+// How composite_bwd2_kernel commits a (warp item, Gaussian) partial of component c.
+enum { GSR_ACC_FLOAT = 0,      // fp32 atomicAdd into dgeom (default)
+       GSR_ACC_DET_MAX = 1,    // deterministic pass A: atomicMax of |partial|'s bits into dmax
+       GSR_ACC_DET_SUM = 2 };  // deterministic pass B: int64 atomicAdd of the fixed-point partial into dfx
+// mb (pass B): dmax of the component, loaded by the caller ahead of the arithmetic that produces v.
+template <int ACC>
+__device__ __forceinline__ void commit_partial(uint32_t* dmax, unsigned long long* dfx, uint32_t g, int c, float v,
+                                               uint32_t mb) {
+    if (ACC == GSR_ACC_DET_MAX) {
+        atomicMax(dmax + GSR_DET_COMPONENTS * (size_t)g + c, __float_as_uint(fabsf(v)));
+    } else if (ACC == GSR_ACC_DET_SUM) {
+        // a non-finite component skips the sums: the result is NaN whatever they hold (gsr_det_dequantise)
+        if (gsr_det_finite(mb))
+            atomicAdd(dfx + GSR_DET_COMPONENTS * (size_t)g + c, (unsigned long long)gsr_det_quantise(v, gsr_det_shift(mb)));
+    }
+}
+
 // ---------------------------------------------------------------------------------------------
 // Backward, round-2 variant ("v2"): same work decomposition and ring as composite_bwd_kernel, with an
 // instruction diet on the per-(warp, Gaussian) body (VERDICT r1 item 2):
@@ -781,7 +806,9 @@ __device__ __forceinline__ void halve2(float (&v)[10], bool hi) {
 }
 
 
-template <int kSlots, int kMinCtas, int KFAST, bool STATS, bool DUAL = false>
+// ACC: how the butterfly's per-(warp item, Gaussian) totals are committed (GSR_ACC_*).  The deterministic passes
+// run with KFAST = 0 and DUAL = false: every commit is a butterfly total, a function of its work item alone.
+template <int kSlots, int kMinCtas, int KFAST, bool STATS, bool DUAL = false, int ACC = GSR_ACC_FLOAT>
 __global__ void __launch_bounds__(kWarps * 32, kMinCtas)
 composite_bwd2_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, const uint32_t* __restrict__ header,
                       const uint32_t* __restrict__ work_order,
@@ -791,7 +818,9 @@ composite_bwd2_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, con
                       const float* __restrict__ out_depth_alpha,
                       const uint32_t* __restrict__ n_contrib, const float* __restrict__ dL_dcolor,
                       const float* __restrict__ dL_ddepth_alpha, float* __restrict__ dgeom,
-                      unsigned long long* __restrict__ stats, const uint32_t* __restrict__ bwd_items) {
+                      unsigned long long* __restrict__ stats, const uint32_t* __restrict__ bwd_items,
+                      uint32_t* __restrict__ dmax, unsigned long long* __restrict__ dfx) {
+    static_assert(ACC == GSR_ACC_FLOAT || (KFAST == 0 && !DUAL), "deterministic passes commit butterfly totals only");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     SmemRing<kSlots>& sm = *reinterpret_cast<SmemRing<kSlots>*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -1039,6 +1068,9 @@ composite_bwd2_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, con
                 if (STATS) ++st_eval;
                 if (cm == 0u) continue;
                 const float4 q2 = rp[2];
+                uint32_t det_mb = 0u;   // pass B: issued here so that its latency hides behind the body and butterfly
+                if (ACC == GSR_ACC_DET_SUM && commit_lane)
+                    det_mb = __ldg(dmax + GSR_DET_COMPONENTS * (size_t)__float_as_uint(q2.w) + vidx);
                 // ---- branch-free body: non-contributing lanes carry alpha = G = 0 ----
                 const float am = contrib ? alpha : 0.0f;
                 const float Gm = contrib ? G : 0.0f;
@@ -1088,7 +1120,11 @@ composite_bwd2_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, con
                 halve2<3, 4>(vv, lane & 4);
                 halve2<2, 2>(vv, lane & 2);
                 const float tot = vv[0] + __shfl_xor_sync(0xffffffffu, vv[0], 1);
-                if (commit_lane) atomicAdd(row + vidx, tot);
+                if (ACC == GSR_ACC_FLOAT) {
+                    if (commit_lane) atomicAdd(row + vidx, tot);
+                } else if (commit_lane) {
+                    commit_partial<ACC>(dmax, dfx, __float_as_uint(q2.w), vidx, tot, det_mb);
+                }
             }
             __syncwarp();
         }
@@ -1109,6 +1145,33 @@ composite_bwd2_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, con
         atomicMax(stats + GSR_STAT_BWD_MAX_ITEM, st_max_item);
         atomicMax(stats + GSR_STAT_BWD_MAX_ITEM_NS, st_max_item_ns);
     }
+}
+
+// Deterministic mode, after pass B: the fixed-point sums of every visible Gaussian become the float dgeom row
+// project_bwd reads, and both integer arrays are cleared for the next backward over this `saved` (read-and-clear,
+// like dgeom itself).  Rows of culled Gaussians were never touched by the composite.
+__global__ void __launch_bounds__(256)
+det_resolve_kernel(int n, const int32_t* __restrict__ radii, uint32_t* __restrict__ dmax,
+                   unsigned long long* __restrict__ dfx, float* __restrict__ dgeom, uint32_t* __restrict__ queue_b) {
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i < GSR_NQUEUE) queue_b[i] = 0u;   // pass B (the previous kernel) has drained its work queue
+    if (i >= n || __ldg(radii + i) <= 0) return;
+    uint32_t* mx = dmax + GSR_DET_COMPONENTS * (size_t)i;
+    unsigned long long* fx = dfx + GSR_DET_COMPONENTS * (size_t)i;
+    float* row = dgeom + 12 * (size_t)i;
+#pragma unroll
+    for (int c = 0; c < GSR_DET_COMPONENTS; ++c) {
+        row[c] = gsr_det_dequantise((long long)fx[c], mx[c]);
+        mx[c] = 0u;
+        fx[c] = 0ull;
+    }
+}
+
+// Deterministic mode, after composite_fwd: fixed-point important score -> float score (every row)
+__global__ void __launch_bounds__(256)
+det_score_kernel(int n, const unsigned long long* __restrict__ score_fx, float* __restrict__ score) {
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i < n) score[i] = gsr_det_score_dequantise((long long)score_fx[i]);
 }
 
 }  // namespace
@@ -1141,15 +1204,15 @@ static CompPtrs comp_ptrs(const uint8_t* saved, const b200gsr_saved_layout& vl, 
     return c;
 }
 
-template <bool SCORE, bool STATS, int ILP = 1>
-static cudaError_t launch_fwd(const GsrFwdArgs& a, int nblocks, const CompPtrs& c, uint32_t* queue) {
+template <bool SCORE, bool STATS, int ILP = 1, bool DET = false>
+static cudaError_t launch_fwd(const GsrFwdArgs& a, int nblocks, const CompPtrs& c, uint32_t* queue, float* score) {
     const int smem = (int)sizeof(SmemCta);
     static std::atomic<unsigned long long> attr_done{0};
-    cudaError_t e = gsr_smem_once(composite_fwd_kernel<SCORE, 1, STATS, 1, ILP>, smem, attr_done);
+    cudaError_t e = gsr_smem_once(composite_fwd_kernel<SCORE, 1, STATS, 1, ILP, DET>, smem, attr_done);
     if (e != cudaSuccess) return e;
-    composite_fwd_kernel<SCORE, 1, STATS, 1, ILP><<<nblocks, 256, smem, a.stream>>>(
+    composite_fwd_kernel<SCORE, 1, STATS, 1, ILP, DET><<<nblocks, 256, smem, a.stream>>>(
         a.prm.image_height, a.prm.image_width, c.grid.gx, a.gy_view, c.H, c.grid.ntiles, c.header, c.work_order, c.tile_start,
-        c.keys, c.geom, a.prm.bg, queue, a.out_color, a.out_depth_alpha, c.n_contrib, a.score, a.stats, c.bwd_fill, c.bwd_items);
+        c.keys, c.geom, a.prm.bg, queue, a.out_color, a.out_depth_alpha, c.n_contrib, score, a.stats, c.bwd_fill, c.bwd_items);
     return cudaGetLastError();
 }
 
@@ -1170,13 +1233,25 @@ cudaError_t gsr_launch_composite_fwd(const GsrFwdArgs& a) {
     if (c.grid.ntiles == 0) return cudaSuccess;
     uint32_t* queue = reinterpret_cast<uint32_t*>(a.scratch + a.sl.counters) + GSR_C_FWD_QUEUE;
     const int nblocks = min(c.grid.ntiles, a.num_sms * 6);
+    if (a.det && a.prm.score_flag) {
+        // deterministic important score: fixed-point commits, then one conversion pass over every row.  The
+        // forward kernel is otherwise the default one (its outputs do not depend on scheduling); the A/B
+        // switches and the instrumented instantiation do not apply.
+        unsigned long long* sfx = reinterpret_cast<unsigned long long*>(a.saved + a.dl.score_fx);
+        cudaError_t e = launch_fwd<true, false, GSR_FWD_ILP, true>(a, nblocks, c, queue, reinterpret_cast<float*>(sfx));
+        if (e != cudaSuccess) return e;
+        const int n = a.num_views * a.P_view;
+        if (n > 0) det_score_kernel<<<(n + 255) / 256, 256, 0, a.stream>>>(n, sfx, a.score);
+        return cudaGetLastError();
+    }
+    if (a.det) return launch_fwd<false, false, GSR_FWD_ILP>(a, nblocks, c, queue, a.score);
     // B200GSR_FWD_VARIANT = 1 | 2: bulk-copy / TMA staging experiments (A/B runs only)
     static const int fwd_variant = [] { const char* e = getenv("B200GSR_FWD_VARIANT"); return e ? atoi(e) : 0; }();
     if (fwd_variant >= 51 && fwd_variant <= 54 && !a.prm.score_flag && a.stats == nullptr) {   // 1/2/3/4 list entries in flight
-        return fwd_variant == 51 ? launch_fwd<false, false, 1>(a, nblocks, c, queue)
-             : fwd_variant == 52 ? launch_fwd<false, false, 2>(a, nblocks, c, queue)
-             : fwd_variant == 53 ? launch_fwd<false, false, 3>(a, nblocks, c, queue)
-                                 : launch_fwd<false, false, 4>(a, nblocks, c, queue);
+        return fwd_variant == 51 ? launch_fwd<false, false, 1>(a, nblocks, c, queue, a.score)
+             : fwd_variant == 52 ? launch_fwd<false, false, 2>(a, nblocks, c, queue, a.score)
+             : fwd_variant == 53 ? launch_fwd<false, false, 3>(a, nblocks, c, queue, a.score)
+                                 : launch_fwd<false, false, 4>(a, nblocks, c, queue, a.score);
     }
     if ((fwd_variant == 42 || fwd_variant == 44) && !a.prm.score_flag && a.stats == nullptr) {
         // a tile rendered by 2 (4) CTAs of 4 (2) warps, two entries in flight: finer work items for the balance
@@ -1213,10 +1288,10 @@ cudaError_t gsr_launch_composite_fwd(const GsrFwdArgs& a) {
         return fwd_variant == 2 ? launch_fwd_tma<2>(a, nb, c, queue) : launch_fwd_tma<1>(a, nb, c, queue);
     }
     if (a.stats != nullptr)
-        return a.prm.score_flag ? launch_fwd<true, true, GSR_FWD_ILP>(a, nblocks, c, queue)
-                                : launch_fwd<false, true, GSR_FWD_ILP>(a, nblocks, c, queue);
-    return a.prm.score_flag ? launch_fwd<true, false, GSR_FWD_ILP>(a, nblocks, c, queue)
-                            : launch_fwd<false, false, GSR_FWD_ILP>(a, nblocks, c, queue);
+        return a.prm.score_flag ? launch_fwd<true, true, GSR_FWD_ILP>(a, nblocks, c, queue, a.score)
+                                : launch_fwd<false, true, GSR_FWD_ILP>(a, nblocks, c, queue, a.score);
+    return a.prm.score_flag ? launch_fwd<true, false, GSR_FWD_ILP>(a, nblocks, c, queue, a.score)
+                            : launch_fwd<false, false, GSR_FWD_ILP>(a, nblocks, c, queue, a.score);
 }
 
 template <int kSlots, int kMinCtas>
@@ -1232,17 +1307,18 @@ static cudaError_t launch_bwd(const GsrBwdArgs& a, const CompPtrs& c, uint32_t* 
     return cudaGetLastError();
 }
 
-template <int kSlots, int kMinCtas, int KFAST, bool STATS, bool DUAL = false>
-static cudaError_t launch_bwd2(const GsrBwdArgs& a, const CompPtrs& c, uint32_t* queue, float* dgeom) {
+template <int kSlots, int kMinCtas, int KFAST, bool STATS, bool DUAL = false, int ACC = GSR_ACC_FLOAT>
+static cudaError_t launch_bwd2(const GsrBwdArgs& a, const CompPtrs& c, uint32_t* queue, float* dgeom,
+                               uint32_t* dmax = nullptr, unsigned long long* dfx = nullptr) {
     const int smem = (int)sizeof(SmemRing<kSlots>);
     const int nblocks = min(c.grid.ntiles, a.num_sms * kMinCtas);
     static std::atomic<unsigned long long> attr_done{0};
-    cudaError_t e = gsr_smem_once(composite_bwd2_kernel<kSlots, kMinCtas, KFAST, STATS, DUAL>, smem, attr_done);
+    cudaError_t e = gsr_smem_once(composite_bwd2_kernel<kSlots, kMinCtas, KFAST, STATS, DUAL, ACC>, smem, attr_done);
     if (e != cudaSuccess) return e;
-    composite_bwd2_kernel<kSlots, kMinCtas, KFAST, STATS, DUAL><<<nblocks, kWarps * 32, smem, a.stream>>>(
+    composite_bwd2_kernel<kSlots, kMinCtas, KFAST, STATS, DUAL, ACC><<<nblocks, kWarps * 32, smem, a.stream>>>(
         a.prm.image_height, a.prm.image_width, c.grid.gx, a.gy_view, c.H, c.grid.ntiles, c.header, c.work_order, c.tile_start,
         c.keys, c.geom, a.prm.bg, queue, a.out_depth_alpha, c.n_contrib, a.dL_dcolor, a.dL_ddepth_alpha, dgeom,
-        a.stats, c.bwd_items);
+        a.stats, c.bwd_items, dmax, dfx);
     return cudaGetLastError();
 }
 
@@ -1251,6 +1327,19 @@ cudaError_t gsr_launch_composite_bwd(const GsrBwdArgs& a) {
     if (c.grid.ntiles == 0) return cudaSuccess;
     uint32_t* queue = reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE;
     float* dgeom = reinterpret_cast<float*>(a.saved + a.vl.dgeom);
+    if (a.det) {
+        // Deterministic mode: one fixed instantiation, run twice (A/B switches and instrumentation do not apply).
+        // Pass B pops its own work queue (header words, zero between calls like the first one): no memset.
+        uint32_t* dmax = reinterpret_cast<uint32_t*>(a.saved + a.dl.dmax);
+        unsigned long long* dfx = reinterpret_cast<unsigned long long*>(a.saved + a.dl.dfx);
+        uint32_t* queue_b = reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE_DET;
+        cudaError_t e = launch_bwd2<3, 4, 0, false, false, GSR_ACC_DET_MAX>(a, c, queue, dgeom, dmax, dfx);
+        if (e == cudaSuccess) e = launch_bwd2<3, 4, 0, false, false, GSR_ACC_DET_SUM>(a, c, queue_b, dgeom, dmax, dfx);
+        if (e != cudaSuccess) return e;
+        const int n = a.num_views * a.P_view;
+        det_resolve_kernel<<<(n + 255) / 256, 256, 0, a.stream>>>(n, a.radii, dmax, dfx, dgeom, queue_b);
+        return cudaGetLastError();
+    }
     if (a.stats != nullptr) return launch_bwd2<3, 4, GSR_BWD_KFAST, true>(a, c, queue, dgeom);
     // B200GSR_BWD_VARIANT selects kernels for A/B runs: 0 = round-1 kernel,
     // 10/11/12/14 = v2 with the direct-commit fast path for <= 0/1/2/4 contributing lanes;

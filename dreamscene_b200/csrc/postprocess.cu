@@ -83,10 +83,13 @@ disp_normalise_kernel(const float* __restrict__ da, const float* __restrict__ fo
     }
 }
 
-// backward pass 1: the two global sums feeding the min / max paths, and the tie counts
+// backward pass 1: the two global sums feeding the min / max paths, and the tie counts.
+// DET (deterministic mode): instead of float atomics, each block writes its two sums - its warps' sums added in
+// warp order - to part[2 * (v * gridDim.x + blockIdx.x)], and disp_bwd_sum_kernel adds them up in block order.
+template <bool DET>
 __global__ void __launch_bounds__(256)
 disp_bwd_reduce_kernel(const float* __restrict__ da, const float* __restrict__ focal, int N,
-                       const float* __restrict__ g_out, DispStats* st) {
+                       const float* __restrict__ g_out, DispStats* st, float* __restrict__ part) {
     const int v = blockIdx.y;
     const float* depth = da + (size_t)v * 2 * N;
     const float* alpha = depth + N;
@@ -114,10 +117,36 @@ disp_bwd_reduce_kernel(const float* __restrict__ da, const float* __restrict__ f
     }
     tm = __reduce_add_sync(0xffffffffu, tm); tM = __reduce_add_sync(0xffffffffu, tM);
     if ((threadIdx.x & 31) == 0) {
-        atomicAdd(&st[v].sum_min, sm); atomicAdd(&st[v].sum_max, sM);
-        if (tm) atomicAdd(&st[v].ties_min, tm);
+        if (!DET) { atomicAdd(&st[v].sum_min, sm); atomicAdd(&st[v].sum_max, sM); }
+        if (tm) atomicAdd(&st[v].ties_min, tm);       // integer counts: exact in any order
         if (tM) atomicAdd(&st[v].ties_max, tM);
     }
+    if (DET) {
+        __shared__ float ws[2][8];
+        if ((threadIdx.x & 31) == 0) { ws[0][threadIdx.x >> 5] = sm; ws[1][threadIdx.x >> 5] = sM; }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            float bm = 0.f, bM = 0.f;
+            for (int w = 0; w < 8; ++w) { bm += ws[0][w]; bM += ws[1][w]; }
+            float* o = part + 2 * ((size_t)v * gridDim.x + blockIdx.x);
+            o[0] = bm; o[1] = bM;
+        }
+    }
+}
+
+// deterministic backward, between the two passes: one warp per view adds the block sums in a fixed order
+__global__ void __launch_bounds__(32)
+disp_bwd_sum_kernel(int nblk, const float* __restrict__ part, DispStats* st) {
+    const int v = blockIdx.x, lane = threadIdx.x;
+    const float* p = part + 2 * (size_t)v * nblk;
+    float sm = 0.f, sM = 0.f;
+    for (int b = lane; b < nblk; b += 32) { sm += p[2 * b]; sM += p[2 * b + 1]; }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        sm += __shfl_xor_sync(0xffffffffu, sm, o);
+        sM += __shfl_xor_sync(0xffffffffu, sM, o);
+    }
+    if (lane == 0) { st[v].sum_min += sm; st[v].sum_max += sM; }
 }
 
 // backward pass 2: d depth_alpha = chain through d = focal / x, x = depth + 10 alpha + 1e-5 (+ the caller's own
@@ -163,11 +192,18 @@ cudaError_t gsr_launch_disparity_fwd(int B, int N, const float* da, const float*
 }
 
 cudaError_t gsr_launch_disparity_bwd(int B, int N, const float* da, const float* focal, const float* g_out,
-                                     const float* g_alpha, void* stats, float* d_da, int num_sms, cudaStream_t s) {
+                                     const float* g_alpha, void* stats, float* d_da, bool deterministic, int num_sms,
+                                     cudaStream_t s) {
     if (B <= 0 || N <= 0) return cudaSuccess;
     DispStats* st = static_cast<DispStats*>(stats);
     const int bx = max(1, min((N + 255) / 256, (num_sms * 8 + B - 1) / B));
-    disp_bwd_reduce_kernel<<<dim3(bx, B), 256, 0, s>>>(da, focal, N, g_out, st);
+    if (deterministic) {
+        // the block sums (2 * bx <= 2N floats per view) live in d_da until disp_bwd_apply_kernel overwrites it
+        disp_bwd_reduce_kernel<true><<<dim3(bx, B), 256, 0, s>>>(da, focal, N, g_out, st, d_da);
+        disp_bwd_sum_kernel<<<B, 32, 0, s>>>(bx, d_da, st);
+    } else {
+        disp_bwd_reduce_kernel<false><<<dim3(bx, B), 256, 0, s>>>(da, focal, N, g_out, st, nullptr);
+    }
     disp_bwd_apply_kernel<<<dim3(bx, B), 256, 0, s>>>(da, focal, N, g_out, g_alpha, st, d_da);
     return cudaGetLastError();
 }

@@ -281,7 +281,9 @@ __device__ __forceinline__ void sh_color(const float (&B)[16], const float* row,
 // =========================================================================================
 // Forward: one Gaussian per thread, kBlock Gaussians per CTA.
 // =========================================================================================
-template <int MT>
+// DET (deterministic mode): also zero this view's rows of the fixed-point accumulators (GsrDetLayout) - the score
+// (det_score_kernel converts every row) and the gradient sums and maxima - and the second backward pass's work queue.
+template <int MT, bool DET = false>
 __global__ void __launch_bounds__(kBlock)
 project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
                   const float* __restrict__ shs, const float* __restrict__ colors,
@@ -290,7 +292,9 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
                   int32_t* __restrict__ radii, uint4* __restrict__ rectdepth,
                   GsrRec* __restrict__ geom, uint32_t* __restrict__ tile_count,
                   uint32_t* __restrict__ zero_words, int num_zero_words, float* __restrict__ dgeom,
-                  int rec_base, int tile_row_off, int ntiles_total) {
+                  int rec_base, int tile_row_off, int ntiles_total,
+                  uint32_t* __restrict__ det_max, unsigned long long* __restrict__ det_fx,
+                  unsigned long long* __restrict__ score_fx, uint32_t* __restrict__ det_queue) {
     extern __shared__ __align__(16) float sh_buf[];
     __shared__ uint8_t vis_s[kBlock];
     const int g0 = blockIdx.x * kBlock;
@@ -347,6 +351,18 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
         }
         radii[rec_base + i] = radius;
         rectdepth[rec_base + i] = rd;
+        if (DET && score_fx != nullptr) score_fx[rec_base + i] = 0ull;
+    }
+    if (DET && det_queue != nullptr && i < GSR_NQUEUE) det_queue[i] = 0u;
+    if (DET && det_fx != nullptr) {
+        // the block's rows as two contiguous spans, coalesced (rows of culled Gaussians are zeroed too: never read)
+        const int rows = min(kBlock, p.P - g0);
+        ulonglong2* fx = reinterpret_cast<ulonglong2*>(det_fx + GSR_DET_COMPONENTS * (size_t)(rec_base + g0));   // 80-B rows
+        uint2* mx = reinterpret_cast<uint2*>(det_max + GSR_DET_COMPONENTS * (size_t)(rec_base + g0));           // 40-B rows
+        for (int k = threadIdx.x; k < rows * (GSR_DET_COMPONENTS / 2); k += kBlock) {
+            fx[k] = make_ulonglong2(0ull, 0ull);
+            mx[k] = make_uint2(0u, 0u);
+        }
     }
     const int stride = sh_row_stride(p.M);
     const int ncoef = (p.sh_degree + 1) * (p.sh_degree + 1);
@@ -758,7 +774,7 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D,
 
 }  // namespace
 
-template <int MT>
+template <int MT, bool DET>
 static void launch_project_sh(const GsrFwdArgs& a, int P, size_t smem) {
     // multisplit path: counters + the single per-tile counter array are zeroed in the prologue
     // (api.cu issues a memset instead on the large-grid fallback, where this kernel counts itself)
@@ -766,23 +782,34 @@ static void launch_project_sh(const GsrFwdArgs& a, int P, size_t smem) {
     tg.gy = a.num_views * a.gy_view; tg.ntiles = tg.gx * tg.gy;      // the stacked image
     const int nzero = gsr_use_multisplit(tg.ntiles)
         ? (int)((a.sl.tile_count + (size_t)tg.ntiles * sizeof(uint32_t)) / sizeof(uint32_t)) : 0;
-    project_sh_kernel<MT><<<(P + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
+    const bool bwd = !(a.flags & B200GSR_FWD_NO_BACKWARD);
+    project_sh_kernel<MT, DET><<<(P + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
         a.prm, a.means3D, a.shs, a.colors, a.opac, a.scales, a.rots, a.cov3d, a.radii,
         reinterpret_cast<uint4*>(a.scratch + a.sl.rectdepth),
         reinterpret_cast<GsrRec*>(a.saved + a.vl.geom),
         reinterpret_cast<uint32_t*>(a.scratch + a.sl.tile_count),
         reinterpret_cast<uint32_t*>(a.scratch), nzero,
-        (a.flags & B200GSR_FWD_NO_BACKWARD) ? nullptr : reinterpret_cast<float*>(a.saved + a.vl.dgeom),
-        a.view * a.P_view, a.view * a.gy_view, tg.ntiles);
+        bwd ? reinterpret_cast<float*>(a.saved + a.vl.dgeom) : nullptr,
+        a.view * a.P_view, a.view * a.gy_view, tg.ntiles,
+        DET && bwd ? reinterpret_cast<uint32_t*>(a.saved + a.dl.dmax) : nullptr,
+        DET && bwd ? reinterpret_cast<unsigned long long*>(a.saved + a.dl.dfx) : nullptr,
+        DET && a.prm.score_flag ? reinterpret_cast<unsigned long long*>(a.saved + a.dl.score_fx) : nullptr,
+        DET && bwd && a.view == 0 ? reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE_DET : nullptr);
 }
 
 cudaError_t gsr_launch_project(const GsrFwdArgs& a) {
     const int P = a.prm.P;
     if (P == 0) return cudaSuccess;
     const size_t smem = a.shs ? (size_t)kBlock * sh_row_stride(a.prm.M) * sizeof(float) : 0;
-    if (a.shs && a.prm.M == 16) launch_project_sh<16>(a, P, smem);
-    else if (a.shs && a.prm.M == 4) launch_project_sh<4>(a, P, smem);
-    else launch_project_sh<0>(a, P, smem);
+    if (a.det) {
+        if (a.shs && a.prm.M == 16) launch_project_sh<16, true>(a, P, smem);
+        else if (a.shs && a.prm.M == 4) launch_project_sh<4, true>(a, P, smem);
+        else launch_project_sh<0, true>(a, P, smem);
+    } else {
+        if (a.shs && a.prm.M == 16) launch_project_sh<16, false>(a, P, smem);
+        else if (a.shs && a.prm.M == 4) launch_project_sh<4, false>(a, P, smem);
+        else launch_project_sh<0, false>(a, P, smem);
+    }
     return cudaGetLastError();
 }
 

@@ -84,7 +84,8 @@ class _RasterizeViews(torch.autograd.Function):
             radii = torch.empty(B, P, dtype=torch.int32, device=dev)
             score = torch.zeros(B, P, dtype=torch.float32, device=dev) if score_flag else None
             stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            flags = 0 if with_backward else _lib.FWD_NO_BACKWARD
+            det = R.deterministic_mode()
+            flags = (0 if with_backward else _lib.FWD_NO_BACKWARD) | (_lib.FWD_DETERMINISTIC if det else 0)
 
             def launch(cap, scratch, saved, notify_ptr, seq):
                 return lib.b200gsr_forward_views(B, prm, vin, C.c_void_p(color.data_ptr()), C.c_void_p(depth_alpha.data_ptr()),
@@ -92,8 +93,8 @@ class _RasterizeViews(torch.autograd.Function):
                                                  C.c_void_p(scratch.data_ptr()), scratch.numel(), C.c_void_p(saved.data_ptr()),
                                                  saved.numel(), cap, flags, notify_ptr, seq, stream)
 
-            saved, cap = R._issue_with_capacity(d, dev, (B, P, H, W), B * P, Hs, W, with_backward, score, launch)
-        ctx.meta = (settings, spec, B, P, M, H, W, Hs, cap, with_backward, len(flat))
+            saved, cap = R._issue_with_capacity(d, dev, (B, P, H, W), B * P, Hs, W, with_backward, score, launch, det)
+        ctx.meta = (settings, spec, B, P, M, H, W, Hs, cap, with_backward, len(flat), det)
         ctx.keep = keep
         ctx.saved_buf = saved
         ctx.save_for_backward(radii, depth_alpha, *tensors)
@@ -106,7 +107,7 @@ class _RasterizeViews(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_color, _g_radii, g_da, *_):
-        settings, spec, B, P, M, H, W, Hs, cap, with_backward, nflat = ctx.meta
+        settings, spec, B, P, M, H, W, Hs, cap, with_backward, nflat, det = ctx.meta
         radii, depth_alpha = ctx.saved_tensors[:2]
         tensors = list(ctx.saved_tensors[2:])
         dev = radii.device
@@ -146,10 +147,11 @@ class _RasterizeViews(torch.autograd.Function):
                 grads[m2d_base + v] = g2
                 out[v].d_means2D = g2.data_ptr()
                 out[v].accumulate = acc
-            rc = lib.b200gsr_backward_views(B, prm, vin, C.c_void_p(radii.data_ptr()), C.c_void_p(depth_alpha.data_ptr()),
-                                            C.c_void_p(g_color.data_ptr()), C.c_void_p(g_da.data_ptr()),
-                                            C.c_void_p(ctx.saved_buf.data_ptr()), ctx.saved_buf.numel(), cap, out,
-                                            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+            rc = lib.b200gsr_backward_views_ex(B, prm, vin, C.c_void_p(radii.data_ptr()), C.c_void_p(depth_alpha.data_ptr()),
+                                               C.c_void_p(g_color.data_ptr()), C.c_void_p(g_da.data_ptr()),
+                                               C.c_void_p(ctx.saved_buf.data_ptr()), ctx.saved_buf.numel(), cap, out,
+                                               _lib.BWD_DETERMINISTIC if det else 0,
+                                               C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
         if rc:
             raise RuntimeError(f"b200gsr_backward_views failed ({rc}): {_lib.last_error()}")
         return (None, None, None) + tuple(grads)

@@ -38,6 +38,7 @@ class _Disparity(torch.autograd.Function):
         if rc:
             raise RuntimeError(f"b200gsr_disparity_forward failed ({rc}): {_lib.last_error()}")
         alpha = da[:, 1:2].clone()
+        ctx.deterministic = torch.are_deterministic_algorithms_enabled()   # the backward runs in the forward's mode
         ctx.save_for_backward(da, focal, stats)
         return out, alpha
 
@@ -52,11 +53,12 @@ class _Disparity(torch.autograd.Function):
         st = stats.clone()          # the backward accumulates into the record: keep the forward's pristine
         lib = _lib.load()
         with torch.cuda.device(dev):
-            rc = lib.b200gsr_disparity_backward(B, H * W, C.c_void_p(da.data_ptr()), C.c_void_p(focal.data_ptr()),
-                                                C.c_void_p(g_disp.data_ptr()),
-                                                None if g_alpha is None else C.c_void_p(g_alpha.data_ptr()),
-                                                C.c_void_p(st.data_ptr()), C.c_void_p(d_da.data_ptr()),
-                                                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+            rc = lib.b200gsr_disparity_backward_ex(B, H * W, C.c_void_p(da.data_ptr()), C.c_void_p(focal.data_ptr()),
+                                                   C.c_void_p(g_disp.data_ptr()),
+                                                   None if g_alpha is None else C.c_void_p(g_alpha.data_ptr()),
+                                                   C.c_void_p(st.data_ptr()), C.c_void_p(d_da.data_ptr()),
+                                                   _lib.BWD_DETERMINISTIC if ctx.deterministic else 0,
+                                                   C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
         if rc:
             raise RuntimeError(f"b200gsr_disparity_backward failed ({rc}): {_lib.last_error()}")
         return d_da, None

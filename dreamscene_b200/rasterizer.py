@@ -220,24 +220,33 @@ def _make_params(rs: GaussianRasterizationSettings, P: int, M: int, keep: list, 
 
 class _State:
     """Everything backward needs that is not a tensor input."""
-    __slots__ = ("params_keep", "P", "M", "capacity", "saved", "rs", "with_backward", "prm")
+    __slots__ = ("params_keep", "P", "M", "capacity", "saved", "rs", "with_backward", "prm", "deterministic")
 
 
 _layout_cache: dict = {}
 
 
-def _layouts(P, H, W, cap, with_backward):
-    key = (P, H, W, cap, with_backward)
+def _layouts(P, H, W, cap, with_backward, deterministic=False):
+    key = (P, H, W, cap, with_backward, deterministic)
     r = _layout_cache.get(key)
     if r is None:
         if len(_layout_cache) > 256:
             _layout_cache.clear()
         r = _layout_cache[key] = (_lib.scratch_layout(P, H, W, cap).total,
-                                  _lib.saved_layout(P, H, W, cap, with_backward).total)
+                                  _lib.saved_layout(P, H, W, cap, with_backward, deterministic).total)
     return r
 
 
-def _issue_with_capacity(d: _Device, dev, key, P_eff: int, H_eff: int, W: int, with_backward: bool, score, launch):
+def deterministic_mode() -> bool:
+    """Deterministic mode follows PyTorch's switch, read at forward time: under
+    torch.use_deterministic_algorithms(True) the important score, every gradient and the disparity backward are
+    summed in fixed point and are bitwise reproducible (include/b200gsr.h, "Deterministic mode").  The backward
+    always runs in the mode of its forward."""
+    return torch.are_deterministic_algorithms_enabled()
+
+
+def _issue_with_capacity(d: _Device, dev, key, P_eff: int, H_eff: int, W: int, with_backward: bool, score, launch,
+                         deterministic: bool = False):
     """The pair-capacity protocol shared by the single- and multi-view forwards.  `launch(cap, scratch,
     saved, notify_ptr, seq)` enqueues the whole forward and returns the C return code; this helper
     sizes the buffers, decides whether to wait for the device's pair count (sync mode / unknown
@@ -255,7 +264,7 @@ def _issue_with_capacity(d: _Device, dev, key, P_eff: int, H_eff: int, W: int, w
     # wait for the count only when it is needed: sync mode, or the capacity is a blind first guess
     wait = (not capturing) and (_pair_mode == "sync" or not known)
     while True:
-        scratch_bytes, saved_bytes = _layouts(P_eff, H_eff, W, cap, with_backward)
+        scratch_bytes, saved_bytes = _layouts(P_eff, H_eff, W, cap, with_backward, deterministic)
         scratch = d.ensure_scratch(stream_h, scratch_bytes)
         saved = torch.empty(saved_bytes, dtype=torch.uint8, device=dev)
         slot, seq, notify_ptr = -1, 0, None
@@ -328,7 +337,8 @@ def _forward_impl(rs, means3D, shs, colors, opac, scales, rots, cov3d, with_back
         radii = torch.empty(P, dtype=torch.int32, device=dev)
         score = torch.zeros(P, dtype=torch.float32, device=dev) if rs.score_flag else None
         stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        flags = 0 if with_backward else _lib.FWD_NO_BACKWARD
+        det = deterministic_mode()
+        flags = (0 if with_backward else _lib.FWD_NO_BACKWARD) | (_lib.FWD_DETERMINISTIC if det else 0)
 
         def launch(cap, scratch, saved, notify_ptr, seq):
             return lib.b200gsr_forward(C.byref(prm), _ptr(means3D), _ptr(shs), _ptr(colors), _ptr(opac),
@@ -336,10 +346,11 @@ def _forward_impl(rs, means3D, shs, colors, opac, scales, rots, cov3d, with_back
                                        _ptr(radii), _ptr(score), _ptr(scratch), scratch.numel(), _ptr(saved),
                                        saved.numel(), cap, flags, notify_ptr, seq, stream)
 
-        saved, cap = _issue_with_capacity(d, dev, (P, H, W), P, H, W, with_backward, score, launch)
+        saved, cap = _issue_with_capacity(d, dev, (P, H, W), P, H, W, with_backward, score, launch, det)
     st = _State()
     st.params_keep = keep; st.P = P; st.M = M; st.capacity = cap; st.saved = saved; st.rs = rs
     st.with_backward = with_backward
+    st.deterministic = det
     st.prm = prm                      # the backward reuses the struct (its device pointers are kept alive by `keep`)
     return color, radii, depth_alpha, score, st
 
@@ -441,6 +452,7 @@ class _RasterizeGaussians(torch.autograd.Function):
             with torch.cuda.device(dev):
                 prm = st.prm
                 stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+                det_bit = _lib.BWD_DETERMINISTIC if st.deterministic else 0
 
                 def launch(stages, g0, g1):
                     rc = lib.b200gsr_backward_ex(
@@ -448,7 +460,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                         _ptr(rots), _ptr(cov3d), _ptr(radii), _ptr(depth_alpha), _ptr(g_color), _ptr(g_da),
                         _ptr(st.saved), st.saved.numel(), None, 0, st.capacity,
                         _ptr(d_means3D), _ptr(d_means2D), _ptr(d_sh), _ptr(d_colors), _ptr(d_opac),
-                        _ptr(d_scales), _ptr(d_rots), _ptr(d_cov), stages, g0, g1,
+                        _ptr(d_scales), _ptr(d_rots), _ptr(d_cov), stages | det_bit, g0, g1,
                         -1 if factored else (ncoef if compact else 0), stream)
                     if rc:
                         raise RuntimeError(f"b200gsr_backward failed ({rc}): {_lib.last_error()}")

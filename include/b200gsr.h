@@ -105,11 +105,32 @@ const char* b200gsr_last_error(void);
 
 /* forward flags */
 #define B200GSR_FWD_NO_BACKWARD 1u   /* `saved` was sized with with_backward = 0: skip the gradient accumulators */
+#define B200GSR_FWD_DETERMINISTIC 2u /* deterministic mode (see below); `saved` sized with B200GSR_SAVED_DETERMINISTIC */
+
+/*
+ * Deterministic mode.  By default the important score and the screen-space gradient accumulators are summed
+ * with fp32 atomics, whose order (and so whose last bits) varies from run to run.  In deterministic mode they
+ * are summed as 64-bit fixed-point integers, which makes the score, every gradient and the disparity backward
+ * bitwise reproducible for the same inputs, shapes, library build and GPU model - across repeats, streams,
+ * processes and CUDA-graph replays - and independent of how the work is split (one view of a multi-view call
+ * equals the single-view call).  Costs: a second replay of the backward's compositing kernel, and
+ * 120 B (+ 8 B with score_flag) per Gaussian of extra `saved` state.  Limits: at most 2^18 16x16 tiles per view
+ * (8192 x 8192), else B200GSR_ERR_UNSUPPORTED.  A NaN or Inf partial gives a NaN gradient component.
+ *   forward  : flags |= B200GSR_FWD_DETERMINISTIC; `score` (score_flag) is then overwritten, not accumulated;
+ *   backward : stages |= B200GSR_BWD_DETERMINISTIC (b200gsr_backward_ex), or flags = B200GSR_BWD_DETERMINISTIC
+ *              for the multi-view and disparity backward entry points.  The backward must use the mode of
+ *              its forward; a deterministic backward on a `saved` buffer sized without the deterministic
+ *              arrays returns B200GSR_ERR_WORKSPACE.
+ *   layouts  : with_backward |= B200GSR_SAVED_DETERMINISTIC appends the arrays after bwd_items (every offset of
+ *              b200gsr_saved_layout is unchanged, only `total` grows): uint32[P*10] per-component maxima and
+ *              int64[P*10] fixed-point sums (with backward), int64[P] fixed-point score (always).
+ */
+#define B200GSR_SAVED_DETERMINISTIC 0x100
 
 /* Sizes/offsets of the two caller-owned buffers.  `saved` must stay alive until backward;
  * `scratch` is transient (forward only).  max_pairs = capacity for (tile,Gaussian) pairs
  * ("num_rendered").  with_backward = 0 drops the 48 B/Gaussian accumulator array (inference,
- * important_score renders). */
+ * important_score renders); B200GSR_SAVED_DETERMINISTIC may be OR-ed in (deterministic mode, above). */
 int b200gsr_saved_layout_query(int32_t P, int32_t H, int32_t W, uint64_t max_pairs,
                                int32_t with_backward, b200gsr_saved_layout* out);
 int b200gsr_scratch_layout_query(int32_t P, int32_t H, int32_t W, uint64_t max_pairs,
@@ -175,6 +196,7 @@ int b200gsr_backward(const b200gsr_params* prm,
  */
 #define B200GSR_BWD_COMPOSITE 1u
 #define B200GSR_BWD_PROJECT 2u
+#define B200GSR_BWD_DETERMINISTIC 4u   /* deterministic mode (see B200GSR_FWD_DETERMINISTIC); give it to every stage */
 int b200gsr_backward_ex(const b200gsr_params* prm,
                         const float* means3D, const float* shs, const float* colors_precomp,
                         const float* opacities, const float* scales, const float* rotations,
@@ -232,6 +254,11 @@ int b200gsr_backward_views(int32_t B, const b200gsr_params* prm, const b200gsr_v
                            const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
                            const float* dL_ddepth_alpha, void* saved, size_t saved_bytes, uint64_t max_pairs,
                            const b200gsr_view_grads* out, void* stream);
+/* The same with a flags word: 0 or B200GSR_BWD_DETERMINISTIC. */
+int b200gsr_backward_views_ex(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in,
+                              const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
+                              const float* dL_ddepth_alpha, void* saved, size_t saved_bytes, uint64_t max_pairs,
+                              const b200gsr_view_grads* out, uint32_t flags, void* stream);
 
 /* Frustum test only (replaces _C.mark_visible; DreamScene never calls it): visible[P] bytes. */
 int b200gsr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix,
@@ -290,6 +317,11 @@ int b200gsr_disparity_forward(int32_t B, int32_t N, const float* depth_alpha, co
 int b200gsr_disparity_backward(int32_t B, int32_t N, const float* depth_alpha, const float* focal,
                                const float* g_disp, const float* g_alpha, void* stats,
                                float* d_depth_alpha, void* stream);
+/* The same with a flags word: B200GSR_BWD_DETERMINISTIC sums the per-view gradient terms in a fixed order
+ * (d_depth_alpha doubles as the scratch space of the partial sums before it is written). */
+int b200gsr_disparity_backward_ex(int32_t B, int32_t N, const float* depth_alpha, const float* focal,
+                                  const float* g_disp, const float* g_alpha, void* stats,
+                                  float* d_depth_alpha, uint32_t flags, void* stream);
 
 /*
  * SURVEY.md 8(f4): densification / pruning primitives (/root/reference/gs_renderer.py:854-1087).
