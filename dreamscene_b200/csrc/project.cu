@@ -10,7 +10,6 @@
 // written in the oracle, so those integers are bit-exact against it.
 #include "common.cuh"
 #include <cuda_fp16.h>
-#include <cstdlib>
 
 #define MUL(a, b) __fmul_rn((a), (b))
 #define ADD(a, b) __fadd_rn((a), (b))
@@ -437,8 +436,9 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
 //   2: sum g*dx*dx  3: sum g*dx*dy  4: sum g*dy*dy
 //   5: sum G*dL/dalpha (dL/dopacity)   6..8: dL/drgb   9: dL/ddepth   10,11: unused
 // =========================================================================================
-template <int MT, int MINB>
-__global__ void __launch_bounds__(kBlock, MINB)
+// 6 CTAs/SM (80 registers): with the parameter loads hoisted above the SH wait, 8 CTAs/SM (64 registers) spills heavily.
+template <int MT>
+__global__ void __launch_bounds__(kBlock, 6)
 project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
                    const float* __restrict__ shs, const float* __restrict__ colors,
                    const float* __restrict__ scales, const float* __restrict__ rots,
@@ -813,29 +813,15 @@ cudaError_t gsr_launch_project(const GsrFwdArgs& a) {
     return cudaGetLastError();
 }
 
-template <int MT, int MINB>
-static void launch_project_bwd_v(const GsrBwdArgs& a, int g_begin, int g_end, size_t smem) {
-    project_bwd_kernel<MT, MINB><<<(g_end - g_begin + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
+template <int MT>
+static void launch_project_bwd(const GsrBwdArgs& a, int g_begin, int g_end, size_t smem) {
+    project_bwd_kernel<MT><<<(g_end - g_begin + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
         a.prm, a.means3D, a.shs, a.colors, a.scales, a.rots, a.cov3d, a.radii,
         reinterpret_cast<float*>(a.saved + a.vl.dgeom),
         reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE, g_begin, g_end,
         a.dsh_coefs > 0 ? a.dsh_coefs : (a.dsh_coefs < 0 ? -1 : a.prm.M), a.view * a.P_view, a.accumulate, a.d_means3D,
         a.d_means2D, a.d_shs,
         a.d_colors, a.d_opac, a.d_scales, a.d_rots, a.d_cov3d);
-}
-
-// register budget of project_bwd.  Since the parameter loads were hoisted above the SH wait (they overlap the
-// cp.async staging), 8 CTAs/SM (64 registers) spills heavily; the default is 6 CTAs/SM (80 registers).
-// B200GSR_PBWD_MINB = 8 | 6 | 5 selects for A/B runs.
-#ifndef GSR_PBWD_DEFAULT_MINB
-#define GSR_PBWD_DEFAULT_MINB 6
-#endif
-template <int MT>
-static void launch_project_bwd(const GsrBwdArgs& a, int g_begin, int g_end, size_t smem) {
-    static const int minb = [] { const char* e = getenv("B200GSR_PBWD_MINB"); return e ? atoi(e) : GSR_PBWD_DEFAULT_MINB; }();
-    if (minb == 8) launch_project_bwd_v<MT, 8>(a, g_begin, g_end, smem);
-    else if (minb == 5) launch_project_bwd_v<MT, 5>(a, g_begin, g_end, smem);
-    else launch_project_bwd_v<MT, 6>(a, g_begin, g_end, smem);
 }
 
 cudaError_t gsr_launch_project_bwd(const GsrBwdArgs& a) {
