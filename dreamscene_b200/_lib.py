@@ -17,7 +17,7 @@ EXPORTS = ["b200gsr_version", "b200gsr_last_error", "b200gsr_saved_layout_query"
            "b200gsr_densify_plan", "b200gsr_densify_map", "b200gsr_compact_plan", "b200gsr_gather_rows",
            "b200gsr_split_children", "b200gsr_kth_smallest", "b200gsr_views_geometry", "b200gsr_forward_views",
            "b200gsr_backward_views", "b200gsr_sh_grad_expand", "b200gsr_backward_views_ex",
-           "b200gsr_disparity_backward_ex"]
+           "b200gsr_disparity_backward_ex", "b200gsr_score_views", "b200gsr_score_finish"]
 
 
 class Params(C.Structure):
@@ -39,6 +39,7 @@ class GroupGrad(C.Structure):       # == b200gsr_group_grad
 
 MAX_GROUPS = 24
 MAX_VIEWS = 16
+SCORE_DET_MAX_PIXELS = 1 << 26     # B200GSR_SCORE_DET_MAX_PIXELS: pixels of all views summed into one int64 score
 
 
 class ViewInputs(C.Structure):      # == b200gsr_view_inputs
@@ -135,6 +136,9 @@ def load():
     lib.b200gsr_backward_views_ex.argtypes = lib.b200gsr_backward_views.argtypes[:-1] + [u32, vp]
     for fn in ("b200gsr_views_geometry", "b200gsr_forward_views", "b200gsr_backward_views", "b200gsr_backward_views_ex"):
         getattr(lib, fn).restype = C.c_int
+    lib.b200gsr_score_views.argtypes = [i32, C.POINTER(Params), C.POINTER(ViewInputs), vp, vp, sz, vp, sz, u64, u32, vp, u32, vp]
+    lib.b200gsr_score_finish.argtypes = [i32, vp, vp, u32, vp]
+    lib.b200gsr_score_views.restype = lib.b200gsr_score_finish.restype = C.c_int
     lib.b200gsr_debug_counters.argtypes = [vp]
     lib.b200gsr_debug_counters.restype = C.c_int
     lib.b200gsr_profile_enable.argtypes = [i32]

@@ -504,6 +504,104 @@ int b200gsr_backward_views(int32_t B, const b200gsr_params* prm, const b200gsr_v
                                      max_pairs, out, 0u, stream);
 }
 
+// Score pass: only geometry and opacity are read, so the colour inputs validate_inputs insists on are not required.
+static int check_score_views(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in) {
+    if (B < 1 || B > B200GSR_MAX_VIEWS) return fail(B200GSR_ERR_UNSUPPORTED, "number of views %d not in 1..%d", B, B200GSR_MAX_VIEWS);
+    if (!prm || !in) return fail(B200GSR_ERR_BAD_ARG, "null view array");
+    for (int v = 0; v < B; ++v) {
+        const b200gsr_params& p = prm[v];
+        if (p.P < 0 || p.image_height < 0 || p.image_width < 0) return fail(B200GSR_ERR_BAD_ARG, "view %d: negative size", v);
+        if (p.image_height > 65535 * 16 || p.image_width > 65535 * 16)
+            return fail(B200GSR_ERR_UNSUPPORTED, "image larger than 65535 tiles per axis");
+        if (!p.viewmatrix || !p.projmatrix || !p.campos)
+            return fail(B200GSR_ERR_BAD_ARG, "view %d: viewmatrix/projmatrix/campos must be device pointers", v);
+        if (p.P != prm[0].P || p.image_height != prm[0].image_height || p.image_width != prm[0].image_width)
+            return fail(B200GSR_ERR_BAD_ARG, "view %d: P and image size must equal view 0's", v);
+        if (p.P > 0) {
+            const b200gsr_view_inputs& x = in[v];
+            if (!x.means3D || !x.opacities) return fail(B200GSR_ERR_BAD_ARG, "view %d: means3D/opacities are required", v);
+            const bool has_sr = x.scales != nullptr || x.rotations != nullptr;
+            if (((x.scales == nullptr || x.rotations == nullptr) && x.cov3D_precomp == nullptr) || (has_sr && x.cov3D_precomp != nullptr))
+                return fail(B200GSR_ERR_BAD_ARG,
+                            "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
+        }
+    }
+    if ((long long)B * prm[0].P > 0x3fffffffLL) return fail(B200GSR_ERR_UNSUPPORTED, "B * P too large");
+    return B200GSR_OK;
+}
+
+int b200gsr_score_views(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, void* score_acc,
+                        void* scratch, size_t scratch_bytes, void* saved, size_t saved_bytes, uint64_t max_pairs,
+                        uint32_t flags, uint32_t* host_notify, uint32_t notify_seq, void* stream) {
+    int rc = check_score_views(B, prm, in);
+    if (rc) return rc;
+    if (flags & ~(B200GSR_FWD_NO_BACKWARD | B200GSR_FWD_DETERMINISTIC)) return fail(B200GSR_ERR_BAD_ARG, "unknown flags 0x%x", flags);
+    const int P = prm[0].P, H = prm[0].image_height, W = prm[0].image_width;
+    if ((P > 0 && !score_acc) || !scratch || !saved) return fail(B200GSR_ERR_BAD_ARG, "null accumulator/workspace pointer");
+    const GsrTileGrid g1 = gsr_grid(H, W);
+    const int Hs = B * g1.gy * GSR_TILE;
+    GsrFwdArgs a{};
+    a.det = (flags & B200GSR_FWD_DETERMINISTIC) != 0;
+    if (a.det && (rc = check_det_size(H, W))) return rc;
+    if (a.det && (long long)B * H * W > B200GSR_SCORE_DET_MAX_PIXELS)
+        return fail(B200GSR_ERR_UNSUPPORTED, "deterministic score: %d views of %dx%d exceed 2^26 pixels per accumulator", B, W, H);
+    if ((rc = b200gsr_scratch_layout_query(B * P, Hs, W, max_pairs, &a.sl))) return rc;
+    if ((rc = b200gsr_saved_layout_query(B * P, Hs, W, max_pairs, 0, &a.vl))) return rc;
+    if (scratch_bytes < a.sl.total || saved_bytes < a.vl.total)
+        return fail(B200GSR_ERR_WORKSPACE, "workspace too small: scratch %zu < %zu or saved %zu < %zu",
+                    scratch_bytes, a.sl.total, saved_bytes, a.vl.total);
+    DeviceState* ds = device_state();
+    if (!ds) return fail(B200GSR_ERR_CUDA, "cannot query the current CUDA device");
+    a.scratch = static_cast<uint8_t*>(scratch); a.saved = static_cast<uint8_t*>(saved);
+    a.max_pairs = (uint32_t)max_pairs;
+    a.host_notify = host_notify; a.notify_seq = notify_seq;
+    a.flags = flags | B200GSR_FWD_NO_BACKWARD; a.num_sms = ds->num_sms; a.stats = nullptr;
+    a.num_views = B; a.P_view = P; a.gy_view = g1.gy;
+    a.stream = static_cast<cudaStream_t>(stream);
+    const int ntiles = g1.gx * g1.gy * B;
+    if (!gsr_use_multisplit(ntiles) || P == 0) {
+        const size_t nbytes = gsr_use_multisplit(ntiles) ? a.sl.tile_count + (size_t)ntiles * sizeof(uint32_t) : a.sl.tile_cursor;
+        if ((rc = check_cuda(cudaMemsetAsync(a.scratch, 0, nbytes, a.stream), "memset"))) return rc;
+    }
+    prof_mark_fwd(0, a.stream);
+    GSR_RANGE_PUSH("b200gsr.score.project_geo");
+    for (int v = 0; v < B && !rc; ++v) {
+        a.prm = prm[v]; a.view = v;
+        a.means3D = in[v].means3D; a.opac = in[v].opacities;
+        a.scales = in[v].scales; a.rots = in[v].rotations; a.cov3d = in[v].cov3D_precomp;
+        rc = check_cuda(gsr_launch_project_geo(a), "project_geo");
+    }
+    a.prm = prm[0]; a.view = 0;
+    if (!rc) rc = check_cuda(gsr_launch_count(a), "tile_count");
+    GSR_RANGE_POP();
+    if (rc) return rc;
+    prof_mark_fwd(1, a.stream);
+    GSR_RANGE_PUSH("b200gsr.score.binning+sort");
+    rc = check_cuda(gsr_launch_scan(a), "scan_order");
+    prof_mark_fwd(2, a.stream);
+    if (!rc) rc = check_cuda(gsr_launch_scatter(a), "scatter");
+    prof_mark_fwd(3, a.stream);
+    if (!rc) rc = check_cuda(gsr_launch_sort(a, ds->stream, ds->fork, ds->join), "tile_sort");
+    GSR_RANGE_POP();
+    if (rc) return rc;
+    prof_mark_fwd(4, a.stream);
+    GSR_RANGE_PUSH("b200gsr.score.composite");
+    rc = check_cuda(gsr_launch_composite_score(a, score_acc), "composite_score");
+    GSR_RANGE_POP();
+    if (rc) return rc;
+    prof_mark_fwd(5, a.stream);
+    if (g_prof.max_calls > 0 && g_prof.nfwd < g_prof.max_calls) ++g_prof.nfwd;
+    return B200GSR_OK;
+}
+
+int b200gsr_score_finish(int32_t P, const void* score_acc, float* score, uint32_t flags, void* stream) {
+    if (P < 0 || (P > 0 && (!score_acc || !score))) return fail(B200GSR_ERR_BAD_ARG, "bad score_finish arguments");
+    if (flags != B200GSR_FWD_DETERMINISTIC)
+        return fail(B200GSR_ERR_BAD_ARG, "score_finish converts a deterministic (int64) accumulator: flags must be B200GSR_FWD_DETERMINISTIC");
+    return check_cuda(gsr_launch_score_finish(P, static_cast<const unsigned long long*>(score_acc), score,
+                                              static_cast<cudaStream_t>(stream)), "score_finish");
+}
+
 int b200gsr_profile_enable(int32_t max_calls) {
     for (int i = 0; i < g_prof.max_calls * kFwdEvents; ++i) cudaEventDestroy(g_prof.fwd[i]);
     for (int i = 0; i < g_prof.max_calls * kBwdEvents; ++i) cudaEventDestroy(g_prof.bwd[i]);

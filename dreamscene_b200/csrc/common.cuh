@@ -263,6 +263,11 @@ cudaError_t gsr_launch_scatter(const GsrFwdArgs& a);       // append keys to til
 cudaError_t gsr_launch_sort(const GsrFwdArgs& a, cudaStream_t side, cudaEvent_t fork, cudaEvent_t join);   // per-tile sort (2 kernels, concurrent when `side` is given)
 cudaError_t gsr_launch_composite_fwd(const GsrFwdArgs& a);
 cudaError_t gsr_launch_composite_bwd(const GsrBwdArgs& a);
+// score pass (b200gsr_score_views): geometry-only projection and score-only compositing into score_acc
+// (float [P_view], or int64 [P_view] with a.det); score_finish converts an int64 accumulator to float
+cudaError_t gsr_launch_project_geo(const GsrFwdArgs& a);
+cudaError_t gsr_launch_composite_score(const GsrFwdArgs& a, void* score_acc);
+cudaError_t gsr_launch_score_finish(int n, const unsigned long long* score_fx, float* score, cudaStream_t s);
 cudaError_t gsr_launch_project_bwd(const GsrBwdArgs& a);
 cudaError_t gsr_launch_sh_grad_expand(int P, int M, int deg, int nviews, const float* means3D, const float* dcol,
                                       size_t stride, float* d_shs, cudaStream_t s);

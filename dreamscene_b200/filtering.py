@@ -1,0 +1,230 @@
+"""3D Gaussian filtering (SURVEY.md section 8(a) a9) - additive API over b200gsr_score_views.
+
+The reference (/root/reference/scene_gaussian.py:1046-1103) prunes an object in three steps:
+  prune_list             48 full score_flag renders from random sphere cameras, scores summed in view order;
+  calculate_v_imp_score  the summed score weighted by (volume / kth) ** v_pow, kth = element int(0.9 n) of the
+                         volumes sorted in descending order;
+  prune_gaussians        drop everything at or below the percent-th element of the sorted weighted score.
+Here:
+  important_score        the summed score of any number of views, as stacked score-only passes (no SH read, no
+                         image, no backward state) adding into one [P] accumulator;
+  volume_weighted_score  calculate_v_imp_score with the same elementwise torch ops and the sort replaced by
+                         b200gsr_kth_smallest (no host sync);
+  gaussian_filtering     both, then densify.prune_by_score; returns what densify.prune_points returns.
+
+Under torch.use_deterministic_algorithms(True) (read at call time) the score is summed in 64-bit fixed point:
+bitwise reproducible and independent of views_per_pass.  Its headroom is 2^26 pixels over all views of one call
+(256 views of 512 x 512); larger camera sets are refused.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import time
+from typing import Dict, Optional, Sequence, Tuple
+
+import torch
+
+from . import _lib
+from . import densify as _densify
+from . import rasterizer as R
+
+
+def _check(rc, what):
+    if rc:
+        raise RuntimeError(f"{what} failed ({rc}): {_lib.last_error()}")
+
+
+def _wait_pairs(d: R._Device, dev, slot: int, seq: int) -> int:
+    """Wait for one pass's tile scan to report its pair count through the notify ring; frees the slot."""
+    n = d.notify_np
+    t0 = time.perf_counter()
+    while int(n[slot, 0]) != seq:
+        if time.perf_counter() - t0 > R._POLL_TIMEOUT_S:
+            torch.cuda.synchronize(dev)
+            if int(n[slot, 0]) == seq:
+                break
+            raise RuntimeError("b200gsr_score_views: device never reported the pair count")
+    pairs = int(n[slot, 1]) & 0xFFFFFFFF
+    d.free_slots.append(slot)
+    d.last_pairs = pairs
+    return pairs
+
+
+def _note_capacity(d: R._Device, key, pairs: int) -> None:
+    if not d.user_capacity:
+        d.caps[key] = max(d.caps.get(key, 0), R._round_cap(2 * pairs))
+        d.capacity = max(d.capacity, d.caps[key])
+
+
+def view_chunks(n_views: int, views_per_pass: int):
+    """[(first, end)] of the stacked passes that cover n_views views, at most views_per_pass each."""
+    return [(b, min(b + views_per_pass, n_views)) for b in range(0, n_views, views_per_pass)]
+
+
+def important_score(settings_list: Sequence[R.GaussianRasterizationSettings], means3D: torch.Tensor,
+                    opacities: torch.Tensor, scales: Optional[torch.Tensor] = None,
+                    rotations: Optional[torch.Tensor] = None, cov3D_precomp: Optional[torch.Tensor] = None, *,
+                    views_per_pass: int = 16) -> torch.Tensor:
+    """-> float32 [P]: the sum over the views of settings_list of the important score that
+    GaussianRasterizer(settings with score_flag=True) returns (sh_degree, bg and score_flag of the settings are
+    irrelevant).  Non-differentiable.  The views run as stacked passes of up to views_per_pass views
+    (1..16) adding into one accumulator.  A pass that overflowed its pair capacity adds nothing and is re-issued
+    with a larger one, so the result never contains a partial pass."""
+    views_per_pass = int(views_per_pass)
+    if not 1 <= views_per_pass <= _lib.MAX_VIEWS:
+        raise ValueError(f"views_per_pass must be in 1..{_lib.MAX_VIEWS}, got {views_per_pass}")
+    if ((scales is None or rotations is None) and cov3D_precomp is None) or \
+            ((scales is not None or rotations is not None) and cov3D_precomp is not None):
+        raise ValueError("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!")
+    settings_list = list(settings_list)
+    n_views = len(settings_list)
+    if n_views:
+        H, W = int(settings_list[0].image_height), int(settings_list[0].image_width)
+        for s in settings_list:
+            if int(s.image_height) != H or int(s.image_width) != W:
+                raise ValueError("all views must share the image size")
+    else:
+        H = W = 0
+    det = R.deterministic_mode()
+    if det and n_views * H * W > _lib.SCORE_DET_MAX_PIXELS:
+        raise ValueError(f"deterministic important score: {n_views} views of {W}x{H} are {n_views * H * W} pixels; the "
+                         f"64-bit fixed-point sum has headroom for {_lib.SCORE_DET_MAX_PIXELS} (2^26) pixels")
+    dev = means3D.device
+    if dev.type != "cuda":
+        raise RuntimeError("important_score (b200gsr): inputs must be CUDA tensors; there is no CPU fallback")
+    if torch.cuda.is_current_stream_capturing():
+        raise RuntimeError("important_score waits for the pair counts of its passes and cannot be captured into a CUDA graph")
+    P = int(means3D.shape[0])
+    if P == 0 or n_views == 0:
+        return torch.zeros(P, dtype=torch.float32, device=dev)
+    lib = _lib.load()
+    with torch.no_grad(), torch.cuda.device(dev):
+        means3D, opacities = R._f32c(means3D.detach()), R._f32c(opacities.detach())
+        scales = R._f32c(None if scales is None else scales.detach())
+        rotations = R._f32c(None if rotations is None else rotations.detach())
+        cov3D_precomp = R._f32c(None if cov3D_precomp is None else cov3D_precomp.detach())
+        d = R._device_state(dev)
+        d.ensure_notify()
+        R._resolve_pending(d)                  # non-blocking overflow check of earlier forwards, as every forward does
+        stream_h = torch.cuda.current_stream(dev).cuda_stream
+        stream = C.c_void_p(stream_h)
+        acc = torch.zeros(P, dtype=torch.int64 if det else torch.float32, device=dev)
+        flags = _lib.FWD_NO_BACKWARD | (_lib.FWD_DETERMINISTIC if det else 0)
+        cams = [(s, R._const(s.viewmatrix, dev), R._const(s.projmatrix, dev), R._const(s.campos, dev))
+                for s in settings_list]
+
+        def issue(b0, b1, cap):
+            B = b1 - b0
+            prm = (_lib.Params * B)()
+            vin = (_lib.ViewInputs * B)()
+            for v in range(B):
+                s, vm, pm, cp = cams[b0 + v]
+                prm[v] = _lib.Params(P, 0, 0, H, W, float(s.tanfovx), float(s.tanfovy), float(s.scale_modifier),
+                                     int(bool(s.prefiltered)), 1, None, vm.data_ptr(), pm.data_ptr(), cp.data_ptr())
+                vin[v] = _lib.ViewInputs(means3D.data_ptr(), None, None, opacities.data_ptr(),
+                                         None if scales is None else scales.data_ptr(),
+                                         None if rotations is None else rotations.data_ptr(),
+                                         None if cov3D_precomp is None else cov3D_precomp.data_ptr())
+            hs = C.c_int32(0)
+            _check(lib.b200gsr_views_geometry(B, H, W, C.byref(hs)), "b200gsr_views_geometry")
+            scratch_bytes, saved_bytes = R._layouts(B * P, int(hs.value), W, cap, False)
+            scratch = d.ensure_scratch(stream_h, scratch_bytes)
+            saved = torch.empty(saved_bytes, dtype=torch.uint8, device=dev)
+            if not d.free_slots:
+                R._resolve_pending(d, block=True)
+            slot, seq = d.free_slots.pop(), d.next_seq()
+            rc = lib.b200gsr_score_views(B, prm, vin, C.c_void_p(acc.data_ptr()), C.c_void_p(scratch.data_ptr()),
+                                         scratch.numel(), C.c_void_p(saved.data_ptr()), saved.numel(), cap, flags,
+                                         C.c_void_p(d.notify.data_ptr() + 16 * slot), seq, stream)
+            if rc:
+                d.free_slots.append(slot)
+                raise RuntimeError(f"b200gsr_score_views failed ({rc}): {_lib.last_error()}")
+            return slot, seq
+
+        def capacity(key, B):
+            measured = d.capacity if d.user_capacity else d.caps.get(key, 0)
+            if measured > 0:
+                return R._round_cap(max(measured, R._MIN_PAIRS_PER_GAUSSIAN * B * P)), True
+            return R._round_cap(6 * B * P), False
+
+        # Every pass is issued without waiting once its shape's capacity is known; the pair counts are read after
+        # the last pass is enqueued, and only passes that overflowed (and so added nothing) are issued again.
+        pending = []
+        for b0, b1 in view_chunks(n_views, views_per_pass):
+            key = (b1 - b0, P, H, W)
+            cap, known = capacity(key, b1 - b0)
+            item = (b0, b1, key, cap) + issue(b0, b1, cap)
+            if known:
+                pending.append(item)
+                if len(pending) >= 64:              # bound the notify slots held by this call
+                    _settle(d, dev, issue, pending)
+                    pending = []
+            else:
+                _settle(d, dev, issue, [item])      # a shape seen for the first time: learn its capacity now
+        _settle(d, dev, issue, pending)
+
+        if not det:
+            return acc
+        score = torch.empty(P, dtype=torch.float32, device=dev)
+        _check(lib.b200gsr_score_finish(P, C.c_void_p(acc.data_ptr()), C.c_void_p(score.data_ptr()),
+                                        _lib.FWD_DETERMINISTIC, stream), "b200gsr_score_finish")
+        return score
+
+
+def _settle(d, dev, issue, pending):
+    """Read the pair count of every pending pass; re-issue (and wait for) each one that overflowed, with room
+    for its measured count, until it fits."""
+    for b0, b1, key, cap, slot, seq in pending:
+        pairs = _wait_pairs(d, dev, slot, seq)
+        while pairs > cap:
+            cap = R._round_cap(2 * pairs)
+            d.capacity = max(d.capacity, cap)
+            slot, seq = issue(b0, b1, cap)
+            pairs = _wait_pairs(d, dev, slot, seq)
+        _note_capacity(d, key, pairs)
+
+
+def _kth_smallest(v: torch.Tensor, k: int) -> torch.Tensor:
+    """-> device tensor [1]: the k-th smallest (0-based) element of v, without a sort or host sync."""
+    v = v.detach().float().contiguous()
+    out = torch.empty(1, dtype=torch.float32, device=v.device)
+    scratch = torch.empty(2048, dtype=torch.uint8, device=v.device)
+    with torch.cuda.device(v.device):
+        _check(_lib.load().b200gsr_kth_smallest(int(v.numel()), C.c_void_p(v.data_ptr()), int(k),
+                                                C.c_void_p(scratch.data_ptr()), C.c_void_p(out.data_ptr()),
+                                                C.c_void_p(torch.cuda.current_stream(v.device).cuda_stream)),
+               "b200gsr_kth_smallest")
+    return out
+
+
+def volume_weighted_score(score: torch.Tensor, scaling_raw: torch.Tensor, v_pow: float) -> torch.Tensor:
+    """calculate_v_imp_score: score * (volume / kth) ** v_pow with volume = prod(exp(scaling_raw), 1) and kth the
+    element int(0.9 n) of the volumes in descending order.  The elementwise ops are the reference's torch ops (so
+    bit-identical); the sort is replaced by b200gsr_kth_smallest at rank n - 1 - int(0.9 n) (no host sync)."""
+    volume = torch.prod(torch.exp(scaling_raw.detach()), dim=1)
+    n = int(volume.numel())
+    if n == 0:
+        return torch.zeros_like(volume)
+    index = int(n * 0.9)
+    kth = _kth_smallest(volume, n - 1 - index).reshape(())
+    v_list = torch.pow(volume / kth, v_pow)
+    return v_list * score.detach()
+
+
+def gaussian_filtering(params: Dict[str, torch.Tensor], adam: Optional[Dict[str, Tuple[torch.Tensor, torch.Tensor]]],
+                       stats: Optional[Dict[str, torch.Tensor]], settings_list: Sequence[R.GaussianRasterizationSettings],
+                       v_pow: float, prune_decay: float, prune_percent: float, *, views_per_pass: int = 16,
+                       score: Optional[torch.Tensor] = None):
+    """The reference's gaussian_filtering on a params dict (raw leaves xyz, opacity, scaling, rotation, ... as in
+    densify): important score over settings_list of the activated Gaussians (sigmoid opacity, exp scaling,
+    normalised rotation), volume weighting, then prune_by_score at percent prune_decay ** 1 * prune_percent.
+    score: a precomputed important score [P] instead of the renders (e.g. one summed over ranks).
+    -> (params, adam, stats) of the kept rows, as densify.prune_points."""
+    if score is None:
+        with torch.no_grad():
+            score = important_score(settings_list, params["xyz"], torch.sigmoid(params["opacity"]),
+                                    scales=torch.exp(params["scaling"]),
+                                    rotations=torch.nn.functional.normalize(params["rotation"]),
+                                    views_per_pass=views_per_pass)
+    v_list = volume_weighted_score(score, params["scaling"], v_pow)
+    return _densify.prune_by_score(params, adam, stats, v_list, (prune_decay ** 1) * prune_percent)

@@ -89,3 +89,31 @@ def camera_from_pose(pose: np.ndarray, fovx: float, height: int, width: int,
 def orbit_camera(radius=3.5, theta_deg=60.0, phi_deg=0.0, fovx=0.55, height=512, width=512,
                  device="cpu") -> OrbitCamera:
     return camera_from_pose(orbit_pose(radius, theta_deg, phi_deg), fovx, height, width, device=device)
+
+
+def _safe_normalize(x: torch.Tensor) -> torch.Tensor:
+    return x / torch.sqrt(torch.clamp(torch.sum(x * x, -1, keepdim=True), min=1e-20))
+
+
+def sphere_poses(n: int, radius: float = 3.5, generator=None) -> np.ndarray:
+    """[n, 4, 4] camera-to-world poses on a sphere around the origin, looking at it (cam_utils.py:1322-1336):
+    centres from torch.randn(n, 3) (drawn from `generator`, else the global CPU generator), the look-at of
+    orbit_pose."""
+    centers = torch.randn(n, 3, generator=generator)
+    centers /= torch.norm(centers, dim=1).unsqueeze(1).repeat(1, 3)
+    centers *= torch.tensor([radius], dtype=torch.float32)
+    fwd = _safe_normalize(centers)
+    up = torch.tensor([[0.0, 0.0, 1.0]]).repeat(n, 1)
+    right = _safe_normalize(torch.cross(fwd, up, dim=-1))
+    up = _safe_normalize(torch.cross(right, fwd, dim=-1))
+    poses = torch.eye(4, dtype=torch.float).unsqueeze(0).repeat(n, 1, 1)
+    poses[:, :3, :3] = torch.stack((-right, up, fwd), dim=-1)
+    poses[:, :3, 3] = centers
+    return poses.numpy()
+
+
+def sphere_cameras(n: int, radius: float = 3.5, fovx: float = 0.55, H: int = 512, W: int = 512, generator=None,
+                   device="cpu") -> list:
+    """The random sphere cameras of 3D Gaussian filtering (loadSphereCam -> GenerateSphereCameras,
+    cam_utils.py:1338-1366,1847-1866; the object trainer uses 48 of them at radius 3.5, FoV 0.55, 512 x 512)."""
+    return [camera_from_pose(p, fovx, H, W, device=device) for p in sphere_poses(n, radius, generator)]

@@ -260,6 +260,35 @@ int b200gsr_backward_views_ex(int32_t B, const b200gsr_params* prm, const b200gs
                               const float* dL_ddepth_alpha, void* saved, size_t saved_bytes, uint64_t max_pairs,
                               const b200gsr_view_grads* out, uint32_t flags, void* stream);
 
+/*
+ * Important score over a camera set (SURVEY.md 8(a) a9, 3D Gaussian filtering; additive, no upstream equivalent).
+ * The score of a Gaussian is sum over pixels of alpha * T, exactly what a score_flag forward returns, and it
+ * depends on geometry and opacity only.  b200gsr_score_views runs B views stacked as in b200gsr_forward_views,
+ * but reads no SH or colours and writes no image, n_contrib, radii or backward state, and ADDS the score of every
+ * view into one [P] accumulator, so any number of views can be summed over several calls:
+ *   prm[B], in[B] : as b200gsr_forward_views; in[v].shs / colors_precomp, prm[v].bg, sh_degree, M and score_flag
+ *                   are ignored (bg may be NULL).  Exactly one of (scales, rotations) / cov3D_precomp.
+ *   score_acc     : float [P], or int64 [P] fixed point with flags = B200GSR_FWD_DETERMINISTIC (then convert
+ *                   with b200gsr_score_finish).  The caller zeroes it before the first call.
+ *   scratch/saved : sized with the layout queries for (B*P, Hs, W, max_pairs) and with_backward = 0; `saved`
+ *                   holds nothing the caller needs after the call.
+ *   overflow      : if the pair count exceeds max_pairs (header[3] / host_notify as in b200gsr_forward) the call
+ *                   adds NOTHING to score_acc: re-issue it with a larger capacity and the sum is exact.
+ * Deterministic mode: the sum is bitwise reproducible and independent of how the views are split into calls (one
+ * view equals the deterministic score_flag forward bit for bit).  Headroom: the views that add into one int64
+ * accumulator may have at most 2^26 pixels in total (256 views of 512 x 512); a single call over more returns
+ * B200GSR_ERR_UNSUPPORTED, and callers that sum over several calls must enforce the total themselves.
+ * The b200gsr_profile_* store records a call like a forward: project_sh is the geometry-only projection,
+ * composite_fwd the score-only compositing.
+ */
+int b200gsr_score_views(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, void* score_acc,
+                        void* scratch, size_t scratch_bytes, void* saved, size_t saved_bytes, uint64_t max_pairs,
+                        uint32_t flags, uint32_t* host_notify, uint32_t notify_seq, void* stream);
+/* score[P] = the int64 fixed-point accumulator of deterministic b200gsr_score_views calls as float.
+ * flags must be B200GSR_FWD_DETERMINISTIC (a float accumulator already is the score). */
+int b200gsr_score_finish(int32_t P, const void* score_acc, float* score, uint32_t flags, void* stream);
+#define B200GSR_SCORE_DET_MAX_PIXELS (1LL << 26)
+
 /* Frustum test only (replaces _C.mark_visible; DreamScene never calls it): visible[P] bytes. */
 int b200gsr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix,
                          const float* projmatrix, uint8_t* visible, void* stream);
