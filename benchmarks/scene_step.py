@@ -7,8 +7,10 @@ The reference modules cannot be imported on the GPU box (absent + missing deps),
 restated here: per view  torch.cat(env, floor, objects) -> SH/scale augmentation -> rasterizer ->
 depth/alpha post-processing; 4 views per step (C_batch_size, config.py:163); one backward.
 
-  python benchmarks/scene_step.py [--steps 10] [--views 4] [--size 512]
-Prints a JSON line with the step time and the share spent inside the rasterizer.
+  python benchmarks/scene_step.py [--steps 10] [--views 4] [--size 512] [--optim none|torch|native]
+Prints a JSON line with the step time and the share spent inside the rasterizer.  --optim adds the optimizer step
+after the backward, one Adam per GaussianModel as the reference builds it: torch.optim.Adam's default path or
+dreamscene_b200.GaussianAdam (default none: no optimizer step, as before).
 """
 import argparse
 import json
@@ -151,10 +153,16 @@ def main():
     ap.add_argument("--views", type=int, default=4)
     ap.add_argument("--size", type=int, default=512)
     ap.add_argument("--glue", default="torch", choices=["torch", "fused", "fused_rng", "views"])
+    ap.add_argument("--optim", default="none", choices=["none", "torch", "native"])
     a = ap.parse_args()
     dev = torch.device("cuda", 0)
     torch.manual_seed(0)
     groups = build_scene(dev)
+    opts = []
+    if a.optim != "none":
+        from dreamscene_b200 import GaussianAdam
+        from harness.adam_ref import reference_adam
+        opts = [reference_adam(g, GaussianAdam if a.optim == "native" else torch.optim.Adam) for g in groups]
     P = sum(g["xyz"].shape[0] for g in groups)
     params = [v for g in groups for v in g.values()]
     target = torch.rand(3, a.size, a.size, device=dev)
@@ -174,6 +182,8 @@ def main():
         images = torch.stack([o["image"] for o in outs]); depths = torch.stack([o["depth"] for o in outs])
         loss = ((images - target) ** 2).mean() * 100 + depths.mean() * 0.1      # SDS -> L2 stub (+ depth path)
         loss.backward()
+        for o in opts:
+            o.step()
         torch.cuda.synchronize(); dt = time.perf_counter() - t0
         if it >= a.warmup:
             times.append(dt)
@@ -189,6 +199,8 @@ def main():
         outs = render_views(groups, cams, dev, bg) if a.glue == "views" else [render(groups, c, dev, bg, glue=a.glue) for c in cams]
         images = torch.stack([o["image"] for o in outs]); depths = torch.stack([o["depth"] for o in outs])
         (((images - target) ** 2).mean() * 100 + depths.mean() * 0.1).backward()
+        for o in opts:
+            o.step()
 
     # (a) back-to-back steps without a host sync in between (the fused paths never force one; the reference glue
     #     syncs per view in its boolean-mask indexing): host and device overlap, time = max(host, device) per step
@@ -207,7 +219,8 @@ def main():
         gpu_ms = sum(e.device_time_total for e in prof.key_averages()) / 1e3
     except Exception:
         pass
-    print(json.dumps({"config": "cfg5_scene_step (re-enactment)", "glue": a.glue, "P": P, "views": a.views, "size": a.size,
+    extra = {"optim": a.optim} if a.optim != "none" else {}
+    print(json.dumps({"config": "cfg5_scene_step (re-enactment)", "glue": a.glue, **extra, "P": P, "views": a.views, "size": a.size,
                       "M": 4, "sh_degree": 1, "step_ms": 1e3 * float(np.median(times)),
                       "step_ms_no_sync_between_steps": pipelined_ms, "device_busy_ms_per_step": gpu_ms,
                       "rasterizer_fwd_ms_per_step": float(np.median(ras_fwd)),

@@ -7,7 +7,8 @@ from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, Pair
                          flush_checks, last_pair_count, rasterize_gaussians, set_pair_count_mode,
                          set_workspace_capacity)
 from . import parallel
+from .optim import GaussianAdam
 
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians",
            "set_workspace_capacity", "set_pair_count_mode", "flush_checks", "last_pair_count",
-           "PairCapacityOverflow", "parallel"]
+           "PairCapacityOverflow", "parallel", "GaussianAdam"]

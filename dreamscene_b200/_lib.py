@@ -17,7 +17,7 @@ EXPORTS = ["b200gsr_version", "b200gsr_last_error", "b200gsr_saved_layout_query"
            "b200gsr_densify_plan", "b200gsr_densify_map", "b200gsr_compact_plan", "b200gsr_gather_rows",
            "b200gsr_split_children", "b200gsr_kth_smallest", "b200gsr_views_geometry", "b200gsr_forward_views",
            "b200gsr_backward_views", "b200gsr_sh_grad_expand", "b200gsr_backward_views_ex",
-           "b200gsr_disparity_backward_ex", "b200gsr_score_views", "b200gsr_score_finish"]
+           "b200gsr_disparity_backward_ex", "b200gsr_score_views", "b200gsr_score_finish", "b200gsr_adam_step"]
 
 
 class Params(C.Structure):
@@ -49,6 +49,14 @@ class ViewInputs(C.Structure):      # == b200gsr_view_inputs
 class ViewGrads(C.Structure):       # == b200gsr_view_grads
     _fields_ = [(n, C.c_void_p) for n in ("d_means3D", "d_means2D", "d_shs", "d_colors", "d_opacities", "d_scales",
                                           "d_rotations", "d_cov3D")] + [("accumulate", C.c_uint32)]
+
+
+ADAM_MAX_TENSORS = 32               # B200GSR_ADAM_MAX_TENSORS: tensors per b200gsr_adam_step call
+
+
+class AdamTensor(C.Structure):      # == b200gsr_adam_tensor
+    _fields_ = [(n, C.c_void_p) for n in ("param", "grad", "exp_avg", "exp_avg_sq")] + [("n", C.c_int64)] + \
+        [(n, C.c_float) for n in ("lerp_weight", "beta2", "one_minus_beta2", "eps", "step_size", "bc2_sqrt")]
 
 
 class SavedLayout(C.Structure):
@@ -139,6 +147,8 @@ def load():
     lib.b200gsr_score_views.argtypes = [i32, C.POINTER(Params), C.POINTER(ViewInputs), vp, vp, sz, vp, sz, u64, u32, vp, u32, vp]
     lib.b200gsr_score_finish.argtypes = [i32, vp, vp, u32, vp]
     lib.b200gsr_score_views.restype = lib.b200gsr_score_finish.restype = C.c_int
+    lib.b200gsr_adam_step.argtypes = [i32, C.POINTER(AdamTensor), vp]
+    lib.b200gsr_adam_step.restype = C.c_int
     lib.b200gsr_debug_counters.argtypes = [vp]
     lib.b200gsr_debug_counters.restype = C.c_int
     lib.b200gsr_profile_enable.argtypes = [i32]

@@ -767,6 +767,19 @@ int b200gsr_kth_smallest(int32_t n, const float* v, uint32_t k, void* scratch, f
     return check_cuda(gsr_kth_smallest(n, v, k, scratch, out, ds->num_sms, GSR_ST(stream)), "kth_smallest");
 }
 
+int b200gsr_adam_step(int32_t n_tensors, const b200gsr_adam_tensor* tensors, void* stream) {
+    if (n_tensors < 0 || (n_tensors > 0 && !tensors)) return fail(B200GSR_ERR_BAD_ARG, "bad adam_step arguments");
+    if (n_tensors > B200GSR_ADAM_MAX_TENSORS)
+        return fail(B200GSR_ERR_UNSUPPORTED, "adam_step: %d tensors, at most %d per call", n_tensors, B200GSR_ADAM_MAX_TENSORS);
+    for (int i = 0; i < n_tensors; ++i) {
+        const b200gsr_adam_tensor& t = tensors[i];
+        if (t.n < 0) return fail(B200GSR_ERR_BAD_ARG, "adam_step: tensor %d has a negative length", i);
+        if (t.n > 0 && (!t.param || !t.grad || !t.exp_avg || !t.exp_avg_sq))
+            return fail(B200GSR_ERR_BAD_ARG, "adam_step: tensor %d has a null pointer", i);
+    }
+    return check_cuda(gsr_launch_adam(n_tensors, tensors, GSR_ST(stream)), "adam_step");
+}
+
 int b200gsr_debug_counters(unsigned long long* device_counters) {
     g_stats = device_counters;
     return B200GSR_OK;

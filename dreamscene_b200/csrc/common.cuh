@@ -307,3 +307,66 @@ cudaError_t gsr_kth_smallest(int n, const float* v, uint32_t k, void* scratch, f
 // simple_knn replacement (knn.cu)
 size_t gsr_knn_scratch_bytes(int P, int* max_cells_out);
 cudaError_t gsr_launch_knn(int P, const float* pts, float* out, uint8_t* scratch, cudaStream_t s);
+
+// ---- Adam step (optim.cu) ----------------------------------------------------------------------
+// One launch over the virtual concatenation of up to B200GSR_ADAM_MAX_TENSORS tensors: every CTA owns
+// GSR_ADAM_CHUNK consecutive elements of one tensor and finds it from the table, which travels in the kernel
+// parameters (32 x 80 B).  A chunk is a multiple of 4 elements, so in a tensor whose four arrays are 16-byte
+// aligned every chunk starts aligned; only the tensor's last chunk can have a scalar tail.
+#define GSR_ADAM_THREADS 256
+#define GSR_ADAM_VEC 4                                               // float4 per thread
+#define GSR_ADAM_CHUNK (GSR_ADAM_THREADS * GSR_ADAM_VEC * 4)         // 4096 elements per CTA
+struct GsrAdamEntry {
+    float* p;
+    const float* g;
+    float* m;
+    float* v;
+    long long n;
+    long long block0;      // first CTA of this tensor
+    float w, beta2, omb2, eps, step_size, bc2_sqrt;
+    int vec;               // all four pointers 16-byte aligned
+};
+struct GsrAdamTable {
+    GsrAdamEntry e[B200GSR_ADAM_MAX_TENSORS];
+    int count;
+};
+
+// Fills `tab` from n <= B200GSR_ADAM_MAX_TENSORS records (empty tensors dropped) -> number of CTAs.
+inline long long gsr_adam_plan(int n, const b200gsr_adam_tensor* t, GsrAdamTable* tab) {
+    long long blocks = 0;
+    int k = 0;
+    for (int i = 0; i < n; ++i) {
+        if (t[i].n <= 0) continue;
+        GsrAdamEntry& e = tab->e[k++];
+        e.p = t[i].param; e.g = t[i].grad; e.m = t[i].exp_avg; e.v = t[i].exp_avg_sq;
+        e.n = t[i].n;
+        e.block0 = blocks;
+        e.w = t[i].lerp_weight; e.beta2 = t[i].beta2; e.omb2 = t[i].one_minus_beta2; e.eps = t[i].eps;
+        e.step_size = t[i].step_size; e.bc2_sqrt = t[i].bc2_sqrt;
+        const uintptr_t any = reinterpret_cast<uintptr_t>(e.p) | reinterpret_cast<uintptr_t>(e.g) |
+                              reinterpret_cast<uintptr_t>(e.m) | reinterpret_cast<uintptr_t>(e.v);
+        e.vec = (any & 15u) == 0;
+        blocks += (e.n + GSR_ADAM_CHUNK - 1) / GSR_ADAM_CHUNK;
+    }
+    tab->count = k;
+    return blocks;
+}
+// The entry CTA b works on (b < the plan's CTA count).
+__host__ __device__ inline int gsr_adam_find(const GsrAdamTable& tab, long long b) {
+    int t = 0;
+#pragma unroll
+    for (int k = 1; k < B200GSR_ADAM_MAX_TENSORS; ++k)
+        if (k < tab.count && b >= tab.e[k].block0) t = k;
+    return t;
+}
+// Elements [start, end) of CTA b within its entry; [start, vend) is a whole number of float4s (empty unless e.vec),
+// [vend, end) the scalar rest.
+struct GsrAdamChunk { long long start, vend, end; };
+__host__ __device__ inline GsrAdamChunk gsr_adam_chunk(const GsrAdamEntry& e, long long b) {
+    GsrAdamChunk c;
+    c.start = (b - e.block0) * GSR_ADAM_CHUNK;
+    c.end = c.start + GSR_ADAM_CHUNK < e.n ? c.start + GSR_ADAM_CHUNK : e.n;
+    c.vend = e.vec ? c.start + ((c.end - c.start) & ~3LL) : c.start;
+    return c;
+}
+cudaError_t gsr_launch_adam(int n, const b200gsr_adam_tensor* t, cudaStream_t s);

@@ -395,6 +395,31 @@ int b200gsr_split_children(int32_t n_out, int32_t first_child, float child_div, 
 int b200gsr_kth_smallest(int32_t n, const float* v, uint32_t k, void* scratch, float* out, void* stream);
 
 /*
+ * DESIGN.md §0 f6: one Adam step over up to B200GSR_ADAM_MAX_TENSORS tensors in ONE launch (additive, no upstream
+ * equivalent; dreamscene_b200.optim.GaussianAdam).  Bitwise equal to torch.optim.Adam's default (non-capturable
+ * foreach) path for amsgrad = False, weight_decay = 0, maximize = False.  Per element, every step rounded to fp32:
+ *   exp_avg    = lerp(exp_avg, grad, lerp_weight)          (lerp_weight = 1 - beta1)
+ *   exp_avg_sq = fma(one_minus_beta2, grad * grad, exp_avg_sq * beta2)
+ *   param      = fma(step_size, exp_avg / (sqrt(exp_avg_sq) / bc2_sqrt + eps), param)
+ * The scalars are the fp32 images of torch's per-tensor double expressions at the tensor's own step count t:
+ *   step_size = (lr / (1 - beta1^t)) * -1,  bc2_sqrt = (1 - beta2^t) ** 0.5.
+ * Each record holds DEVICE pointers to four dense fp32 arrays of n elements (param, exp_avg, exp_avg_sq updated in
+ * place).  Records with n = 0 are skipped.  16-byte aligned tensors take a vectorised path, others a scalar one;
+ * the results are the same.  The table is passed by value in the kernel parameters: no device allocation, no
+ * memset, no host sync.  n_tensors > B200GSR_ADAM_MAX_TENSORS returns B200GSR_ERR_UNSUPPORTED (split the call).
+ */
+#define B200GSR_ADAM_MAX_TENSORS 32
+typedef struct b200gsr_adam_tensor {
+    float* param;
+    const float* grad;
+    float* exp_avg;
+    float* exp_avg_sq;
+    int64_t n;
+    float lerp_weight, beta2, one_minus_beta2, eps, step_size, bc2_sqrt;
+} b200gsr_adam_tensor;
+int b200gsr_adam_step(int32_t n_tensors, const b200gsr_adam_tensor* tensors, void* stream);
+
+/*
  * SURVEY.md 8(f3): replaces simple_knn._C.distCUDA2 (un-vendored; /root/reference/gs_renderer.py:9,590-593):
  * out[i] = mean of the squared distances from points[i] to its 3 nearest OTHER points (points f32[P,3]).
  * `scratch` = b200gsr_dist2_scratch_bytes(P) bytes of device memory.
