@@ -91,24 +91,36 @@ DeviceState* device_state() {
     return &s;
 }
 
+// The checks the score pass shares with a full forward: the image size, and exactly one shape input per Gaussian.
+// `view` < 0 leaves the view out of the messages (single-view entry points).
+int check_size(const b200gsr_params& p, int view) {
+    if (p.P < 0 || p.image_height < 0 || p.image_width < 0)
+        return view < 0 ? fail(B200GSR_ERR_BAD_ARG, "negative size") : fail(B200GSR_ERR_BAD_ARG, "view %d: negative size", view);
+    if (p.image_height > 65535 * 16 || p.image_width > 65535 * 16)
+        return fail(B200GSR_ERR_UNSUPPORTED, "image larger than 65535 tiles per axis");
+    return B200GSR_OK;
+}
+
+int check_shape_inputs(const float* scales, const float* rots, const float* cov3d) {
+    const bool has_sr = scales != nullptr || rots != nullptr;
+    if (((scales == nullptr || rots == nullptr) && cov3d == nullptr) || (has_sr && cov3d != nullptr))
+        return fail(B200GSR_ERR_BAD_ARG, "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
+    return B200GSR_OK;
+}
+
 int validate_inputs(const b200gsr_params* p, const float* means3D, const float* shs,
                     const float* colors, const float* opac, const float* scales,
                     const float* rots, const float* cov3d) {
     if (!p) return fail(B200GSR_ERR_BAD_ARG, "params is null");
-    if (p->P < 0 || p->image_height < 0 || p->image_width < 0)
-        return fail(B200GSR_ERR_BAD_ARG, "negative size");
-    if (p->image_height > 65535 * 16 || p->image_width > 65535 * 16)
-        return fail(B200GSR_ERR_UNSUPPORTED, "image larger than 65535 tiles per axis");
+    int rc = check_size(*p, -1);
+    if (rc) return rc;
     if (!p->bg || !p->viewmatrix || !p->projmatrix || !p->campos)
         return fail(B200GSR_ERR_BAD_ARG, "bg/viewmatrix/projmatrix/campos must be device pointers");
     if (p->P > 0) {
         if (!means3D || !opac) return fail(B200GSR_ERR_BAD_ARG, "means3D/opacities are required");
         if ((shs != nullptr) == (colors != nullptr))
             return fail(B200GSR_ERR_BAD_ARG, "Please provide excatly one of either SHs or precomputed colors!");
-        const bool has_sr = scales != nullptr || rots != nullptr;
-        if (((scales == nullptr || rots == nullptr) && cov3d == nullptr) || (has_sr && cov3d != nullptr))
-            return fail(B200GSR_ERR_BAD_ARG,
-                        "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
+        if ((rc = check_shape_inputs(scales, rots, cov3d))) return rc;
         if (shs) {
             if (p->sh_degree < 0 || p->sh_degree > 3)
                 return fail(B200GSR_ERR_UNSUPPORTED, "sh_degree %d not in 0..3", p->sh_degree);
@@ -140,6 +152,138 @@ int check_det_size(int32_t H, int32_t W) {
         return fail(B200GSR_ERR_UNSUPPORTED, "deterministic mode supports at most %d 16x16 tiles per view (8192x8192); "
                     "the image is %dx%d", GSR_DET_MAX_VIEW_TILES, W, H);
     return B200GSR_OK;
+}
+
+// The three forwards differ only in their validation, in the height their layouts describe, and in the two
+// per-view / per-tile stages:
+//   kImage  b200gsr_forward: one view; the layouts describe the image itself; records the profiling events.
+//   kViews  b200gsr_forward_views: the layouts describe the stacked image (even for B = 1); no profiling events.
+//   kScore  b200gsr_score_views: stacked; geometry-only projection and score-only compositing into the caller's
+//           accumulator, which holds the deterministic sum itself, so `saved` carries no deterministic state.
+enum class Pass { kImage, kViews, kScore };
+
+// Everything a forward does after its entry point's validation, for B views stacked vertically.  Every size and
+// workspace refusal comes before device_state(), the first CUDA call.  `score` is the float [B*P] score of a
+// render, or the [P] accumulator of the score pass.
+int run_forward(Pass pass, int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, float* out_color,
+                float* out_depth_alpha, int32_t* radii, void* score, void* scratch, size_t scratch_bytes, void* saved,
+                size_t saved_bytes, uint64_t max_pairs, uint32_t flags, uint32_t* host_notify, uint32_t notify_seq,
+                void* stream) {
+    const bool score_pass = pass == Pass::kScore;
+    const int P = prm[0].P, H = prm[0].image_height, W = prm[0].image_width;
+    const GsrTileGrid g1 = gsr_grid(H, W);
+    const int Hs = pass == Pass::kImage ? H : B * g1.gy * GSR_TILE;
+    if (score_pass) flags |= B200GSR_FWD_NO_BACKWARD;
+    GsrFwdArgs a{};
+    const int with_bwd = (flags & B200GSR_FWD_NO_BACKWARD) ? 0 : 1;
+    a.det = (flags & B200GSR_FWD_DETERMINISTIC) != 0;
+    int rc;
+    if (a.det && (rc = check_det_size(H, W))) return rc;
+    if (a.det && score_pass && (long long)B * H * W > B200GSR_SCORE_DET_MAX_PIXELS)
+        return fail(B200GSR_ERR_UNSUPPORTED, "deterministic score: %d views of %dx%d exceed 2^26 pixels per accumulator", B, W, H);
+    if ((rc = b200gsr_scratch_layout_query(B * P, Hs, W, max_pairs, &a.sl))) return rc;
+    if ((rc = b200gsr_saved_layout_query(B * P, Hs, W, max_pairs, with_bwd, &a.vl))) return rc;
+    a.dl = det_layout(B * P, a.vl.total, with_bwd != 0);
+    const size_t saved_need = a.det && !score_pass ? a.dl.total : a.vl.total;
+    if (scratch_bytes < a.sl.total || saved_bytes < saved_need)
+        return fail(B200GSR_ERR_WORKSPACE, "workspace too small: scratch %zu < %zu or saved %zu < %zu",
+                    scratch_bytes, a.sl.total, saved_bytes, saved_need);
+    DeviceState* ds = device_state();
+    if (!ds) return fail(B200GSR_ERR_CUDA, "cannot query the current CUDA device");
+    a.out_color = out_color; a.out_depth_alpha = out_depth_alpha; a.radii = radii;
+    a.score = score_pass ? nullptr : static_cast<float*>(score);
+    a.scratch = static_cast<uint8_t*>(scratch); a.saved = static_cast<uint8_t*>(saved);
+    a.max_pairs = (uint32_t)max_pairs;
+    a.host_notify = host_notify; a.notify_seq = notify_seq;
+    a.flags = flags; a.num_sms = ds->num_sms; a.stats = score_pass ? nullptr : g_stats;
+    a.num_views = B; a.P_view = P; a.gy_view = g1.gy;
+    a.stream = static_cast<cudaStream_t>(stream);
+    const bool profile = pass != Pass::kViews;
+
+    // The counters at the start of scratch must be zero before the count kernel runs.  On the main path
+    // (multisplit binning, P > 0) the projection prologue zeroes them; only the large-grid fallback (the
+    // projection itself counts with global atomics) and the P == 0 case need a memset node.
+    const int ntiles = g1.gx * g1.gy * B;
+    if (!gsr_use_multisplit(ntiles) || P == 0) {
+        const size_t nbytes = gsr_counter_words(a.sl, ntiles) * sizeof(uint32_t);
+        if ((rc = check_cuda(cudaMemsetAsync(a.scratch, 0, nbytes, a.stream), "memset"))) return rc;
+    }
+    if (profile) prof_mark_fwd(0, a.stream);
+    GSR_RANGE_PUSH("b200gsr.project+count");
+    for (int v = 0; v < B && !rc; ++v) {
+        a.prm = prm[v]; a.view = v;
+        a.means3D = in[v].means3D; a.shs = in[v].shs; a.colors = in[v].colors_precomp; a.opac = in[v].opacities;
+        a.scales = in[v].scales; a.rots = in[v].rotations; a.cov3d = in[v].cov3D_precomp;
+        rc = score_pass ? check_cuda(gsr_launch_project_geo(a), "project_geo") : check_cuda(gsr_launch_project(a), "project_sh");
+    }
+    a.prm = prm[0]; a.view = 0;     // per-view constants are not used past this point (bg is indexed by tile row)
+    if (!rc) rc = check_cuda(gsr_launch_count(a), "tile_count");
+    GSR_RANGE_POP();
+    if (rc) return rc;
+    if (profile) prof_mark_fwd(1, a.stream);
+    GSR_RANGE_PUSH("b200gsr.scan_order");
+    rc = check_cuda(gsr_launch_scan(a), "scan_order");
+    GSR_RANGE_POP();
+    if (rc) return rc;
+    if (profile) prof_mark_fwd(2, a.stream);
+    GSR_RANGE_PUSH("b200gsr.scatter");
+    rc = check_cuda(gsr_launch_scatter(a), "scatter");
+    GSR_RANGE_POP();
+    if (rc) return rc;
+    if (profile) prof_mark_fwd(3, a.stream);
+    GSR_RANGE_PUSH("b200gsr.tile_sort");
+    rc = check_cuda(gsr_launch_sort(a, ds->stream, ds->fork, ds->join), "tile_sort");
+    GSR_RANGE_POP();
+    if (rc) return rc;
+    if (profile) prof_mark_fwd(4, a.stream);
+    GSR_RANGE_PUSH("b200gsr.composite");
+    rc = score_pass ? check_cuda(gsr_launch_composite_score(a, score), "composite_score")
+                    : check_cuda(gsr_launch_composite_fwd(a), "composite_fwd");
+    GSR_RANGE_POP();
+    if (rc) return rc;
+    if (profile) {
+        prof_mark_fwd(5, a.stream);
+        if (g_prof.max_calls > 0 && g_prof.nfwd < g_prof.max_calls) ++g_prof.nfwd;
+    }
+    return B200GSR_OK;
+}
+
+// The setup both backward entry points share after their validation: the saved layout of the forward (`stacked`
+// as in run_forward's kViews) and its size check, then every field of `a` but the per-view and per-range ones.
+int setup_backward(bool stacked, int32_t B, const b200gsr_params* prm, const int32_t* radii,
+                   const float* out_depth_alpha, const float* dL_dcolor, const float* dL_ddepth_alpha, void* saved,
+                   size_t saved_bytes, uint64_t max_pairs, bool det, void* stream, GsrBwdArgs& a) {
+    const int P = prm[0].P, H = prm[0].image_height, W = prm[0].image_width;
+    const GsrTileGrid g1 = gsr_grid(H, W);
+    a = GsrBwdArgs{};
+    a.det = det;
+    int rc;
+    if (a.det && (rc = check_det_size(H, W))) return rc;
+    if ((rc = b200gsr_saved_layout_query(B * P, stacked ? B * g1.gy * GSR_TILE : H, W, max_pairs, 1, &a.vl))) return rc;
+    a.dl = det_layout(B * P, a.vl.total, true);
+    const size_t saved_need = a.det ? a.dl.total : a.vl.total;
+    if (saved_bytes < saved_need)
+        return fail(B200GSR_ERR_WORKSPACE, "saved buffer too small for backward: %zu < %zu (was the forward "
+                    "run with B200GSR_FWD_NO_BACKWARD, or without B200GSR_FWD_DETERMINISTIC?)", saved_bytes, saved_need);
+    DeviceState* ds = device_state();
+    if (!ds) return fail(B200GSR_ERR_CUDA, "cannot query the current CUDA device");
+    a.prm = prm[0];
+    a.radii = radii; a.out_depth_alpha = out_depth_alpha; a.dL_dcolor = dL_dcolor; a.dL_ddepth_alpha = dL_ddepth_alpha;
+    a.saved = static_cast<uint8_t*>(saved); a.max_pairs = (uint32_t)max_pairs;
+    a.num_sms = ds->num_sms; a.stats = g_stats;
+    a.num_views = B; a.P_view = P; a.gy_view = g1.gy;
+    a.stream = static_cast<cudaStream_t>(stream);
+    return B200GSR_OK;
+}
+
+void set_view_inputs(GsrBwdArgs& a, const b200gsr_view_inputs& in) {
+    a.means3D = in.means3D; a.shs = in.shs; a.colors = in.colors_precomp; a.opac = in.opacities;
+    a.scales = in.scales; a.rots = in.rotations; a.cov3d = in.cov3D_precomp;
+}
+
+bool has_view_grads(const b200gsr_view_inputs& in, const b200gsr_view_grads& o) {
+    return o.d_means3D && o.d_means2D && o.d_opacities && (!in.shs || o.d_shs) && (!in.colors_precomp || o.d_colors) &&
+           (!in.cov3D_precomp || o.d_cov3D) && (in.cov3D_precomp || (o.d_scales && o.d_rotations));
 }
 
 }  // namespace
@@ -200,71 +344,9 @@ int b200gsr_forward(const b200gsr_params* prm, const float* means3D, const float
         return fail(B200GSR_ERR_BAD_ARG, "null output/workspace pointer");
     if (prm->score_flag && prm->P > 0 && !score)
         return fail(B200GSR_ERR_BAD_ARG, "score_flag set but score buffer is null");
-    DeviceState* ds = device_state();
-    if (!ds) return fail(B200GSR_ERR_CUDA, "cannot query the current CUDA device");
-    GsrFwdArgs a;
-    a.prm = *prm;
-    const int with_bwd = (flags & B200GSR_FWD_NO_BACKWARD) ? 0 : 1;
-    a.det = (flags & B200GSR_FWD_DETERMINISTIC) != 0;
-    if (a.det && (rc = check_det_size(prm->image_height, prm->image_width))) return rc;
-    if ((rc = b200gsr_scratch_layout_query(prm->P, prm->image_height, prm->image_width, max_pairs, &a.sl))) return rc;
-    if ((rc = b200gsr_saved_layout_query(prm->P, prm->image_height, prm->image_width, max_pairs, with_bwd, &a.vl))) return rc;
-    a.dl = det_layout(prm->P, a.vl.total, with_bwd != 0);
-    const size_t saved_need = a.det ? a.dl.total : a.vl.total;
-    if (scratch_bytes < a.sl.total || saved_bytes < saved_need)
-        return fail(B200GSR_ERR_WORKSPACE, "workspace too small: scratch %zu < %zu or saved %zu < %zu",
-                    scratch_bytes, a.sl.total, saved_bytes, saved_need);
-    a.means3D = means3D; a.shs = shs; a.colors = colors_precomp; a.opac = opacities;
-    a.scales = scales; a.rots = rotations; a.cov3d = cov3D_precomp;
-    a.out_color = out_color; a.out_depth_alpha = out_depth_alpha; a.score = score; a.radii = radii;
-    a.scratch = static_cast<uint8_t*>(scratch); a.saved = static_cast<uint8_t*>(saved);
-    a.max_pairs = (uint32_t)max_pairs;
-    a.host_notify = host_notify; a.notify_seq = notify_seq;
-    a.flags = flags; a.num_sms = ds->num_sms; a.stats = g_stats;
-    a.view = 0; a.num_views = 1; a.P_view = prm->P; a.gy_view = gsr_grid(prm->image_height, prm->image_width).gy;
-    a.stream = static_cast<cudaStream_t>(stream);
-
-    // The queue counters and the per-tile pair counters (contiguous at the start of scratch) must be
-    // zero before the count kernel runs.  On the main path (smem multisplit binning, P > 0) the
-    // project_sh prologue zeroes them; only the large-grid fallback (project_sh itself counts with
-    // global atomics) and the P == 0 case need a memset node.
-    {
-        const GsrTileGrid tg = gsr_grid(prm->image_height, prm->image_width);
-        if (!gsr_use_multisplit(tg.ntiles) || prm->P == 0) {
-            const size_t nbytes = gsr_use_multisplit(tg.ntiles) ? a.sl.tile_count + (size_t)tg.ntiles * sizeof(uint32_t)
-                                                                : a.sl.tile_cursor;
-            if ((rc = check_cuda(cudaMemsetAsync(a.scratch, 0, nbytes, a.stream), "memset"))) return rc;
-        }
-    }
-    prof_mark_fwd(0, a.stream);
-    GSR_RANGE_PUSH("b200gsr.project_sh+count");
-    rc = check_cuda(gsr_launch_project(a), "project_sh");
-    if (!rc) rc = check_cuda(gsr_launch_count(a), "tile_count");
-    GSR_RANGE_POP();
-    if (rc) return rc;
-    prof_mark_fwd(1, a.stream);
-    GSR_RANGE_PUSH("b200gsr.scan_order");
-    rc = check_cuda(gsr_launch_scan(a), "scan_order");
-    GSR_RANGE_POP();
-    if (rc) return rc;
-    prof_mark_fwd(2, a.stream);
-    GSR_RANGE_PUSH("b200gsr.scatter");
-    rc = check_cuda(gsr_launch_scatter(a), "scatter");
-    GSR_RANGE_POP();
-    if (rc) return rc;
-    prof_mark_fwd(3, a.stream);
-    GSR_RANGE_PUSH("b200gsr.tile_sort");
-    rc = check_cuda(gsr_launch_sort(a, ds->stream, ds->fork, ds->join), "tile_sort");
-    GSR_RANGE_POP();
-    if (rc) return rc;
-    prof_mark_fwd(4, a.stream);
-    GSR_RANGE_PUSH("b200gsr.composite_fwd");
-    rc = check_cuda(gsr_launch_composite_fwd(a), "composite_fwd");
-    GSR_RANGE_POP();
-    if (rc) return rc;
-    prof_mark_fwd(5, a.stream);
-    if (g_prof.max_calls > 0 && g_prof.nfwd < g_prof.max_calls) ++g_prof.nfwd;
-    return B200GSR_OK;
+    const b200gsr_view_inputs in = {means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp};
+    return run_forward(Pass::kImage, 1, prm, &in, out_color, out_depth_alpha, radii, score, scratch, scratch_bytes, saved,
+                       saved_bytes, max_pairs, flags, host_notify, notify_seq, stream);
 }
 
 int b200gsr_backward_ex(const b200gsr_params* prm, const float* means3D, const float* shs,
@@ -287,35 +369,17 @@ int b200gsr_backward_ex(const b200gsr_params* prm, const float* means3D, const f
     if (!shs && dsh_coefs < 0) return fail(B200GSR_ERR_BAD_ARG, "dsh_coefs=-1 (factored SH gradient) needs shs");
     if (!radii || !out_depth_alpha || !dL_dcolor || !dL_ddepth_alpha || !saved)
         return fail(B200GSR_ERR_BAD_ARG, "null saved-state/gradient pointer");
-    if (!d_means3D || !d_means2D || !d_opacities || (shs && !d_shs) || (colors_precomp && !d_colors) ||
-        (cov3D_precomp && !d_cov3D) || (!cov3D_precomp && (!d_scales || !d_rotations)))
-        return fail(B200GSR_ERR_BAD_ARG, "null gradient output pointer");
-    DeviceState* ds = device_state();
-    if (!ds) return fail(B200GSR_ERR_CUDA, "cannot query the current CUDA device");
+    const b200gsr_view_inputs in = {means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp};
+    const b200gsr_view_grads o = {d_means3D, d_means2D, d_shs, d_colors, d_opacities, d_scales, d_rotations, d_cov3D, 0};
+    if (!has_view_grads(in, o)) return fail(B200GSR_ERR_BAD_ARG, "null gradient output pointer");
     GsrBwdArgs a;
-    a.prm = *prm;
-    a.sl = b200gsr_scratch_layout{};
-    a.det = (stages & B200GSR_BWD_DETERMINISTIC) != 0;
-    if (a.det && (rc = check_det_size(prm->image_height, prm->image_width))) return rc;
-    if ((rc = b200gsr_saved_layout_query(prm->P, prm->image_height, prm->image_width, max_pairs, 1, &a.vl))) return rc;
-    a.dl = det_layout(prm->P, a.vl.total, true);
-    if (saved_bytes < (a.det ? a.dl.total : a.vl.total))
-        return fail(B200GSR_ERR_WORKSPACE, "saved buffer too small for backward: %zu < %zu (was the forward "
-                    "run with B200GSR_FWD_NO_BACKWARD, or without B200GSR_FWD_DETERMINISTIC?)", saved_bytes,
-                    a.det ? a.dl.total : a.vl.total);
-    a.means3D = means3D; a.shs = shs; a.colors = colors_precomp; a.opac = opacities;
-    a.scales = scales; a.rots = rotations; a.cov3d = cov3D_precomp;
-    a.radii = radii; a.out_depth_alpha = out_depth_alpha;
-    a.dL_dcolor = dL_dcolor; a.dL_ddepth_alpha = dL_ddepth_alpha;
-    a.saved = static_cast<uint8_t*>(saved); a.scratch = nullptr;
-    a.max_pairs = (uint32_t)max_pairs;
+    if ((rc = setup_backward(false, 1, prm, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes,
+                             max_pairs, (stages & B200GSR_BWD_DETERMINISTIC) != 0, stream, a)))
+        return rc;
+    set_view_inputs(a, in);
     a.d_means3D = d_means3D; a.d_means2D = d_means2D; a.d_shs = d_shs; a.d_colors = d_colors;
     a.d_opac = d_opacities; a.d_scales = d_scales; a.d_rots = d_rotations; a.d_cov3d = d_cov3D;
-    a.num_sms = ds->num_sms; a.stats = g_stats;
     a.g_begin = g_begin; a.g_end = g_end; a.dsh_coefs = dsh_coefs;
-    a.view = 0; a.num_views = 1; a.P_view = prm->P; a.gy_view = gsr_grid(prm->image_height, prm->image_width).gy;
-    a.accumulate = 0;
-    a.stream = static_cast<cudaStream_t>(stream);
 
     // no memsets: the work-queue counters and the gradient accumulators live in `saved`, zeroed by
     // the forward and restored to zero by project_bwd
@@ -392,55 +456,12 @@ int b200gsr_forward_views(int32_t B, const b200gsr_params* prm, const b200gsr_vi
                           uint32_t notify_seq, void* stream) {
     int rc = check_views(B, prm, in);
     if (rc) return rc;
-    const int P = prm[0].P, H = prm[0].image_height, W = prm[0].image_width;
+    const int P = prm[0].P;
     if (!out_color || !out_depth_alpha || (P > 0 && !radii) || !scratch || !saved)
         return fail(B200GSR_ERR_BAD_ARG, "null output/workspace pointer");
     if (prm[0].score_flag && P > 0 && !score) return fail(B200GSR_ERR_BAD_ARG, "score_flag set but score buffer is null");
-    DeviceState* ds = device_state();
-    if (!ds) return fail(B200GSR_ERR_CUDA, "cannot query the current CUDA device");
-    const GsrTileGrid g1 = gsr_grid(H, W);
-    const int Hs = B * g1.gy * GSR_TILE;
-    GsrFwdArgs a;
-    const int with_bwd = (flags & B200GSR_FWD_NO_BACKWARD) ? 0 : 1;
-    a.det = (flags & B200GSR_FWD_DETERMINISTIC) != 0;
-    if (a.det && (rc = check_det_size(H, W))) return rc;
-    if ((rc = b200gsr_scratch_layout_query(B * P, Hs, W, max_pairs, &a.sl))) return rc;
-    if ((rc = b200gsr_saved_layout_query(B * P, Hs, W, max_pairs, with_bwd, &a.vl))) return rc;
-    a.dl = det_layout(B * P, a.vl.total, with_bwd != 0);
-    const size_t saved_need = a.det ? a.dl.total : a.vl.total;
-    if (scratch_bytes < a.sl.total || saved_bytes < saved_need)
-        return fail(B200GSR_ERR_WORKSPACE, "workspace too small: scratch %zu < %zu or saved %zu < %zu",
-                    scratch_bytes, a.sl.total, saved_bytes, saved_need);
-    a.out_color = out_color; a.out_depth_alpha = out_depth_alpha; a.score = score; a.radii = radii;
-    a.scratch = static_cast<uint8_t*>(scratch); a.saved = static_cast<uint8_t*>(saved);
-    a.max_pairs = (uint32_t)max_pairs;
-    a.host_notify = host_notify; a.notify_seq = notify_seq;
-    a.flags = flags; a.num_sms = ds->num_sms; a.stats = g_stats;
-    a.num_views = B; a.P_view = P; a.gy_view = g1.gy;
-    a.stream = static_cast<cudaStream_t>(stream);
-    const int ntiles = g1.gx * g1.gy * B;
-    if (!gsr_use_multisplit(ntiles) || P == 0) {
-        const size_t nbytes = gsr_use_multisplit(ntiles) ? a.sl.tile_count + (size_t)ntiles * sizeof(uint32_t) : a.sl.tile_cursor;
-        if ((rc = check_cuda(cudaMemsetAsync(a.scratch, 0, nbytes, a.stream), "memset"))) return rc;
-    }
-    GSR_RANGE_PUSH("b200gsr.views.project_sh");
-    for (int v = 0; v < B && !rc; ++v) {
-        a.prm = prm[v]; a.view = v;
-        a.means3D = in[v].means3D; a.shs = in[v].shs; a.colors = in[v].colors_precomp; a.opac = in[v].opacities;
-        a.scales = in[v].scales; a.rots = in[v].rotations; a.cov3d = in[v].cov3D_precomp;
-        rc = check_cuda(gsr_launch_project(a), "project_sh");
-    }
-    GSR_RANGE_POP();
-    if (rc) return rc;
-    a.prm = prm[0]; a.view = 0;     // per-view constants are not used past this point (bg is indexed by tile row)
-    GSR_RANGE_PUSH("b200gsr.views.binning+sort+composite");
-    rc = check_cuda(gsr_launch_count(a), "tile_count");
-    if (!rc) rc = check_cuda(gsr_launch_scan(a), "scan_order");
-    if (!rc) rc = check_cuda(gsr_launch_scatter(a), "scatter");
-    if (!rc) rc = check_cuda(gsr_launch_sort(a, ds->stream, ds->fork, ds->join), "tile_sort");
-    if (!rc) rc = check_cuda(gsr_launch_composite_fwd(a), "composite_fwd");
-    GSR_RANGE_POP();
-    return rc;
+    return run_forward(Pass::kViews, B, prm, in, out_color, out_depth_alpha, radii, score, scratch, scratch_bytes, saved,
+                       saved_bytes, max_pairs, flags, host_notify, notify_seq, stream);
 }
 
 int b200gsr_backward_views_ex(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, const int32_t* radii,
@@ -449,30 +470,18 @@ int b200gsr_backward_views_ex(int32_t B, const b200gsr_params* prm, const b200gs
                               uint32_t flags, void* stream) {
     int rc = check_views(B, prm, in);
     if (rc) return rc;
-    const int P = prm[0].P, H = prm[0].image_height, W = prm[0].image_width;
+    const int P = prm[0].P;
     if (P == 0) return B200GSR_OK;
     if (!radii || !out_depth_alpha || !dL_dcolor || !dL_ddepth_alpha || !saved || !out)
         return fail(B200GSR_ERR_BAD_ARG, "null saved-state/gradient pointer");
-    DeviceState* ds = device_state();
-    if (!ds) return fail(B200GSR_ERR_CUDA, "cannot query the current CUDA device");
-    const GsrTileGrid g1 = gsr_grid(H, W);
-    const int Hs = B * g1.gy * GSR_TILE;
+    for (int v = 0; v < B; ++v)     // before any launch: composite_bwd consumes the work lists project_bwd needs
+        if (!has_view_grads(in[v], out[v])) return fail(B200GSR_ERR_BAD_ARG, "view %d: null gradient output pointer", v);
     GsrBwdArgs a;
-    a.sl = b200gsr_scratch_layout{};
-    a.det = (flags & B200GSR_BWD_DETERMINISTIC) != 0;
-    if (a.det && (rc = check_det_size(H, W))) return rc;
-    if ((rc = b200gsr_saved_layout_query(B * P, Hs, W, max_pairs, 1, &a.vl))) return rc;
-    a.dl = det_layout(B * P, a.vl.total, true);
-    const size_t saved_need = a.det ? a.dl.total : a.vl.total;
-    if (saved_bytes < saved_need) return fail(B200GSR_ERR_WORKSPACE, "saved buffer too small for backward: %zu < %zu", saved_bytes, saved_need);
-    a.radii = radii; a.out_depth_alpha = out_depth_alpha; a.dL_dcolor = dL_dcolor; a.dL_ddepth_alpha = dL_ddepth_alpha;
-    a.saved = static_cast<uint8_t*>(saved); a.scratch = nullptr; a.max_pairs = (uint32_t)max_pairs;
-    a.num_sms = ds->num_sms; a.stats = g_stats;
-    a.num_views = B; a.P_view = P; a.gy_view = g1.gy; a.dsh_coefs = 0; a.g_begin = 0; a.g_end = P;
-    a.stream = static_cast<cudaStream_t>(stream);
-    a.prm = prm[0]; a.view = 0; a.accumulate = 0;
-    a.means3D = in[0].means3D; a.shs = in[0].shs; a.colors = in[0].colors_precomp; a.opac = in[0].opacities;
-    a.scales = in[0].scales; a.rots = in[0].rotations; a.cov3d = in[0].cov3D_precomp;
+    if ((rc = setup_backward(true, B, prm, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes,
+                             max_pairs, (flags & B200GSR_BWD_DETERMINISTIC) != 0, stream, a)))
+        return rc;
+    set_view_inputs(a, in[0]);
+    a.g_begin = 0; a.g_end = P;
     GSR_RANGE_PUSH("b200gsr.views.composite_bwd");
     rc = check_cuda(gsr_launch_composite_bwd(a), "composite_bwd");
     GSR_RANGE_POP();
@@ -480,14 +489,8 @@ int b200gsr_backward_views_ex(int32_t B, const b200gsr_params* prm, const b200gs
     GSR_RANGE_PUSH("b200gsr.views.project_bwd");
     for (int v = 0; v < B && !rc; ++v) {
         const b200gsr_view_grads& o = out[v];
-        if (!o.d_means3D || !o.d_means2D || !o.d_opacities || (in[v].shs && !o.d_shs) || (in[v].colors_precomp && !o.d_colors) ||
-            (in[v].cov3D_precomp && !o.d_cov3D) || (!in[v].cov3D_precomp && (!o.d_scales || !o.d_rotations))) {
-            rc = fail(B200GSR_ERR_BAD_ARG, "view %d: null gradient output pointer", v);
-            break;
-        }
         a.prm = prm[v]; a.view = v; a.accumulate = (int)o.accumulate;
-        a.means3D = in[v].means3D; a.shs = in[v].shs; a.colors = in[v].colors_precomp; a.opac = in[v].opacities;
-        a.scales = in[v].scales; a.rots = in[v].rotations; a.cov3d = in[v].cov3D_precomp;
+        set_view_inputs(a, in[v]);
         a.d_means3D = o.d_means3D; a.d_means2D = o.d_means2D; a.d_shs = o.d_shs; a.d_colors = o.d_colors;
         a.d_opac = o.d_opacities; a.d_scales = o.d_scales; a.d_rots = o.d_rotations; a.d_cov3d = o.d_cov3D;
         rc = check_cuda(gsr_launch_project_bwd(a), "project_bwd");
@@ -510,9 +513,8 @@ static int check_score_views(int32_t B, const b200gsr_params* prm, const b200gsr
     if (!prm || !in) return fail(B200GSR_ERR_BAD_ARG, "null view array");
     for (int v = 0; v < B; ++v) {
         const b200gsr_params& p = prm[v];
-        if (p.P < 0 || p.image_height < 0 || p.image_width < 0) return fail(B200GSR_ERR_BAD_ARG, "view %d: negative size", v);
-        if (p.image_height > 65535 * 16 || p.image_width > 65535 * 16)
-            return fail(B200GSR_ERR_UNSUPPORTED, "image larger than 65535 tiles per axis");
+        int rc = check_size(p, v);
+        if (rc) return rc;
         if (!p.viewmatrix || !p.projmatrix || !p.campos)
             return fail(B200GSR_ERR_BAD_ARG, "view %d: viewmatrix/projmatrix/campos must be device pointers", v);
         if (p.P != prm[0].P || p.image_height != prm[0].image_height || p.image_width != prm[0].image_width)
@@ -520,10 +522,7 @@ static int check_score_views(int32_t B, const b200gsr_params* prm, const b200gsr
         if (p.P > 0) {
             const b200gsr_view_inputs& x = in[v];
             if (!x.means3D || !x.opacities) return fail(B200GSR_ERR_BAD_ARG, "view %d: means3D/opacities are required", v);
-            const bool has_sr = x.scales != nullptr || x.rotations != nullptr;
-            if (((x.scales == nullptr || x.rotations == nullptr) && x.cov3D_precomp == nullptr) || (has_sr && x.cov3D_precomp != nullptr))
-                return fail(B200GSR_ERR_BAD_ARG,
-                            "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
+            if ((rc = check_shape_inputs(x.scales, x.rotations, x.cov3D_precomp))) return rc;
         }
     }
     if ((long long)B * prm[0].P > 0x3fffffffLL) return fail(B200GSR_ERR_UNSUPPORTED, "B * P too large");
@@ -536,62 +535,9 @@ int b200gsr_score_views(int32_t B, const b200gsr_params* prm, const b200gsr_view
     int rc = check_score_views(B, prm, in);
     if (rc) return rc;
     if (flags & ~(B200GSR_FWD_NO_BACKWARD | B200GSR_FWD_DETERMINISTIC)) return fail(B200GSR_ERR_BAD_ARG, "unknown flags 0x%x", flags);
-    const int P = prm[0].P, H = prm[0].image_height, W = prm[0].image_width;
-    if ((P > 0 && !score_acc) || !scratch || !saved) return fail(B200GSR_ERR_BAD_ARG, "null accumulator/workspace pointer");
-    const GsrTileGrid g1 = gsr_grid(H, W);
-    const int Hs = B * g1.gy * GSR_TILE;
-    GsrFwdArgs a{};
-    a.det = (flags & B200GSR_FWD_DETERMINISTIC) != 0;
-    if (a.det && (rc = check_det_size(H, W))) return rc;
-    if (a.det && (long long)B * H * W > B200GSR_SCORE_DET_MAX_PIXELS)
-        return fail(B200GSR_ERR_UNSUPPORTED, "deterministic score: %d views of %dx%d exceed 2^26 pixels per accumulator", B, W, H);
-    if ((rc = b200gsr_scratch_layout_query(B * P, Hs, W, max_pairs, &a.sl))) return rc;
-    if ((rc = b200gsr_saved_layout_query(B * P, Hs, W, max_pairs, 0, &a.vl))) return rc;
-    if (scratch_bytes < a.sl.total || saved_bytes < a.vl.total)
-        return fail(B200GSR_ERR_WORKSPACE, "workspace too small: scratch %zu < %zu or saved %zu < %zu",
-                    scratch_bytes, a.sl.total, saved_bytes, a.vl.total);
-    DeviceState* ds = device_state();
-    if (!ds) return fail(B200GSR_ERR_CUDA, "cannot query the current CUDA device");
-    a.scratch = static_cast<uint8_t*>(scratch); a.saved = static_cast<uint8_t*>(saved);
-    a.max_pairs = (uint32_t)max_pairs;
-    a.host_notify = host_notify; a.notify_seq = notify_seq;
-    a.flags = flags | B200GSR_FWD_NO_BACKWARD; a.num_sms = ds->num_sms; a.stats = nullptr;
-    a.num_views = B; a.P_view = P; a.gy_view = g1.gy;
-    a.stream = static_cast<cudaStream_t>(stream);
-    const int ntiles = g1.gx * g1.gy * B;
-    if (!gsr_use_multisplit(ntiles) || P == 0) {
-        const size_t nbytes = gsr_use_multisplit(ntiles) ? a.sl.tile_count + (size_t)ntiles * sizeof(uint32_t) : a.sl.tile_cursor;
-        if ((rc = check_cuda(cudaMemsetAsync(a.scratch, 0, nbytes, a.stream), "memset"))) return rc;
-    }
-    prof_mark_fwd(0, a.stream);
-    GSR_RANGE_PUSH("b200gsr.score.project_geo");
-    for (int v = 0; v < B && !rc; ++v) {
-        a.prm = prm[v]; a.view = v;
-        a.means3D = in[v].means3D; a.opac = in[v].opacities;
-        a.scales = in[v].scales; a.rots = in[v].rotations; a.cov3d = in[v].cov3D_precomp;
-        rc = check_cuda(gsr_launch_project_geo(a), "project_geo");
-    }
-    a.prm = prm[0]; a.view = 0;
-    if (!rc) rc = check_cuda(gsr_launch_count(a), "tile_count");
-    GSR_RANGE_POP();
-    if (rc) return rc;
-    prof_mark_fwd(1, a.stream);
-    GSR_RANGE_PUSH("b200gsr.score.binning+sort");
-    rc = check_cuda(gsr_launch_scan(a), "scan_order");
-    prof_mark_fwd(2, a.stream);
-    if (!rc) rc = check_cuda(gsr_launch_scatter(a), "scatter");
-    prof_mark_fwd(3, a.stream);
-    if (!rc) rc = check_cuda(gsr_launch_sort(a, ds->stream, ds->fork, ds->join), "tile_sort");
-    GSR_RANGE_POP();
-    if (rc) return rc;
-    prof_mark_fwd(4, a.stream);
-    GSR_RANGE_PUSH("b200gsr.score.composite");
-    rc = check_cuda(gsr_launch_composite_score(a, score_acc), "composite_score");
-    GSR_RANGE_POP();
-    if (rc) return rc;
-    prof_mark_fwd(5, a.stream);
-    if (g_prof.max_calls > 0 && g_prof.nfwd < g_prof.max_calls) ++g_prof.nfwd;
-    return B200GSR_OK;
+    if ((prm[0].P > 0 && !score_acc) || !scratch || !saved) return fail(B200GSR_ERR_BAD_ARG, "null accumulator/workspace pointer");
+    return run_forward(Pass::kScore, B, prm, in, nullptr, nullptr, nullptr, score_acc, scratch, scratch_bytes, saved,
+                       saved_bytes, max_pairs, flags, host_notify, notify_seq, stream);
 }
 
 int b200gsr_score_finish(int32_t P, const void* score_acc, float* score, uint32_t flags, void* stream) {

@@ -98,6 +98,12 @@ __host__ __device__ inline int gsr_ms_blocks(long long P) {
 }
 #define GSR_MS_MAX_TILES 12288   // 4 B x tiles of dynamic smem (48 KB); 12 tiles per thread in the scan kernel
 __host__ __device__ inline bool gsr_use_multisplit(int ntiles) { return ntiles <= GSR_MS_MAX_TILES; }
+// uint32 words at the start of scratch that must be zero before the count kernel runs: the queue counters and the
+// per-tile pair counters (one array on the multisplit path, all GSR_COPIES on the large-grid fallback).  The
+// multisplit projection zeroes them in its prologue; otherwise the forward issues a memset.  Host code only.
+inline size_t gsr_counter_words(const b200gsr_scratch_layout& sl, int ntiles) {
+    return (gsr_use_multisplit(ntiles) ? sl.tile_count + (size_t)ntiles * sizeof(uint32_t) : sl.tile_cursor) / sizeof(uint32_t);
+}
 
 // ---- deterministic mode (B200GSR_FWD_DETERMINISTIC / B200GSR_BWD_DETERMINISTIC) ------------------------
 // Float atomics sum in whatever order the warps commit.  Deterministic mode commits integer images of the
@@ -226,8 +232,6 @@ struct GsrBwdArgs {
     const int32_t* radii;
     const float *out_depth_alpha, *dL_dcolor, *dL_ddepth_alpha;
     uint8_t* saved;     // counters + gradient accumulators inside are consumed and restored
-    uint8_t* scratch;   // unused (kept for layout symmetry)
-    b200gsr_scratch_layout sl;
     b200gsr_saved_layout vl;
     uint32_t max_pairs;
     float *d_means3D, *d_means2D, *d_shs, *d_colors, *d_opac, *d_scales, *d_rots, *d_cov3d;

@@ -876,8 +876,7 @@ static void launch_project_sh(const GsrFwdArgs& a, int P, size_t smem) {
     // (api.cu issues a memset instead on the large-grid fallback, where this kernel counts itself)
     GsrTileGrid tg = gsr_grid(a.prm.image_height, a.prm.image_width);
     tg.gy = a.num_views * a.gy_view; tg.ntiles = tg.gx * tg.gy;      // the stacked image
-    const int nzero = gsr_use_multisplit(tg.ntiles)
-        ? (int)((a.sl.tile_count + (size_t)tg.ntiles * sizeof(uint32_t)) / sizeof(uint32_t)) : 0;
+    const int nzero = gsr_use_multisplit(tg.ntiles) ? (int)gsr_counter_words(a.sl, tg.ntiles) : 0;
     const bool bwd = !(a.flags & B200GSR_FWD_NO_BACKWARD);
     project_sh_kernel<MT, DET><<<(P + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
         a.prm, a.means3D, a.shs, a.colors, a.opac, a.scales, a.rots, a.cov3d, a.radii,
@@ -914,8 +913,7 @@ cudaError_t gsr_launch_project_geo(const GsrFwdArgs& a) {
     if (P == 0) return cudaSuccess;
     GsrTileGrid tg = gsr_grid(a.prm.image_height, a.prm.image_width);
     tg.gy = a.num_views * a.gy_view; tg.ntiles = tg.gx * tg.gy;      // the stacked image
-    const int nzero = gsr_use_multisplit(tg.ntiles)
-        ? (int)((a.sl.tile_count + (size_t)tg.ntiles * sizeof(uint32_t)) / sizeof(uint32_t)) : 0;
+    const int nzero = gsr_use_multisplit(tg.ntiles) ? (int)gsr_counter_words(a.sl, tg.ntiles) : 0;
     project_geo_kernel<<<(P + kBlock - 1) / kBlock, kBlock, 0, a.stream>>>(
         a.prm, a.means3D, a.opac, a.scales, a.rots, a.cov3d, a.radii,
         reinterpret_cast<uint4*>(a.scratch + a.sl.rectdepth), reinterpret_cast<GsrRec*>(a.saved + a.vl.geom),

@@ -19,7 +19,6 @@ bitwise reproducible and independent of views_per_pass.  Its headroom is 2^26 pi
 from __future__ import annotations
 
 import ctypes as C
-import time
 from typing import Dict, Optional, Sequence, Tuple
 
 import torch
@@ -32,28 +31,6 @@ from . import rasterizer as R
 def _check(rc, what):
     if rc:
         raise RuntimeError(f"{what} failed ({rc}): {_lib.last_error()}")
-
-
-def _wait_pairs(d: R._Device, dev, slot: int, seq: int) -> int:
-    """Wait for one pass's tile scan to report its pair count through the notify ring; frees the slot."""
-    n = d.notify_np
-    t0 = time.perf_counter()
-    while int(n[slot, 0]) != seq:
-        if time.perf_counter() - t0 > R._POLL_TIMEOUT_S:
-            torch.cuda.synchronize(dev)
-            if int(n[slot, 0]) == seq:
-                break
-            raise RuntimeError("b200gsr_score_views: device never reported the pair count")
-    pairs = int(n[slot, 1]) & 0xFFFFFFFF
-    d.free_slots.append(slot)
-    d.last_pairs = pairs
-    return pairs
-
-
-def _note_capacity(d: R._Device, key, pairs: int) -> None:
-    if not d.user_capacity:
-        d.caps[key] = max(d.caps.get(key, 0), R._round_cap(2 * pairs))
-        d.capacity = max(d.capacity, d.caps[key])
 
 
 def view_chunks(n_views: int, views_per_pass: int):
@@ -104,8 +81,7 @@ def important_score(settings_list: Sequence[R.GaussianRasterizationSettings], me
         rotations = R._f32c(None if rotations is None else rotations.detach())
         cov3D_precomp = R._f32c(None if cov3D_precomp is None else cov3D_precomp.detach())
         d = R._device_state(dev)
-        d.ensure_notify()
-        R._resolve_pending(d)                  # non-blocking overflow check of earlier forwards, as every forward does
+        d.resolve()                            # non-blocking overflow check of earlier forwards, as every forward does
         stream_h = torch.cuda.current_stream(dev).cuda_stream
         stream = C.c_void_p(stream_h)
         acc = torch.zeros(P, dtype=torch.int64 if det else torch.float32, device=dev)
@@ -130,38 +106,35 @@ def important_score(settings_list: Sequence[R.GaussianRasterizationSettings], me
             scratch_bytes, saved_bytes = R._layouts(B * P, int(hs.value), W, cap, False)
             scratch = d.ensure_scratch(stream_h, scratch_bytes)
             saved = torch.empty(saved_bytes, dtype=torch.uint8, device=dev)
-            if not d.free_slots:
-                R._resolve_pending(d, block=True)
-            slot, seq = d.free_slots.pop(), d.next_seq()
+            slot, seq, notify_ptr = d.claim()
             rc = lib.b200gsr_score_views(B, prm, vin, C.c_void_p(acc.data_ptr()), C.c_void_p(scratch.data_ptr()),
                                          scratch.numel(), C.c_void_p(saved.data_ptr()), saved.numel(), cap, flags,
-                                         C.c_void_p(d.notify.data_ptr() + 16 * slot), seq, stream)
+                                         notify_ptr, seq, stream)
             if rc:
-                d.free_slots.append(slot)
+                d.release(slot)
                 raise RuntimeError(f"b200gsr_score_views failed ({rc}): {_lib.last_error()}")
             return slot, seq
 
-        def capacity(key, B):
-            measured = d.capacity if d.user_capacity else d.caps.get(key, 0)
-            if measured > 0:
-                return R._round_cap(max(measured, R._MIN_PAIRS_PER_GAUSSIAN * B * P)), True
-            return R._round_cap(6 * B * P), False
+        def settle(items):
+            # A pass that overflowed added nothing to `acc`: it is re-issued as it is, without zeroing anything.
+            for b0, b1, key, cap, slot, seq in items:
+                d.settle(key, cap, slot, seq, lambda c, b0=b0, b1=b1: issue(b0, b1, c))
 
         # Every pass is issued without waiting once its shape's capacity is known; the pair counts are read after
         # the last pass is enqueued, and only passes that overflowed (and so added nothing) are issued again.
         pending = []
         for b0, b1 in view_chunks(n_views, views_per_pass):
             key = (b1 - b0, P, H, W)
-            cap, known = capacity(key, b1 - b0)
+            cap, known = d.capacity_for(key, (b1 - b0) * P, False)
             item = (b0, b1, key, cap) + issue(b0, b1, cap)
             if known:
                 pending.append(item)
                 if len(pending) >= 64:              # bound the notify slots held by this call
-                    _settle(d, dev, issue, pending)
+                    settle(pending)
                     pending = []
             else:
-                _settle(d, dev, issue, [item])      # a shape seen for the first time: learn its capacity now
-        _settle(d, dev, issue, pending)
+                settle([item])                      # a shape seen for the first time: learn its capacity now
+        settle(pending)
 
         if not det:
             return acc
@@ -169,19 +142,6 @@ def important_score(settings_list: Sequence[R.GaussianRasterizationSettings], me
         _check(lib.b200gsr_score_finish(P, C.c_void_p(acc.data_ptr()), C.c_void_p(score.data_ptr()),
                                         _lib.FWD_DETERMINISTIC, stream), "b200gsr_score_finish")
         return score
-
-
-def _settle(d, dev, issue, pending):
-    """Read the pair count of every pending pass; re-issue (and wait for) each one that overflowed, with room
-    for its measured count, until it fits."""
-    for b0, b1, key, cap, slot, seq in pending:
-        pairs = _wait_pairs(d, dev, slot, seq)
-        while pairs > cap:
-            cap = R._round_cap(2 * pairs)
-            d.capacity = max(d.capacity, cap)
-            slot, seq = issue(b0, b1, cap)
-            pairs = _wait_pairs(d, dev, slot, seq)
-        _note_capacity(d, key, pairs)
 
 
 def _kth_smallest(v: torch.Tensor, k: int) -> torch.Tensor:

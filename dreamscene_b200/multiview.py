@@ -59,9 +59,9 @@ class _RasterizeViews(torch.autograd.Function):
         score_flag = bool(settings[0].score_flag)
         with_backward = any(ctx.needs_input_grad)
         d = R._device_state(dev)
-        if not torch.cuda.is_current_stream_capturing():
-            d.ensure_notify()
-            R._resolve_pending(d)
+        capturing = torch.cuda.is_current_stream_capturing()
+        if not capturing:
+            d.resolve()
         keep: list = []
         with torch.cuda.device(dev):
             hs = C.c_int32(0)
@@ -83,7 +83,8 @@ class _RasterizeViews(torch.autograd.Function):
             depth_alpha = torch.empty(2, Hs, W, dtype=torch.float32, device=dev)
             radii = torch.empty(B, P, dtype=torch.int32, device=dev)
             score = torch.zeros(B, P, dtype=torch.float32, device=dev) if score_flag else None
-            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            stream_h = torch.cuda.current_stream(dev).cuda_stream
+            stream = C.c_void_p(stream_h)
             det = R.deterministic_mode()
             flags = (0 if with_backward else _lib.FWD_NO_BACKWARD) | (_lib.FWD_DETERMINISTIC if det else 0)
 
@@ -93,8 +94,10 @@ class _RasterizeViews(torch.autograd.Function):
                                                  C.c_void_p(scratch.data_ptr()), scratch.numel(), C.c_void_p(saved.data_ptr()),
                                                  saved.numel(), cap, flags, notify_ptr, seq, stream)
 
-            saved, cap = R._issue_with_capacity(d, dev, (B, P, H, W), B * P, Hs, W, with_backward, score, launch, det)
-        ctx.meta = (settings, spec, B, P, M, H, W, Hs, cap, with_backward, len(flat), det)
+            saved, cap = R._issue_with_capacity(d, (B, P, H, W), B * P, Hs, W, with_backward, det, score, launch, capturing,
+                                                stream_h)
+        ctx.meta = (spec, B, P, W, Hs, cap, with_backward, len(flat), det)
+        ctx.views = (prm, vin)            # the backward reuses the arrays; `keep` holds their device constants
         ctx.keep = keep
         ctx.saved_buf = saved
         ctx.save_for_backward(radii, depth_alpha, *tensors)
@@ -107,7 +110,8 @@ class _RasterizeViews(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_color, _g_radii, g_da, *_):
-        settings, spec, B, P, M, H, W, Hs, cap, with_backward, nflat, det = ctx.meta
+        spec, B, P, W, Hs, cap, with_backward, nflat, det = ctx.meta
+        prm, vin = ctx.views
         radii, depth_alpha = ctx.saved_tensors[:2]
         tensors = list(ctx.saved_tensors[2:])
         dev = radii.device
@@ -120,21 +124,11 @@ class _RasterizeViews(torch.autograd.Function):
         grads: List[Optional[torch.Tensor]] = [None] * nflat
         m2d_base = nflat - B
         with torch.cuda.device(dev):
-            bg_all = ctx.keep[0]
-            prm = (_lib.Params * B)()
-            vin = (_lib.ViewInputs * B)()
             out = (_lib.ViewGrads * B)()
-            k = 1
-            for v, s in enumerate(settings):
-                vm, pm, cp = ctx.keep[k], ctx.keep[k + 1], ctx.keep[k + 2]
-                k += 3
-                prm[v] = _lib.Params(P, M, int(s.sh_degree), H, W, float(s.tanfovx), float(s.tanfovy), float(s.scale_modifier),
-                                     int(bool(s.prefiltered)), int(bool(s.score_flag)), bg_all.data_ptr() + 12 * v, vm.data_ptr(),
-                                     pm.data_ptr(), cp.data_ptr())
+            for v in range(B):
                 acc = 0
                 for name in _NAMES:
                     t = get(name, v)
-                    setattr(vin[v], name, _ptr(t))
                     if t is None:
                         continue
                     idx = spec[name][1] if spec[name][0] == "shared" else spec[name][1][v]

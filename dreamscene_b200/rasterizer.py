@@ -85,9 +85,103 @@ class _Device:
             t = self.scratch[stream] = torch.empty(int(nbytes * 1.1) + 4096, dtype=torch.uint8, device=self.device)
         return t
 
-    def next_seq(self) -> int:
+    # ---- the pair-capacity protocol, shared by every forward flavour.  The key buffer is sized before the device
+    # knows the pair count D; each forward reports D through a slot of the notify ring, and a forward whose D
+    # exceeded its capacity has to be re-issued (synchronously) or reported (asynchronously).  Module globals
+    # (_round_cap, _MIN_PAIRS_PER_GAUSSIAN, ...) are looked up at call time.
+    def capacity_for(self, key, n_gaussians: int, capturing: bool):
+        """-> (capacity, known) for a forward of n_gaussians (virtual) Gaussians with shape `key`: the user's
+        capacity or the shape's measured one, at least _MIN_PAIRS_PER_GAUSSIAN pairs per Gaussian; a blind 6 n guess
+        when nothing is known.  A capture cannot wait, so it trusts the device's high-water mark."""
+        measured = self.capacity if self.user_capacity else self.caps.get(key, 0)
+        known = measured > 0
+        if capturing and not known and self.capacity > 0:
+            known, measured = True, self.capacity
+        if capturing and not known:
+            raise RuntimeError("b200gsr: capturing into a CUDA graph needs a known pair capacity: run one eager "
+                               "forward on this device first or call set_workspace_capacity()")
+        if known:
+            return _round_cap(max(measured, _MIN_PAIRS_PER_GAUSSIAN * n_gaussians)), True
+        return _round_cap(6 * n_gaussians), False
+
+    def claim(self):
+        """-> (slot, seq, device-mapped pointer to the slot) for one forward's report; waits for the pending
+        forwards only when the ring is full."""
+        self.ensure_notify()
+        if not self.free_slots:
+            self.resolve(block=True)
+        slot = self.free_slots.pop()
         self.seq = (self.seq + 1) & 0x7FFFFFFF or 1
-        return self.seq
+        return slot, self.seq, C.c_void_p(self.notify.data_ptr() + 16 * slot)
+
+    def release(self, slot: int) -> None:
+        self.free_slots.append(slot)
+
+    def reported(self, slot: int, seq: int) -> bool:
+        return int(self.notify_np[slot, 0]) == seq
+
+    def wait(self, slot: int, seq: int) -> int:
+        """Wait for the forward of (slot, seq) to report its pair count (only its tile scan has to run; the later
+        kernels keep running); frees the slot.  -> the pair count."""
+        t0 = time.perf_counter()
+        while not self.reported(slot, seq):
+            if time.perf_counter() - t0 > _POLL_TIMEOUT_S:
+                torch.cuda.synchronize(self.device)
+                if not self.reported(slot, seq):
+                    raise RuntimeError("b200gsr: device never reported a pair count")
+        pairs = int(self.notify_np[slot, 1]) & 0xFFFFFFFF
+        self.release(slot)
+        self.last_pairs = pairs
+        return pairs
+
+    def note(self, key, pairs: int) -> None:
+        """Record a shape's measured pair count: a high-water mark with 2x head-room (capacity only costs 8 B per
+        pair in `saved`, and the views of a training step differ a lot in pair count).  A user capacity is trusted
+        as it is."""
+        if self.user_capacity:
+            return
+        self.caps[key] = max(self.caps.get(key, 0), _round_cap(2 * pairs))
+        self.capacity = max(self.capacity, self.caps[key])
+        if len(self.caps) > 64:                 # densification changes P every 100 steps: keep the table small
+            for k in list(self.caps)[:-32]:
+                del self.caps[k]
+
+    def grow(self, pairs: int) -> int:
+        """-> the capacity a forward of `pairs` pairs is re-issued with; raises the device's high-water mark."""
+        cap = _round_cap(2 * pairs)
+        self.capacity = max(self.capacity, cap)
+        return cap
+
+    def settle(self, key, cap: int, slot: int, seq: int, reissue) -> int:
+        """Wait for a forward's pair count; while it exceeded `cap`, re-issue it with room for the count
+        (`reissue(cap) -> (slot, seq)`) and wait again.  -> the capacity it ran with."""
+        pairs = self.wait(slot, seq)
+        while pairs > cap:
+            cap = self.grow(pairs)
+            slot, seq = reissue(cap)
+            pairs = self.wait(slot, seq)
+        self.note(key, pairs)
+        return cap
+
+    def resolve(self, block: bool = False) -> None:
+        """Read the pair counts of the forwards issued without waiting (all of them if `block`, else those
+        already reported).  Raises PairCapacityOverflow if one of them overflowed."""
+        still, overflow = [], None
+        for slot, seq, cap, key in self.pending:
+            if not block and not self.reported(slot, seq):
+                still.append((slot, seq, cap, key))
+                continue
+            pairs = self.wait(slot, seq)
+            self.grow(pairs)
+            self.note(key, pairs)
+            if pairs > cap:
+                overflow = (pairs, cap)
+        self.pending = still
+        if overflow is not None:
+            raise PairCapacityOverflow(
+                f"b200gsr: an earlier forward produced {overflow[0]} (tile, Gaussian) pairs but its key buffer held "
+                f"{overflow[1]}; its images/gradients are invalid. The capacity has been raised to {self.capacity}; "
+                "re-run the step, or call set_workspace_capacity()/set_pair_count_mode('sync').")
 
 
 _devices: dict = {}
@@ -138,34 +232,7 @@ def _round_cap(n: int) -> int:
 
 def _resolve_pending(d: _Device, block: bool = False) -> None:
     """Read the pair counts the device has reported so far (never waits unless `block`)."""
-    if not d.pending:
-        return
-    n = d.notify_np
-    still, overflow = [], None
-    t0 = time.perf_counter()
-    for slot, seq, cap, key in d.pending:
-        while block and int(n[slot, 0]) != seq:
-            if time.perf_counter() - t0 > _POLL_TIMEOUT_S:
-                torch.cuda.synchronize(d.device)
-                if int(n[slot, 0]) != seq:
-                    raise RuntimeError("b200gsr: device never reported a pair count")
-        if int(n[slot, 0]) != seq:
-            still.append((slot, seq, cap, key))
-            continue
-        pairs = int(n[slot, 1]) & 0xFFFFFFFF
-        d.free_slots.append(slot)
-        d.last_pairs = pairs
-        d.capacity = max(d.capacity, _round_cap(2 * pairs))
-        if key is not None and not d.user_capacity:
-            d.caps[key] = max(d.caps.get(key, 0), _round_cap(2 * pairs))
-        if pairs > cap:
-            overflow = (pairs, cap)
-    d.pending = still
-    if overflow is not None:
-        raise PairCapacityOverflow(
-            f"b200gsr: an earlier forward produced {overflow[0]} (tile, Gaussian) pairs but its key buffer held "
-            f"{overflow[1]}; its images/gradients are invalid. The capacity has been raised to {d.capacity}; "
-            "re-run the step, or call set_workspace_capacity()/set_pair_count_mode('sync').")
+    d.resolve(block)
 
 
 def flush_checks(device=None) -> None:
@@ -245,74 +312,45 @@ def deterministic_mode() -> bool:
     return torch.are_deterministic_algorithms_enabled()
 
 
-def _issue_with_capacity(d: _Device, dev, key, P_eff: int, H_eff: int, W: int, with_backward: bool, score, launch,
-                         deterministic: bool = False):
-    """The pair-capacity protocol shared by the single- and multi-view forwards.  `launch(cap, scratch,
-    saved, notify_ptr, seq)` enqueues the whole forward and returns the C return code; this helper
-    sizes the buffers, decides whether to wait for the device's pair count (sync mode / unknown
-    capacity) and re-issues on overflow.  -> (saved tensor, capacity)."""
-    capturing = torch.cuda.is_current_stream_capturing()
-    stream_h = torch.cuda.current_stream(dev).cuda_stream
-    measured = d.capacity if d.user_capacity else d.caps.get(key, 0)
-    known = measured > 0
-    if capturing and not known and d.capacity > 0:
-        known, measured = True, d.capacity      # cannot wait inside a capture: trust the device's high-water mark
-    if capturing and not known:
-        raise RuntimeError("b200gsr: capturing into a CUDA graph needs a known pair capacity: run one eager "
-                           "forward on this device first or call set_workspace_capacity()")
-    cap = _round_cap(max(measured, _MIN_PAIRS_PER_GAUSSIAN * P_eff)) if known else _round_cap(6 * P_eff)
-    # wait for the count only when it is needed: sync mode, or the capacity is a blind first guess
-    wait = (not capturing) and (_pair_mode == "sync" or not known)
-    while True:
+def _issue_with_capacity(d: _Device, key, P_eff: int, H_eff: int, W: int, with_backward: bool, deterministic: bool,
+                         score, launch, capturing: bool, stream_h: int):
+    """The single- and multi-view forwards' side of the pair-capacity protocol.  `launch(cap, scratch, saved,
+    notify_ptr, seq)` enqueues the whole forward and returns the C return code; this helper sizes the buffers,
+    decides whether to wait for the device's pair count (sync mode / unknown capacity) and re-issues on overflow,
+    with `score` zeroed.  `capturing` and `stream_h` (the current stream's handle) come from the caller.
+    -> (saved tensor, capacity)."""
+    cap, known = d.capacity_for(key, P_eff, capturing)
+    saved = None
+
+    def issue(cap):
+        nonlocal saved
         scratch_bytes, saved_bytes = _layouts(P_eff, H_eff, W, cap, with_backward, deterministic)
         scratch = d.ensure_scratch(stream_h, scratch_bytes)
-        saved = torch.empty(saved_bytes, dtype=torch.uint8, device=dev)
-        slot, seq, notify_ptr = -1, 0, None
-        if not capturing:
-            if not d.free_slots:
-                _resolve_pending(d, block=True)
-            slot, seq = d.free_slots.pop(), d.next_seq()
-            notify_ptr = C.c_void_p(d.notify.data_ptr() + 16 * slot)
+        saved = torch.empty(saved_bytes, dtype=torch.uint8, device=d.device)
+        slot, seq, notify_ptr = d.claim() if not capturing else (-1, 0, None)
         rc = launch(cap, scratch, saved, notify_ptr, seq)
         if rc:
             if slot >= 0:
-                d.free_slots.append(slot)
+                d.release(slot)
             msg = _lib.last_error()
             if rc == -1:
                 raise Exception(msg)
             raise RuntimeError(f"b200gsr_forward failed ({rc}): {msg}")
-        if capturing:
-            break
-        if not wait:
-            d.pending.append((slot, seq, cap, key))  # resolved lazily, never blocks the host
-            break
-        # Wait only for the tile scan (project + count + scan kernels); sort/composite keep running.
-        t0 = time.perf_counter()
-        n = d.notify_np
-        while int(n[slot, 0]) != seq:
-            if time.perf_counter() - t0 > _POLL_TIMEOUT_S:
-                torch.cuda.synchronize(dev)
-                if int(n[slot, 0]) == seq:
-                    break
-                raise RuntimeError("b200gsr_forward: device never reported the pair count")
-        pairs = int(n[slot, 1]) & 0xFFFFFFFF
-        d.free_slots.append(slot)
-        d.last_pairs = pairs
-        if pairs <= cap:
-            # high-water mark with 2x head-room: capacity only costs 8 B per pair in `saved`, and
-            # views of one training step differ a lot in pair count (random cameras).  A new
-            # shape starts its own high-water mark.
-            if not d.user_capacity:
-                d.caps[key] = max(d.caps.get(key, 0), _round_cap(2 * pairs))
-                d.capacity = max(d.capacity, d.caps[key])
-                if len(d.caps) > 64:                 # densification changes P every 100 steps: keep the table small
-                    for k in list(d.caps)[:-32]:
-                        del d.caps[k]
-            break
-        cap = _round_cap(2 * pairs)                  # overflow: re-issue with enough room
-        d.capacity = max(d.capacity, cap)
+        return slot, seq
+
+    def reissue(cap):
         if score is not None:
             score.zero_()
+        return issue(cap)
+
+    slot, seq = issue(cap)
+    if capturing:
+        return saved, cap
+    # wait for the count only when it is needed: sync mode, or the capacity is a blind first guess
+    if _pair_mode != "sync" and known:
+        d.pending.append((slot, seq, cap, key))      # resolved lazily, never blocks the host
+        return saved, cap
+    cap = d.settle(key, cap, slot, seq, reissue)     # `saved` is the buffer of the issue that fitted
     return saved, cap
 
 
@@ -326,9 +364,9 @@ def _forward_impl(rs, means3D, shs, colors, opac, scales, rots, cov3d, with_back
     M = int(shs.shape[1]) if shs is not None else 0
     H, W = int(rs.image_height), int(rs.image_width)
     d = _device_state(dev)
-    if not torch.cuda.is_current_stream_capturing():
-        d.ensure_notify()
-        _resolve_pending(d)               # non-blocking: may raise PairCapacityOverflow for an earlier call
+    capturing = torch.cuda.is_current_stream_capturing()
+    if not capturing:
+        d.resolve()                       # non-blocking: may raise PairCapacityOverflow for an earlier call
     keep: list = []
     with torch.cuda.device(dev):          # the library launches on the CURRENT device; restored on exit
         prm = _make_params(rs, P, M, keep, dev)
@@ -336,7 +374,8 @@ def _forward_impl(rs, means3D, shs, colors, opac, scales, rots, cov3d, with_back
         depth_alpha = torch.empty(2, H, W, dtype=torch.float32, device=dev)
         radii = torch.empty(P, dtype=torch.int32, device=dev)
         score = torch.zeros(P, dtype=torch.float32, device=dev) if rs.score_flag else None
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        stream_h = torch.cuda.current_stream(dev).cuda_stream
+        stream = C.c_void_p(stream_h)
         det = deterministic_mode()
         flags = (0 if with_backward else _lib.FWD_NO_BACKWARD) | (_lib.FWD_DETERMINISTIC if det else 0)
 
@@ -346,7 +385,7 @@ def _forward_impl(rs, means3D, shs, colors, opac, scales, rots, cov3d, with_back
                                        _ptr(radii), _ptr(score), _ptr(scratch), scratch.numel(), _ptr(saved),
                                        saved.numel(), cap, flags, notify_ptr, seq, stream)
 
-        saved, cap = _issue_with_capacity(d, dev, (P, H, W), P, H, W, with_backward, score, launch, det)
+        saved, cap = _issue_with_capacity(d, (P, H, W), P, H, W, with_backward, det, score, launch, capturing, stream_h)
     st = _State()
     st.params_keep = keep; st.P = P; st.M = M; st.capacity = cap; st.saved = saved; st.rs = rs
     st.with_backward = with_backward

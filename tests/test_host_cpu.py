@@ -130,6 +130,117 @@ def test_deferred_overflow_check_reads_the_notify_ring_without_blocking():
     assert not d.pending and d.capacity >= 6 << 20      # raised so that a retry fits
 
 
+def _fake_device():
+    """A _Device on the CPU with an unpinned notify ring, and a fake `launch` that reports a pair count into it the
+    way the tile scan does: (seq, pairs) into the slot its notify pointer names."""
+    from dreamscene_b200 import rasterizer as R
+    d = R._Device(torch.device("cpu"))
+    d.ensure_notify = lambda: None
+    d.notify = torch.zeros(R._NOTIFY_SLOTS, 4, dtype=torch.int32)
+    d.notify_np = d.notify.numpy()
+    d.free_slots = list(range(R._NOTIFY_SLOTS - 1, -1, -1))
+    calls = []
+
+    def launch_with(pairs):
+        def launch(cap, scratch, saved, notify_ptr, seq):
+            calls.append((cap, saved.numel()))
+            if notify_ptr is not None:
+                d.notify_np[(notify_ptr.value - d.notify.data_ptr()) // 16, :2] = (seq, pairs)
+            return 0
+        return launch
+    return d, calls, launch_with
+
+
+def test_sync_overflow_reissues_with_room_for_the_count_and_zeroes_the_score():
+    from dreamscene_b200 import _lib, rasterizer as R
+    d, calls, launch_with = _fake_device()
+    d.capacity, d.user_capacity = 1 << 20, True
+    score = torch.ones(8)
+    pairs = 3 << 20
+    old = R._pair_mode
+    R.set_pair_count_mode("sync")
+    try:
+        saved, cap = R._issue_with_capacity(d, (8, 64, 64), 8, 64, 64, True, False, score, launch_with(pairs), False, 0)
+        assert [c for c, _ in calls] == [R._round_cap(1 << 20), R._round_cap(2 * pairs)]
+        assert cap == R._round_cap(2 * pairs) and saved.numel() == _lib.saved_layout(8, 64, 64, cap).total
+        assert torch.equal(score, torch.zeros(8))              # the overflowed issue's partial score is dropped
+        assert d.capacity == cap and d.caps == {} and d.last_pairs == pairs and not d.pending
+        assert len(d.free_slots) == R._NOTIFY_SLOTS            # both slots were released
+        # a synchronous success under a user capacity leaves the capacity and the shape table as they are
+        calls.clear()
+        R._issue_with_capacity(d, (8, 64, 64), 8, 64, 64, True, False, score, launch_with(1000), False, 0)
+        assert len(calls) == 1 and d.capacity == cap and d.caps == {} and d.last_pairs == 1000
+    finally:
+        R.set_pair_count_mode(old)
+
+
+def test_first_forward_of_a_shape_is_measured_then_later_ones_are_deferred():
+    from dreamscene_b200 import rasterizer as R
+    d, calls, launch_with = _fake_device()
+    key = (100, 64, 64)
+    _, cap = R._issue_with_capacity(d, key, 100, 64, 64, False, False, None, launch_with(5000), False, 0)
+    assert cap == R._round_cap(600) and d.caps[key] == R._round_cap(10_000) and not d.pending
+    _, cap2 = R._issue_with_capacity(d, key, 100, 64, 64, False, False, None, launch_with(6000), False, 0)
+    assert cap2 == d.caps[key] and [p[2:] for p in d.pending] == [(cap2, key)]   # async: not waited for
+    d.resolve()
+    assert not d.pending and d.last_pairs == 6000
+    with pytest.raises(RuntimeError, match="CUDA graph"):      # a capture cannot measure an unknown shape
+        R._issue_with_capacity(R._Device(torch.device("cpu")), key, 100, 64, 64, False, False, None, launch_with(1),
+                               True, 0)
+
+
+def test_score_pass_settle_reissues_without_touching_the_accumulator():
+    """The score pass adds into an accumulator that holds the earlier passes' sums; an overflowed pass adds nothing,
+    so settling re-issues it as it is."""
+    from dreamscene_b200 import rasterizer as R
+    d, calls, launch_with = _fake_device()
+    d.capacity, d.user_capacity = 1 << 20, True
+    key = (4, 100, 64, 64)
+    cap, known = d.capacity_for(key, 400, False)
+    assert known and cap == R._round_cap(1 << 20)
+    acc = torch.full((4,), 7.0)
+    pairs = 5 << 20
+    launch = launch_with(pairs)
+
+    def issue(c):
+        slot, seq, ptr = d.claim()
+        launch(c, torch.empty(0), torch.empty(0), ptr, seq)
+        return slot, seq
+
+    slot, seq = issue(cap)
+    got = d.settle(key, cap, slot, seq, issue)
+    assert got == R._round_cap(2 * pairs) and [c for c, _ in calls] == [cap, got]
+    assert torch.equal(acc, torch.full((4,), 7.0)) and d.capacity == got and d.caps == {}
+
+
+def test_claim_on_a_full_ring_waits_for_the_pending_forwards():
+    from dreamscene_b200 import rasterizer as R
+    d, _, _ = _fake_device()
+    held = [d.claim() for _ in range(R._NOTIFY_SLOTS)]
+    assert not d.free_slots
+    for slot, seq, _ in held:
+        d.notify_np[slot, :2] = (seq, 10)
+        d.pending.append((slot, seq, 1 << 20, (1, 16, 16)))
+    slot, seq, ptr = d.claim()
+    assert not d.pending and len(d.free_slots) == R._NOTIFY_SLOTS - 1
+    assert ptr.value == d.notify.data_ptr() + 16 * slot and seq == held[-1][1] + 1
+
+
+def test_shape_table_keeps_the_32_newest_shapes_once_it_exceeds_64():
+    from dreamscene_b200 import rasterizer as R
+    d, _, _ = _fake_device()
+    for P in range(64):
+        d.note((P, 16, 16), 1000)
+    assert len(d.caps) == 64
+    d.note((64, 16, 16), 1000)
+    assert list(d.caps) == [(P, 16, 16) for P in range(33, 65)]
+    d.pending = [(0, 5, 1 << 20, (65, 16, 16))]                # a deferred count records its shape the same way
+    d.notify_np[0, :2] = (5, 1000)
+    d.free_slots.remove(0)
+    d.resolve()
+    assert len(d.caps) == 33 and d.caps[(65, 16, 16)] == R._round_cap(2000)
+
+
 def test_shared_inline_helpers_native_check(tmp_path):
     """common.cuh helpers used by both host and device code (multisplit grid, backward size classes, tile grid):
     tests/native/common_check.cu is compiled with nvcc and run on the CPU."""
