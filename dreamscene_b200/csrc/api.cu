@@ -214,7 +214,7 @@ int run_forward(Pass pass, int32_t B, const b200gsr_params* prm, const b200gsr_v
         a.prm = prm[v]; a.view = v;
         a.means3D = in[v].means3D; a.shs = in[v].shs; a.colors = in[v].colors_precomp; a.opac = in[v].opacities;
         a.scales = in[v].scales; a.rots = in[v].rotations; a.cov3d = in[v].cov3D_precomp;
-        rc = score_pass ? check_cuda(gsr_launch_project_geo(a), "project_geo") : check_cuda(gsr_launch_project(a), "project_sh");
+        rc = check_cuda(gsr_launch_project(a, score_pass), score_pass ? "project_geo" : "project_sh");
     }
     a.prm = prm[0]; a.view = 0;     // per-view constants are not used past this point (bg is indexed by tile row)
     if (!rc) rc = check_cuda(gsr_launch_count(a), "tile_count");

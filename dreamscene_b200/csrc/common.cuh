@@ -260,16 +260,16 @@ inline cudaError_t gsr_smem_once(F func, int bytes, std::atomic<unsigned long lo
     return e;
 }
 
-cudaError_t gsr_launch_project(const GsrFwdArgs& a);
+// geo: the score pass's geometry-only projection (no SH row or colour read, no backward state)
+cudaError_t gsr_launch_project(const GsrFwdArgs& a, bool geo);
 cudaError_t gsr_launch_count(const GsrFwdArgs& a);         // multisplit path: per-tile pair counts
 cudaError_t gsr_launch_scan(const GsrFwdArgs& a);          // exclusive scan + work order + host notify
 cudaError_t gsr_launch_scatter(const GsrFwdArgs& a);       // append keys to tile lists
 cudaError_t gsr_launch_sort(const GsrFwdArgs& a, cudaStream_t side, cudaEvent_t fork, cudaEvent_t join);   // per-tile sort (2 kernels, concurrent when `side` is given)
 cudaError_t gsr_launch_composite_fwd(const GsrFwdArgs& a);
 cudaError_t gsr_launch_composite_bwd(const GsrBwdArgs& a);
-// score pass (b200gsr_score_views): geometry-only projection and score-only compositing into score_acc
-// (float [P_view], or int64 [P_view] with a.det); score_finish converts an int64 accumulator to float
-cudaError_t gsr_launch_project_geo(const GsrFwdArgs& a);
+// score pass (b200gsr_score_views): score-only compositing into score_acc (float [P_view], or int64 [P_view] with
+// a.det); score_finish converts an int64 accumulator to float
 cudaError_t gsr_launch_composite_score(const GsrFwdArgs& a, void* score_acc);
 cudaError_t gsr_launch_score_finish(int n, const unsigned long long* score_fx, float* score, cudaStream_t s);
 cudaError_t gsr_launch_project_bwd(const GsrBwdArgs& a);

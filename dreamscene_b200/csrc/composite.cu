@@ -139,7 +139,11 @@ struct __align__(128) SmemCta {
 // state stays in PPL-element arrays: written as scalars, the kernel compiles to different code from the measured one.
 // DET (deterministic mode, with SCORE): `score` points to the int64 fixed-point accumulators (GsrDetLayout::score_fx)
 // and each warp's weight sum is committed as an integer (gsr_det_score_quantise).
-template <bool SCORE, bool STATS, bool DET = false>
+// SCORE_ONLY (with SCORE; the score pass, b200gsr_score_views): the same tile loop, cull, blending test, T recurrence
+// and early-outs, but no image, n_contrib or backward work list is written.  Every view of the stacked pass adds into
+// ONE accumulator of P_view rows: entry idx of view v commits to row idx - v * P_view.  A pass that overflowed its pair
+// capacity commits nothing, so re-issuing it with a larger capacity adds exactly what one complete pass adds.
+template <bool SCORE, bool STATS, bool DET = false, bool SCORE_ONLY = false>
 __global__ void __launch_bounds__(256)
 composite_fwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, const uint32_t* __restrict__ header,
                      const uint32_t* __restrict__ work_order,
@@ -148,7 +152,7 @@ composite_fwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, cons
                      const float* __restrict__ bg, uint32_t* __restrict__ queue,
                      float* __restrict__ out_color, float* __restrict__ out_depth_alpha,
                      uint32_t* __restrict__ n_contrib, float* __restrict__ score,
-                     unsigned long long* __restrict__ stats, uint32_t* bwd_fill, uint32_t* bwd_items) {
+                     unsigned long long* __restrict__ stats, uint32_t* bwd_fill, uint32_t* bwd_items, int P_view) {
     constexpr int PPL = 1;
     constexpr int kThreads = 256;
     unsigned int st_eval = 0, st_lanes = 0;
@@ -158,6 +162,7 @@ composite_fwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, cons
     extern __shared__ __align__(128) unsigned char smem_raw[];
     SmemCta& sm = *reinterpret_cast<SmemCta*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    if (SCORE_ONLY && header[GSR_H_OVERFLOW] != 0u) return;
     const uint32_t max_pairs = header[GSR_H_MAX_PAIRS];
 
     for (;;) {
@@ -187,7 +192,9 @@ composite_fwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, cons
         const int view = tys / gy_view, tyi = tys - view * gy_view;
         const int row0 = view * gy_view * GSR_TILE;
         const float* bgv = bg + 3 * view;
-        const float bg0 = __ldg(bgv), bg1 = __ldg(bgv + 1), bg2 = __ldg(bgv + 2);
+        const float bg0 = SCORE_ONLY ? 0.f : __ldg(bgv), bg1 = SCORE_ONLY ? 0.f : __ldg(bgv + 1),
+                    bg2 = SCORE_ONLY ? 0.f : __ldg(bgv + 2);
+        const uint32_t idx0 = SCORE_ONLY ? (uint32_t)view * (uint32_t)P_view : 0u;   // first score row of this view
         const int X0i = txi * GSR_TILE + (blk & 1) * 8, Y0i = tyi * GSR_TILE + (blk >> 1) * (4 * PPL);
         const int Xi = X0i + (lane & 7), Yi = Y0i + (lane >> 3);
         const float X0 = (float)X0i, Y0 = (float)Y0i, X = (float)Xi;
@@ -218,8 +225,9 @@ composite_fwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, cons
         for (int c = 0; c < nchunks; ++c) {
             cp_async_wait<0>();   // my copies for chunk c have landed
             // barrier: everyone's copies for chunk c are visible, everyone is done with chunk c-1;
-            // it doubles as the CTA-wide early-out vote
-            const int ndone = __syncthreads_count(all_done);
+            // it doubles as the CTA-wide early-out vote.  all_done is done[0] (PPL is 1); SCORE_ONLY votes on done[0]
+            // itself, which saves that instantiation the register a separate all_done costs.
+            const int ndone = __syncthreads_count(SCORE_ONLY ? done[0] : all_done);
             if (ndone == kThreads) break;
             // issue the gathers for chunk c+1 (they fly while chunk c is blended), then fetch the
             // keys of chunk c+2
@@ -233,7 +241,7 @@ composite_fwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, cons
 
             const GsrRec* st = sm.rec[c & 1];
             const int cnt = min(kChunk, n - c * kChunk);
-            if (__all_sync(0xffffffffu, all_done)) continue;   // this warp is saturated
+            if (__all_sync(0xffffffffu, SCORE_ONLY ? done[0] : all_done)) continue;   // this warp is saturated
             for (int sub = 0; sub * 32 < cnt; ++sub) {
                 const int r = sub * 32 + lane;
                 bool pass = false;
@@ -273,10 +281,10 @@ composite_fwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, cons
                         for (int o = 16; o > 0; o >>= 1) wsum += __shfl_xor_sync(0xffffffffu, wsum, o);
                         if (lane == 0 && wsum != 0.f) {
                             if (DET)
-                                atomicAdd(reinterpret_cast<unsigned long long*>(score) + __float_as_uint(q2.w),
+                                atomicAdd(reinterpret_cast<unsigned long long*>(score) + (__float_as_uint(q2.w) - idx0),
                                           (unsigned long long)gsr_det_score_quantise(wsum));
                             else
-                                atomicAdd(score + __float_as_uint(q2.w), wsum);
+                                atomicAdd(score + (__float_as_uint(q2.w) - idx0), wsum);
                         }
                     }
                 };
@@ -319,6 +327,7 @@ composite_fwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, cons
             }
         }
         cp_async_wait<0>();   // never leave copies in flight across tiles (early-out case)
+        if constexpr (SCORE_ONLY) continue;   // no image, n_contrib or backward work list
 
         const size_t plane = (size_t)Hs * W;
 #pragma unroll
@@ -562,19 +571,11 @@ composite_bwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, cons
                 const float4* rp = sp + 3 * b;
                 const float4 q0 = rp[0], q1 = rp[1];
                 const uint32_t pos = pos0 + (uint32_t)b;
-                // ---- the blending test (identical decisions to eval_pair) ----
-                const float2 d = fadd2_rn(make_float2(q0.x, q0.y), XY);          // (dx, dy)
-#ifdef GSR_EXACT_EXP
+                // ---- the blending test ----
                 const PairEval e = eval_pair(q0.x, q0.y, q0.w, q1.x, q1.y, q1.z, -XY.x, -XY.y);
+                const float2 d = make_float2(e.dx, e.dy);
                 const float G = e.G, alpha = e.alpha;
                 const bool valid = e.valid;
-#else
-                const float u = __fmaf_rn(q0.w, d.x, __fmul_rn(q1.x, d.y));
-                const float p2 = __fmaf_rn(__fmul_rn(q1.y, d.y), d.y, __fmul_rn(u, d.x));
-                const float G = ex2_approx(p2);
-                const float alpha = fminf(GSR_ALPHA_MAX, __fmul_rn(q1.z, G));
-                const bool valid = (p2 <= 0.0f) && (alpha >= GSR_ALPHA_MIN);
-#endif
                 const bool contrib = valid && pos <= last;
                 const uint32_t cm = __ballot_sync(0xffffffffu, contrib);
                 if (STATS) ++st_eval;
@@ -678,139 +679,6 @@ det_score_kernel(int n, const unsigned long long* __restrict__ score_fx, float* 
     if (i < n) score[i] = gsr_det_score_dequantise((long long)score_fx[i]);
 }
 
-// =============================================================================================
-// Score-only compositing (b200gsr_score_views): composite_fwd_kernel's tile loop, cull, eval_pair, T recurrence,
-// 1/255 skip, T < 1e-4 stop and two entries in flight, carrying T alone.  No image, n_contrib or backward work
-// list is written.  Every view of the stacked pass adds into ONE accumulator of P_view rows: entry idx of view v
-// commits to row idx - v * P_view.  DET: `score` is int64 [P_view] and each warp's weight sum is committed as
-// gsr_det_score_quantise(wsum), otherwise float [P_view].  A pass that overflowed its pair capacity commits nothing,
-// so re-issuing it with a larger capacity adds exactly what one complete pass adds.
-// =============================================================================================
-template <bool DET>
-__global__ void __launch_bounds__(256)
-composite_score_kernel(int H, int W, int gx, int gy_view, int ntiles, int P_view, const uint32_t* __restrict__ header,
-                       const uint32_t* __restrict__ work_order, const uint32_t* __restrict__ tile_start,
-                       const unsigned long long* __restrict__ keys, const GsrRec* __restrict__ geom,
-                       uint32_t* __restrict__ queue, void* __restrict__ score) {
-    constexpr int kThreads = 256;
-    constexpr int kPer = kChunk / kThreads;
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    SmemCta& sm = *reinterpret_cast<SmemCta*>(smem_raw);
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    if (header[GSR_H_OVERFLOW] != 0u) return;
-    const uint32_t max_pairs = header[GSR_H_MAX_PAIRS];
-
-    for (;;) {
-        if (tid == 0) sm.work = atomicAdd(queue, 1u);
-        __syncthreads();
-        const uint32_t w = sm.work;
-        __syncthreads();
-        if (w >= (uint32_t)ntiles) break;
-        const uint32_t tile = work_order[w];
-        uint32_t beg = tile_start[tile], end = tile_start[tile + 1];
-        if (end > max_pairs) end = max_pairs;
-        if (beg > end) beg = end;
-        const int n = (int)(end - beg);
-        const int nchunks = (n + kChunk - 1) / kChunk;
-        const unsigned long long* tk = keys + beg;
-        const int tys = tile / gx, txi = tile - tys * gx;
-        const int view = tys / gy_view, tyi = tys - view * gy_view;
-        const uint32_t idx0 = (uint32_t)view * (uint32_t)P_view;
-        const int X0i = txi * GSR_TILE + (wid & 1) * 8, Y0i = tyi * GSR_TILE + (wid >> 1) * 4;
-        const int Xi = X0i + (lane & 7), Yi = Y0i + (lane >> 3);
-        const float X0 = (float)X0i, Y0 = (float)Y0i, X = (float)Xi, Y = (float)Yi;
-        bool done = !(Xi < W && Yi < H);
-        float T = 1.0f;
-
-        unsigned long long knext[kPer];
-#pragma unroll
-        for (int u = 0; u < kPer; ++u) {
-            const int e = u * kThreads + tid;
-            if (e < n) gather_record(&sm.rec[0][e], geom, __ldg(tk + e));
-            knext[u] = (kChunk + e < n) ? __ldg(tk + kChunk + e) : 0ull;
-        }
-        cp_async_commit();
-
-        for (int c = 0; c < nchunks; ++c) {
-            cp_async_wait<0>();
-            const int ndone = __syncthreads_count(done);
-            if (ndone == kThreads) break;
-#pragma unroll
-            for (int u = 0; u < kPer; ++u) {
-                const int e = u * kThreads + tid;
-                if ((c + 1) * kChunk + e < n) gather_record(&sm.rec[(c + 1) & 1][e], geom, knext[u]);
-                knext[u] = ((c + 2) * kChunk + e < n) ? __ldg(tk + (c + 2) * kChunk + e) : 0ull;
-            }
-            cp_async_commit();
-
-            const GsrRec* st = sm.rec[c & 1];
-            const int cnt = min(kChunk, n - c * kChunk);
-            if (__all_sync(0xffffffffu, done)) continue;
-            for (int sub = 0; sub * 32 < cnt; ++sub) {
-                const int r = sub * 32 + lane;
-                bool pass = false;
-                if (r < cnt) {
-                    const float4 q0 = *reinterpret_cast<const float4*>(&st[r]);
-                    pass = cull_pass(q0.x, q0.y, __float_as_uint(q0.z), X0, Y0);
-                }
-                uint32_t mask = __ballot_sync(0xffffffffu, pass);
-                const float4* sp = reinterpret_cast<const float4*>(&st[sub * 32]);
-                // the weight this lane's pixel gives one entry, summed over the warp and committed by lane 0
-                auto blend = [&](const PairEval& e, uint32_t idx) {
-                    float wsum = 0.f;
-                    if (e.valid && !done) {
-                        const float Tn = T * (1.0f - e.alpha);
-                        if (Tn < GSR_T_STOP) {
-                            done = true;
-                        } else {
-                            wsum = e.alpha * T;
-                            T = Tn;
-                        }
-                    }
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) wsum += __shfl_xor_sync(0xffffffffu, wsum, o);
-                    if (lane == 0 && wsum != 0.f) {
-                        if (DET)
-                            atomicAdd(reinterpret_cast<unsigned long long*>(score) + (idx - idx0),
-                                      (unsigned long long)gsr_det_score_quantise(wsum));
-                        else
-                            atomicAdd(reinterpret_cast<float*>(score) + (idx - idx0), wsum);
-                    }
-                };
-                while (mask) {
-                    int bb[kIlp];
-                    bb[0] = __ffs(mask) - 1;
-                    mask &= mask - 1;
-                    int have = 1;                                      // warp-uniform
-#pragma unroll
-                    for (int j = 1; j < kIlp; ++j) {
-                        const bool more = mask != 0u;
-                        bb[j] = more ? __ffs(mask) - 1 : bb[0];
-                        mask &= mask - 1;
-                        have += more ? 1 : 0;
-                    }
-                    float4 r0[kIlp], r1[kIlp];
-                    uint32_t ri[kIlp];
-#pragma unroll
-                    for (int j = 0; j < kIlp; ++j) {
-                        const float4* rj = sp + 3 * bb[j];
-                        r0[j] = rj[0]; r1[j] = rj[1];
-                        ri[j] = __float_as_uint(rj[2].w);
-                    }
-                    PairEval ev[kIlp];
-#pragma unroll
-                    for (int j = 0; j < kIlp; ++j) ev[j] = eval_pair(r0[j].x, r0[j].y, r0[j].w, r1[j].x, r1[j].y, r1[j].z, X, Y);
-#pragma unroll
-                    for (int j = 0; j < kIlp; ++j)
-                        if (j < have) blend(ev[j], ri[j]);
-                }
-                if (__all_sync(0xffffffffu, done)) break;
-            }
-        }
-        cp_async_wait<0>();
-    }
-}
-
 }  // namespace
 
 struct CompPtrs {
@@ -841,15 +709,16 @@ static CompPtrs comp_ptrs(const uint8_t* saved, const b200gsr_saved_layout& vl, 
     return c;
 }
 
-template <bool SCORE, bool STATS, bool DET = false>
+template <bool SCORE, bool STATS, bool DET = false, bool SCORE_ONLY = false>
 static cudaError_t launch_fwd(const GsrFwdArgs& a, int nblocks, const CompPtrs& c, uint32_t* queue, float* score) {
     const int smem = (int)sizeof(SmemCta);
     static std::atomic<unsigned long long> attr_done{0};
-    cudaError_t e = gsr_smem_once(composite_fwd_kernel<SCORE, STATS, DET>, smem, attr_done);
+    cudaError_t e = gsr_smem_once(composite_fwd_kernel<SCORE, STATS, DET, SCORE_ONLY>, smem, attr_done);
     if (e != cudaSuccess) return e;
-    composite_fwd_kernel<SCORE, STATS, DET><<<nblocks, 256, smem, a.stream>>>(
+    composite_fwd_kernel<SCORE, STATS, DET, SCORE_ONLY><<<nblocks, 256, smem, a.stream>>>(
         a.prm.image_height, a.prm.image_width, c.grid.gx, a.gy_view, c.H, c.grid.ntiles, c.header, c.work_order, c.tile_start,
-        c.keys, c.geom, a.prm.bg, queue, a.out_color, a.out_depth_alpha, c.n_contrib, score, a.stats, c.bwd_fill, c.bwd_items);
+        c.keys, c.geom, a.prm.bg, queue, a.out_color, a.out_depth_alpha, c.n_contrib, score, a.stats, c.bwd_fill, c.bwd_items,
+        a.P_view);
     return cudaGetLastError();
 }
 
@@ -877,24 +746,14 @@ cudaError_t gsr_launch_composite_fwd(const GsrFwdArgs& a) {
                             : launch_fwd<false, false>(a, nblocks, c, queue, a.score);
 }
 
-template <bool DET>
-static cudaError_t launch_score(const GsrFwdArgs& a, int nblocks, const CompPtrs& c, uint32_t* queue, void* score_acc) {
-    const int smem = (int)sizeof(SmemCta);
-    static std::atomic<unsigned long long> attr_done{0};
-    cudaError_t e = gsr_smem_once(composite_score_kernel<DET>, smem, attr_done);
-    if (e != cudaSuccess) return e;
-    composite_score_kernel<DET><<<nblocks, 256, smem, a.stream>>>(
-        a.prm.image_height, a.prm.image_width, c.grid.gx, a.gy_view, c.grid.ntiles, a.P_view, c.header, c.work_order,
-        c.tile_start, c.keys, c.geom, queue, score_acc);
-    return cudaGetLastError();
-}
-
 cudaError_t gsr_launch_composite_score(const GsrFwdArgs& a, void* score_acc) {
     const CompPtrs c = comp_ptrs(a.saved, a.vl, a.prm.image_height, a.prm.image_width, a.num_views, a.gy_view);
     if (c.grid.ntiles == 0 || a.P_view == 0) return cudaSuccess;
     uint32_t* queue = reinterpret_cast<uint32_t*>(a.scratch + a.sl.counters) + GSR_C_FWD_QUEUE;
     const int nblocks = min(c.grid.ntiles, a.num_sms * 6);
-    return a.det ? launch_score<true>(a, nblocks, c, queue, score_acc) : launch_score<false>(a, nblocks, c, queue, score_acc);
+    float* acc = static_cast<float*>(score_acc);   // int64 [P_view] with a.det (DET reinterprets it)
+    return a.det ? launch_fwd<true, false, true, true>(a, nblocks, c, queue, acc)
+                 : launch_fwd<true, false, false, true>(a, nblocks, c, queue, acc);
 }
 
 cudaError_t gsr_launch_score_finish(int n, const unsigned long long* score_fx, float* score, cudaStream_t s) {

@@ -282,7 +282,12 @@ __device__ __forceinline__ void sh_color(const float (&B)[16], const float* row,
 // =========================================================================================
 // DET (deterministic mode): also zero this view's rows of the fixed-point accumulators (GsrDetLayout) - the score
 // (det_score_kernel converts every row) and the gradient sums and maxima - and the second backward pass's work queue.
-template <int MT, bool DET = false>
+// GEO: the geometry-only projection of the score pass (b200gsr_score_views).  The important score depends on geometry
+// and opacity only, so this mode stages no SH row and reads no colour (at M = 16 that is 192 of the 236 bytes read per
+// Gaussian); record part 2 carries only the index.  The cull, radius, tile rect, depth bits and record parts 0/1 are
+// the default mode's statements, so the tile lists are those of a score_flag render.  No backward state is written and
+// `radii` may be null.  Every GEO difference is a compile-time guard, so the other instantiations carry no trace of it.
+template <int MT, bool DET = false, bool GEO = false>
 __global__ void __launch_bounds__(kBlock)
 project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
                   const float* __restrict__ shs, const float* __restrict__ colors,
@@ -348,7 +353,7 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
             rd.y += (uint32_t)tile_row_off << 16;
             miny += tile_row_off; maxy += tile_row_off;
         }
-        radii[rec_base + i] = radius;
+        if (!GEO || radii != nullptr) radii[rec_base + i] = radius;
         rectdepth[rec_base + i] = rd;
         if (DET && score_fx != nullptr) score_fx[rec_base + i] = 0ull;
     }
@@ -365,7 +370,7 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
     }
     const int stride = sh_row_stride(p.M);
     const int ncoef = (p.sh_degree + 1) * (p.sh_degree + 1);
-    if (shs != nullptr) {
+    if (!GEO && shs != nullptr) {
         vis_s[threadIdx.x] = vis;
         __syncthreads();
         stage_sh_rows<MT>(shs, p.M, 3 * ncoef, g0, p.P, vis_s, sh_buf, stride);
@@ -382,7 +387,9 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
     }
 
     float rgb[3];
-    if (shs != nullptr) {
+    if constexpr (GEO) {
+        rgb[0] = rgb[1] = rgb[2] = 0.0f;
+    } else if (shs != nullptr) {
         float dx = x - C.cam[0], dy = y - C.cam[1], dz = z - C.cam[2];
         float dn = sqrtf(dx * dx + dy * dy + dz * dz);
         if (dn == 0.0f) dn = 1.0f;
@@ -423,107 +430,11 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
     float4* dst = reinterpret_cast<float4*>(geom + rec_base + i);
     const float4* src = reinterpret_cast<const float4*>(&rec);
     dst[0] = src[0]; dst[1] = src[1]; dst[2] = src[2];
-    if (dgeom != nullptr) {   // gradient accumulators of this (visible) Gaussian start at zero
+    if (!GEO && dgeom != nullptr) {   // gradient accumulators of this (visible) Gaussian start at zero
         float4* dz = reinterpret_cast<float4*>(dgeom + 12 * (size_t)(rec_base + i));
         const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
         dz[0] = z4; dz[1] = z4; dz[2] = z4;
     }
-}
-
-// =========================================================================================
-// Geometry-only forward of the score pass (b200gsr_score_views).  The important score depends on geometry and
-// opacity only, so this sibling of project_sh_kernel reads neither SH rows nor colours (at M = 16 that is
-// 192 of the 236 bytes read per Gaussian).  The cull, radius, tile rect, depth bits and record parts 0/1 are
-// computed by the same statements as project_sh_kernel's, so the tile lists are the lists of a score_flag
-// render; part 2 carries only the index.  No backward state is written; `radii` may be null.  The statements are
-// repeated rather than shared: moving them into helpers changes project_sh_kernel's generated code.
-// =========================================================================================
-__global__ void __launch_bounds__(kBlock)
-project_geo_kernel(b200gsr_params p, const float* __restrict__ means3D, const float* __restrict__ opac,
-                   const float* __restrict__ scales, const float* __restrict__ rots, const float* __restrict__ cov3d,
-                   int32_t* __restrict__ radii, uint4* __restrict__ rectdepth, GsrRec* __restrict__ geom,
-                   uint32_t* __restrict__ tile_count, uint32_t* __restrict__ zero_words, int num_zero_words,
-                   int rec_base, int tile_row_off, int ntiles_total) {
-    const int i = blockIdx.x * kBlock + threadIdx.x;
-    for (int zw = i; zw < num_zero_words; zw += gridDim.x * kBlock) zero_words[zw] = 0u;
-    if (i >= p.P) return;
-    Cam C;
-    load_cam(p, C);
-    const GsrTileGrid grid = gsr_grid(p.image_height, p.image_width);
-    Geo g;
-    const float x = __ldg(means3D + 3 * (size_t)i), y = __ldg(means3D + 3 * (size_t)i + 1),
-                z = __ldg(means3D + 3 * (size_t)i + 2);
-    int radius = 0;
-    int minx = 0, maxx = 0, miny = 0, maxy = 0;
-    uint4 rd = make_uint4(0u, 0u, 0u, 0u);
-    bool vis = false;
-    geo_view(C, x, y, z, g);
-    rd.z = __float_as_uint(g.tz);
-    if (g.tz > GSR_NEAR_Z) {
-        RawShape raw;
-        load_shape(scales, rots, cov3d, i, raw);
-        geo_rest(C, p, x, y, z, cov3d != nullptr, raw, g);
-        if (g.det != 0.0f) {
-            const float mid = MUL(0.5f, ADD(g.a, g.c));
-            const float sq = SQRT(fmaxf(SUB(MUL(mid, mid), g.det), 0.1f));
-            const float lam = fmaxf(ADD(mid, sq), SUB(mid, sq));
-            float rad_f = ceilf(MUL(3.0f, SQRT(lam)));
-            if (isnan(rad_f)) rad_f = 0.0f;
-            rad_f = fminf(fmaxf(rad_f, 0.0f), 1.0e9f);
-            minx = tile_coord(SUB(g.px, rad_f), grid.gx);
-            maxx = tile_coord(ADD(ADD(g.px, rad_f), 15.0f), grid.gx);
-            miny = tile_coord(SUB(g.py, rad_f), grid.gy);
-            maxy = tile_coord(ADD(ADD(g.py, rad_f), 15.0f), grid.gy);
-            const int touched = (maxx - minx) * (maxy - miny);
-            if (touched > 0) {
-                vis = true;
-                radius = (int)rad_f;
-                rd.x = (uint32_t)minx | ((uint32_t)miny << 16);
-                rd.y = (uint32_t)maxx | ((uint32_t)maxy << 16);
-                rd.w = (uint32_t)touched;
-            }
-        }
-    }
-    if (vis) {
-        rd.x += (uint32_t)tile_row_off << 16;
-        rd.y += (uint32_t)tile_row_off << 16;
-        miny += tile_row_off; maxy += tile_row_off;
-    }
-    if (radii != nullptr) radii[rec_base + i] = radius;
-    rectdepth[rec_base + i] = rd;
-    if (!vis) return;
-    if (!gsr_use_multisplit(ntiles_total)) {
-        uint32_t* cnt = tile_count + (size_t)(((rec_base + i) >> 5) & (GSR_COPIES - 1)) * ntiles_total;
-        for (int ty = miny; ty < maxy; ++ty)
-            for (int tx = minx; tx < maxx; ++tx) atomicAdd(cnt + ty * grid.gx + tx, 1u);
-    }
-    const float o = __ldg(opac + i);
-    float ex = -1.0f, ey = -1.0f;
-    if (o * 255.0f > 1.0f) {
-        const float tau2 = 2.0f * __logf(o * 255.0f) * 1.01f + 0.01f;
-        ex = sqrtf(tau2 * g.a) * 1.003f + 0.05f;
-        ey = sqrtf(tau2 * g.c) * 1.003f + 0.05f;
-        if (!(ex == ex)) ex = 65504.0f * 2.0f;
-        if (!(ey == ey)) ey = 65504.0f * 2.0f;
-    }
-    const __half2 eh = __floats2half2_rn(ex, ey);
-    GsrRec rec;
-    rec.px = g.px; rec.py = g.py;
-#ifdef GSR_EXACT_EXP
-    rec.A = MUL(g.c, g.det_inv);
-    rec.B = MUL(-g.b, g.det_inv);
-    rec.C = MUL(g.a, g.det_inv);
-#else
-    rec.A = -0.5f * GSR_LOG2E * MUL(g.c, g.det_inv);
-    rec.B = GSR_LOG2E * MUL(g.b, g.det_inv);
-    rec.C = -0.5f * GSR_LOG2E * MUL(g.a, g.det_inv);
-#endif
-    rec.opacity = o; rec.depth = g.tz;
-    rec.ext = *reinterpret_cast<const uint32_t*>(&eh);
-    float4* dst = reinterpret_cast<float4*>(geom + rec_base + i);
-    const float4* src = reinterpret_cast<const float4*>(&rec);
-    dst[0] = src[0]; dst[1] = src[1];
-    dst[2] = make_float4(0.f, 0.f, 0.f, __uint_as_float((uint32_t)(rec_base + i)));
 }
 
 // =========================================================================================
@@ -870,7 +781,7 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D,
 
 }  // namespace
 
-template <int MT, bool DET>
+template <int MT, bool DET, bool GEO = false>
 static void launch_project_sh(const GsrFwdArgs& a, int P, size_t smem) {
     // multisplit path: counters + the single per-tile counter array are zeroed in the prologue
     // (api.cu issues a memset instead on the large-grid fallback, where this kernel counts itself)
@@ -878,7 +789,7 @@ static void launch_project_sh(const GsrFwdArgs& a, int P, size_t smem) {
     tg.gy = a.num_views * a.gy_view; tg.ntiles = tg.gx * tg.gy;      // the stacked image
     const int nzero = gsr_use_multisplit(tg.ntiles) ? (int)gsr_counter_words(a.sl, tg.ntiles) : 0;
     const bool bwd = !(a.flags & B200GSR_FWD_NO_BACKWARD);
-    project_sh_kernel<MT, DET><<<(P + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
+    project_sh_kernel<MT, DET, GEO><<<(P + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
         a.prm, a.means3D, a.shs, a.colors, a.opac, a.scales, a.rots, a.cov3d, a.radii,
         reinterpret_cast<uint4*>(a.scratch + a.sl.rectdepth),
         reinterpret_cast<GsrRec*>(a.saved + a.vl.geom),
@@ -892,11 +803,14 @@ static void launch_project_sh(const GsrFwdArgs& a, int P, size_t smem) {
         DET && bwd && a.view == 0 ? reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE_DET : nullptr);
 }
 
-cudaError_t gsr_launch_project(const GsrFwdArgs& a) {
+cudaError_t gsr_launch_project(const GsrFwdArgs& a, bool geo) {
     const int P = a.prm.P;
     if (P == 0) return cudaSuccess;
     const size_t smem = a.shs ? (size_t)kBlock * sh_row_stride(a.prm.M) * sizeof(float) : 0;
-    if (a.det) {
+    if (geo) {
+        // the score pass accumulates into the caller's buffer, deterministic or not: no DET instantiation
+        launch_project_sh<0, false, true>(a, P, 0);
+    } else if (a.det) {
         if (a.shs && a.prm.M == 16) launch_project_sh<16, true>(a, P, smem);
         else if (a.shs && a.prm.M == 4) launch_project_sh<4, true>(a, P, smem);
         else launch_project_sh<0, true>(a, P, smem);
@@ -905,20 +819,6 @@ cudaError_t gsr_launch_project(const GsrFwdArgs& a) {
         else if (a.shs && a.prm.M == 4) launch_project_sh<4, false>(a, P, smem);
         else launch_project_sh<0, false>(a, P, smem);
     }
-    return cudaGetLastError();
-}
-
-cudaError_t gsr_launch_project_geo(const GsrFwdArgs& a) {
-    const int P = a.prm.P;
-    if (P == 0) return cudaSuccess;
-    GsrTileGrid tg = gsr_grid(a.prm.image_height, a.prm.image_width);
-    tg.gy = a.num_views * a.gy_view; tg.ntiles = tg.gx * tg.gy;      // the stacked image
-    const int nzero = gsr_use_multisplit(tg.ntiles) ? (int)gsr_counter_words(a.sl, tg.ntiles) : 0;
-    project_geo_kernel<<<(P + kBlock - 1) / kBlock, kBlock, 0, a.stream>>>(
-        a.prm, a.means3D, a.opac, a.scales, a.rots, a.cov3d, a.radii,
-        reinterpret_cast<uint4*>(a.scratch + a.sl.rectdepth), reinterpret_cast<GsrRec*>(a.saved + a.vl.geom),
-        reinterpret_cast<uint32_t*>(a.scratch + a.sl.tile_count), reinterpret_cast<uint32_t*>(a.scratch), nzero,
-        a.view * a.P_view, a.view * a.gy_view, tg.ntiles);
     return cudaGetLastError();
 }
 
