@@ -4,20 +4,12 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+from typing import Optional
+
+import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200GSR_LIB", os.path.join(HERE, "libb200gsr.so"))   # override: A/B builds only
-
-EXPORTS = ["b200gsr_version", "b200gsr_last_error", "b200gsr_saved_layout_query",
-           "b200gsr_scratch_layout_query", "b200gsr_forward", "b200gsr_backward", "b200gsr_backward_ex",
-           "b200gsr_mark_visible", "b200gsr_profile_enable", "b200gsr_profile_counts",
-           "b200gsr_profile_read", "b200gsr_debug_counters", "b200gsr_dist2_scratch_bytes", "b200gsr_dist2_knn3",
-           "b200gsr_assemble_forward", "b200gsr_assemble_backward", "b200gsr_disparity_forward",
-           "b200gsr_disparity_backward", "b200gsr_densify_stats", "b200gsr_densify_scratch_bytes",
-           "b200gsr_densify_plan", "b200gsr_densify_map", "b200gsr_compact_plan", "b200gsr_gather_rows",
-           "b200gsr_split_children", "b200gsr_kth_smallest", "b200gsr_views_geometry", "b200gsr_forward_views",
-           "b200gsr_backward_views", "b200gsr_sh_grad_expand", "b200gsr_backward_views_ex",
-           "b200gsr_disparity_backward_ex", "b200gsr_score_views", "b200gsr_score_finish", "b200gsr_adam_step"]
 
 
 class Params(C.Structure):
@@ -69,8 +61,54 @@ class ScratchLayout(C.Structure):
                                           "ms_hist", "total")]
 
 
+i32, u32, u64, sz, f32, vp, _P = C.c_int32, C.c_uint32, C.c_uint64, C.c_size_t, C.c_float, C.c_void_p, C.POINTER
+# b200gsr_backward / _ex: the seven inputs, radii, depth_alpha, the two incoming gradients, saved, scratch, max_pairs and
+# the eight gradient outputs
+_BWD_ARGS = [vp] * 11 + [vp, sz, vp, sz, u64] + [vp] * 8
+
+# Every entry point of include/b200gsr.h: name -> (restype, argtypes), in the header's order.
+SIGNATURES = {
+    "b200gsr_version": (C.c_int, []),
+    "b200gsr_last_error": (C.c_char_p, []),
+    "b200gsr_saved_layout_query": (C.c_int, [i32, i32, i32, u64, i32, _P(SavedLayout)]),
+    "b200gsr_scratch_layout_query": (C.c_int, [i32, i32, i32, u64, _P(ScratchLayout)]),
+    "b200gsr_forward": (C.c_int, [_P(Params)] + [vp] * 11 + [vp, sz, vp, sz, u64, u32, vp, u32, vp]),
+    "b200gsr_backward": (C.c_int, [_P(Params)] + _BWD_ARGS + [vp]),
+    "b200gsr_backward_ex": (C.c_int, [_P(Params)] + _BWD_ARGS + [u32, i32, i32, i32, vp]),
+    "b200gsr_sh_grad_expand": (C.c_int, [i32, i32, i32, i32, vp, vp, sz, vp, vp]),
+    "b200gsr_views_geometry": (C.c_int, [i32, i32, i32, _P(i32)]),
+    "b200gsr_forward_views": (C.c_int, [i32, _P(Params), _P(ViewInputs)] + [vp] * 5 + [sz, vp, sz, u64, u32, vp, u32, vp]),
+    "b200gsr_backward_views": (C.c_int, [i32, _P(Params), _P(ViewInputs)] + [vp] * 5 + [sz, u64, _P(ViewGrads), vp]),
+    "b200gsr_backward_views_ex": (C.c_int, [i32, _P(Params), _P(ViewInputs)] + [vp] * 5 + [sz, u64, _P(ViewGrads), u32, vp]),
+    "b200gsr_score_views": (C.c_int, [i32, _P(Params), _P(ViewInputs), vp, vp, sz, vp, sz, u64, u32, vp, u32, vp]),
+    "b200gsr_score_finish": (C.c_int, [i32, vp, vp, u32, vp]),
+    "b200gsr_mark_visible": (C.c_int, [i32, vp, vp, vp, vp, vp]),
+    "b200gsr_assemble_forward": (C.c_int, [i32, _P(Group), i32, i32, f32, f32, vp, vp, u64] + [vp] * 5 + [vp]),
+    "b200gsr_assemble_backward": (C.c_int, [i32, _P(Group), _P(GroupGrad), i32, i32, f32, f32, vp, vp, u64] + [vp] * 5 + [vp]),
+    "b200gsr_disparity_forward": (C.c_int, [i32, i32, vp, vp, vp, vp, vp]),
+    "b200gsr_disparity_backward": (C.c_int, [i32, i32, vp, vp, vp, vp, vp, vp, vp]),
+    "b200gsr_disparity_backward_ex": (C.c_int, [i32, i32, vp, vp, vp, vp, vp, vp, u32, vp]),
+    "b200gsr_densify_stats": (C.c_int, [i32, vp, vp, vp, vp, vp, vp]),
+    "b200gsr_densify_scratch_bytes": (C.c_size_t, [i32]),
+    "b200gsr_densify_plan": (C.c_int, [i32, vp, vp, vp, vp, f32, f32, f32, f32, f32, vp, vp, vp]),
+    "b200gsr_densify_map": (C.c_int, [i32, i32, vp, vp, vp, vp, vp]),
+    "b200gsr_compact_plan": (C.c_int, [i32, vp, vp, vp, vp, vp]),
+    "b200gsr_gather_rows": (C.c_int, [i32, i32, vp, vp, vp, i32, vp]),
+    "b200gsr_split_children": (C.c_int, [i32, i32, f32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "b200gsr_kth_smallest": (C.c_int, [i32, vp, u32, vp, vp, vp]),
+    "b200gsr_adam_step": (C.c_int, [i32, _P(AdamTensor), vp]),
+    "b200gsr_dist2_scratch_bytes": (C.c_size_t, [i32]),
+    "b200gsr_dist2_knn3": (C.c_int, [i32, vp, vp, vp, sz, vp]),
+    "b200gsr_profile_enable": (C.c_int, [i32]),
+    "b200gsr_debug_counters": (C.c_int, [vp]),
+    "b200gsr_profile_counts": (C.c_int, [_P(i32), _P(i32)]),
+    "b200gsr_profile_read": (C.c_int, [i32, i32, _P(f32)]),
+}
+EXPORTS = list(SIGNATURES)
+
 _lib = None
 ABI_VERSION = 3
+ERR_BAD_ARG = -1
 FWD_NO_BACKWARD = 1
 FWD_DETERMINISTIC = 2
 BWD_COMPOSITE, BWD_PROJECT = 1, 2
@@ -96,69 +134,9 @@ def load():
                 f"{LIB_PATH} is missing and could not be built ({err}). Build it with "
                 "`python -m dreamscene_b200._build` (needs nvcc; sm_90a only). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    vp, sz, u64, u32, i32 = C.c_void_p, C.c_size_t, C.c_uint64, C.c_uint32, C.c_int32
-    lib.b200gsr_version.restype = C.c_int
-    lib.b200gsr_last_error.restype = C.c_char_p
-    lib.b200gsr_saved_layout_query.argtypes = [i32, i32, i32, u64, i32, C.POINTER(SavedLayout)]
-    lib.b200gsr_scratch_layout_query.argtypes = [i32, i32, i32, u64, C.POINTER(ScratchLayout)]
-    lib.b200gsr_forward.argtypes = [C.POINTER(Params)] + [vp] * 7 + [vp] * 4 + \
-        [vp, sz, vp, sz, u64, u32, vp, u32, vp]
-    lib.b200gsr_backward.argtypes = [C.POINTER(Params)] + [vp] * 7 + [vp] * 4 + \
-        [vp, sz, vp, sz, u64] + [vp] * 8 + [vp]
-    lib.b200gsr_backward_ex.argtypes = lib.b200gsr_backward.argtypes[:-1] + [u32, i32, i32, i32, vp]
-    lib.b200gsr_backward_ex.restype = C.c_int
-    lib.b200gsr_mark_visible.argtypes = [i32, vp, vp, vp, vp, vp]
-    lib.b200gsr_sh_grad_expand.argtypes = [i32, i32, i32, i32, vp, vp, sz, vp, vp]
-    lib.b200gsr_sh_grad_expand.restype = C.c_int
-    lib.b200gsr_dist2_scratch_bytes.argtypes = [i32]
-    lib.b200gsr_dist2_scratch_bytes.restype = C.c_size_t
-    lib.b200gsr_dist2_knn3.argtypes = [i32, vp, vp, vp, sz, vp]
-    lib.b200gsr_dist2_knn3.restype = C.c_int
-    lib.b200gsr_assemble_forward.argtypes = [i32, C.POINTER(Group), i32, i32, C.c_float, C.c_float, vp, vp, u64] + [vp] * 5 + [vp]
-    lib.b200gsr_assemble_backward.argtypes = [i32, C.POINTER(Group), C.POINTER(GroupGrad), i32, i32, C.c_float, C.c_float,
-                                              vp, vp, u64] + [vp] * 5 + [vp]
-    lib.b200gsr_assemble_forward.restype = lib.b200gsr_assemble_backward.restype = C.c_int
-    lib.b200gsr_disparity_forward.argtypes = [i32, i32, vp, vp, vp, vp, vp]
-    lib.b200gsr_disparity_backward.argtypes = [i32, i32, vp, vp, vp, vp, vp, vp, vp]
-    lib.b200gsr_disparity_backward_ex.argtypes = [i32, i32, vp, vp, vp, vp, vp, vp, u32, vp]
-    lib.b200gsr_disparity_forward.restype = lib.b200gsr_disparity_backward.restype = C.c_int
-    lib.b200gsr_disparity_backward_ex.restype = C.c_int
-    f = C.c_float
-    lib.b200gsr_densify_stats.argtypes = [i32, vp, vp, vp, vp, vp, vp]
-    lib.b200gsr_densify_scratch_bytes.argtypes = [i32]
-    lib.b200gsr_densify_scratch_bytes.restype = C.c_size_t
-    lib.b200gsr_densify_plan.argtypes = [i32, vp, vp, vp, vp, f, f, f, f, f, vp, vp, vp]
-    lib.b200gsr_densify_map.argtypes = [i32, i32, vp, vp, vp, vp, vp]
-    lib.b200gsr_compact_plan.argtypes = [i32, vp, vp, vp, vp, vp]
-    lib.b200gsr_gather_rows.argtypes = [i32, i32, vp, vp, vp, i32, vp]
-    lib.b200gsr_split_children.argtypes = [i32, i32, f, vp, vp, vp, vp, vp, vp, vp, vp, vp]
-    lib.b200gsr_kth_smallest.argtypes = [i32, vp, u32, vp, vp, vp]
-    for fn in ("b200gsr_densify_stats", "b200gsr_densify_plan", "b200gsr_densify_map", "b200gsr_compact_plan",
-               "b200gsr_gather_rows", "b200gsr_split_children", "b200gsr_kth_smallest"):
-        getattr(lib, fn).restype = C.c_int
-    lib.b200gsr_views_geometry.argtypes = [i32, i32, i32, C.POINTER(i32)]
-    lib.b200gsr_forward_views.argtypes = [i32, C.POINTER(Params), C.POINTER(ViewInputs), vp, vp, vp, vp, vp, sz, vp, sz,
-                                          u64, u32, vp, u32, vp]
-    lib.b200gsr_backward_views.argtypes = [i32, C.POINTER(Params), C.POINTER(ViewInputs), vp, vp, vp, vp, vp, sz, u64,
-                                           C.POINTER(ViewGrads), vp]
-    lib.b200gsr_backward_views_ex.argtypes = lib.b200gsr_backward_views.argtypes[:-1] + [u32, vp]
-    for fn in ("b200gsr_views_geometry", "b200gsr_forward_views", "b200gsr_backward_views", "b200gsr_backward_views_ex"):
-        getattr(lib, fn).restype = C.c_int
-    lib.b200gsr_score_views.argtypes = [i32, C.POINTER(Params), C.POINTER(ViewInputs), vp, vp, sz, vp, sz, u64, u32, vp, u32, vp]
-    lib.b200gsr_score_finish.argtypes = [i32, vp, vp, u32, vp]
-    lib.b200gsr_score_views.restype = lib.b200gsr_score_finish.restype = C.c_int
-    lib.b200gsr_adam_step.argtypes = [i32, C.POINTER(AdamTensor), vp]
-    lib.b200gsr_adam_step.restype = C.c_int
-    lib.b200gsr_debug_counters.argtypes = [vp]
-    lib.b200gsr_debug_counters.restype = C.c_int
-    lib.b200gsr_profile_enable.argtypes = [i32]
-    lib.b200gsr_profile_counts.argtypes = [C.POINTER(i32), C.POINTER(i32)]
-    lib.b200gsr_profile_read.argtypes = [i32, i32, C.POINTER(C.c_float)]
-    for f in ("b200gsr_profile_enable", "b200gsr_profile_counts", "b200gsr_profile_read"):
-        getattr(lib, f).restype = C.c_int
-    for f in ("b200gsr_saved_layout_query", "b200gsr_scratch_layout_query", "b200gsr_forward",
-              "b200gsr_backward", "b200gsr_mark_visible"):
-        getattr(lib, f).restype = C.c_int
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:
         raise RuntimeError(f"{LIB_PATH} has ABI version {lib.b200gsr_version()}, this package needs "
                            f"{ABI_VERSION}: rebuild with `python -m dreamscene_b200._build --force`")
@@ -170,24 +148,60 @@ def last_error() -> str:
     return load().b200gsr_last_error().decode("utf-8", "replace")
 
 
+def check(rc: int, what: str, bad_arg=None) -> None:
+    """Raise for a non-zero return code of the entry point `what`: RuntimeError("<what> failed (<rc>): <message>").
+    With `bad_arg`, B200GSR_ERR_BAD_ARG raises bad_arg(<message>) instead (the rasterizer raises a bare Exception for
+    misused inputs, as the reference's own checks do)."""
+    if rc:
+        msg = last_error()
+        if rc == ERR_BAD_ARG and bad_arg is not None:
+            raise bad_arg(msg)
+        raise RuntimeError(f"{what} failed ({rc}): {msg}")
+
+
+def ptr(t: Optional[torch.Tensor]) -> Optional[C.c_void_p]:
+    return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def stream(dev) -> C.c_void_p:
+    """The current stream of `dev`, as the `void* stream` every entry point takes."""
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def prepare(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    """An input as the kernels read it: float32, contiguous, and 16-byte aligned (they use 16-byte vector loads on
+    rows).  `t` itself when it already is.  It does not detach: autograd saves the prepared tensors."""
+    if t is None:
+        return None
+    if t.dtype != torch.float32:
+        t = t.float()
+    t = t.contiguous()
+    if t.data_ptr() % 16:
+        t = t.clone()
+    return t
+
+
 def saved_layout(P: int, H: int, W: int, max_pairs: int, with_backward: bool = True,
                  deterministic: bool = False) -> SavedLayout:
     """deterministic: `total` also covers the fixed-point accumulators of deterministic mode (appended; every
     offset is the same as without)."""
     out = SavedLayout()
     flag = int(bool(with_backward)) | (SAVED_DETERMINISTIC if deterministic else 0)
-    rc = load().b200gsr_saved_layout_query(P, H, W, max_pairs, flag, C.byref(out))
-    if rc:
-        raise RuntimeError(f"b200gsr_saved_layout_query failed ({rc}): {last_error()}")
+    check(load().b200gsr_saved_layout_query(P, H, W, max_pairs, flag, C.byref(out)), "b200gsr_saved_layout_query")
     return out
 
 
 def scratch_layout(P: int, H: int, W: int, max_pairs: int) -> ScratchLayout:
     out = ScratchLayout()
-    rc = load().b200gsr_scratch_layout_query(P, H, W, max_pairs, C.byref(out))
-    if rc:
-        raise RuntimeError(f"b200gsr_scratch_layout_query failed ({rc}): {last_error()}")
+    check(load().b200gsr_scratch_layout_query(P, H, W, max_pairs, C.byref(out)), "b200gsr_scratch_layout_query")
     return out
+
+
+def stacked_height(B: int, H: int, W: int) -> int:
+    """Height of the image that B stacked views of H x W occupy (b200gsr_forward_views, b200gsr_score_views)."""
+    hs = C.c_int32(0)
+    check(load().b200gsr_views_geometry(B, H, W, C.byref(hs)), "b200gsr_views_geometry")
+    return int(hs.value)
 
 
 FWD_STAGES = ("project_sh", "scan_order", "scatter", "tile_sort", "composite_fwd")
@@ -195,9 +209,7 @@ BWD_STAGES = ("composite_bwd", "project_bwd")
 
 
 def profile_enable(max_calls: int) -> None:
-    rc = load().b200gsr_profile_enable(int(max_calls))
-    if rc:
-        raise RuntimeError(f"b200gsr_profile_enable failed ({rc}): {last_error()}")
+    check(load().b200gsr_profile_enable(int(max_calls)), "b200gsr_profile_enable")
 
 
 def profile_collect() -> dict:

@@ -18,7 +18,6 @@ bitwise reproducible and independent of views_per_pass.  Its headroom is 2^26 pi
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Dict, Optional, Sequence, Tuple
 
 import torch
@@ -26,11 +25,6 @@ import torch
 from . import _lib
 from . import densify as _densify
 from . import rasterizer as R
-
-
-def _check(rc, what):
-    if rc:
-        raise RuntimeError(f"{what} failed ({rc}): {_lib.last_error()}")
 
 
 def view_chunks(n_views: int, views_per_pass: int):
@@ -76,43 +70,29 @@ def important_score(settings_list: Sequence[R.GaussianRasterizationSettings], me
         return torch.zeros(P, dtype=torch.float32, device=dev)
     lib = _lib.load()
     with torch.no_grad(), torch.cuda.device(dev):
-        means3D, opacities = R._f32c(means3D.detach()), R._f32c(opacities.detach())
-        scales = R._f32c(None if scales is None else scales.detach())
-        rotations = R._f32c(None if rotations is None else rotations.detach())
-        cov3D_precomp = R._f32c(None if cov3D_precomp is None else cov3D_precomp.detach())
+        inputs = [_lib.prepare(None if t is None else t.detach())
+                  for t in (means3D, None, None, opacities, scales, rotations, cov3D_precomp)]
         d = R._device_state(dev)
         d.resolve()                            # non-blocking overflow check of earlier forwards, as every forward does
-        stream_h = torch.cuda.current_stream(dev).cuda_stream
-        stream = C.c_void_p(stream_h)
+        stream = _lib.stream(dev)
         acc = torch.zeros(P, dtype=torch.int64 if det else torch.float32, device=dev)
         flags = _lib.FWD_NO_BACKWARD | (_lib.FWD_DETERMINISTIC if det else 0)
-        cams = [(s, R._const(s.viewmatrix, dev), R._const(s.projmatrix, dev), R._const(s.campos, dev))
-                for s in settings_list]
+        keep: list = []
+        # M = 0 and no background: the score pass reads no colour (nor sh_degree or score_flag)
+        params = [R._make_params(s, P, 0, keep, dev, None) for s in settings_list]
 
         def issue(b0, b1, cap):
             B = b1 - b0
-            prm = (_lib.Params * B)()
-            vin = (_lib.ViewInputs * B)()
-            for v in range(B):
-                s, vm, pm, cp = cams[b0 + v]
-                prm[v] = _lib.Params(P, 0, 0, H, W, float(s.tanfovx), float(s.tanfovy), float(s.scale_modifier),
-                                     int(bool(s.prefiltered)), 1, None, vm.data_ptr(), pm.data_ptr(), cp.data_ptr())
-                vin[v] = _lib.ViewInputs(means3D.data_ptr(), None, None, opacities.data_ptr(),
-                                         None if scales is None else scales.data_ptr(),
-                                         None if rotations is None else rotations.data_ptr(),
-                                         None if cov3D_precomp is None else cov3D_precomp.data_ptr())
-            hs = C.c_int32(0)
-            _check(lib.b200gsr_views_geometry(B, H, W, C.byref(hs)), "b200gsr_views_geometry")
-            scratch_bytes, saved_bytes = R._layouts(B * P, int(hs.value), W, cap, False)
-            scratch = d.ensure_scratch(stream_h, scratch_bytes)
-            saved = torch.empty(saved_bytes, dtype=torch.uint8, device=dev)
-            slot, seq, notify_ptr = d.claim()
-            rc = lib.b200gsr_score_views(B, prm, vin, C.c_void_p(acc.data_ptr()), C.c_void_p(scratch.data_ptr()),
-                                         scratch.numel(), C.c_void_p(saved.data_ptr()), saved.numel(), cap, flags,
-                                         notify_ptr, seq, stream)
-            if rc:
-                d.release(slot)
-                raise RuntimeError(f"b200gsr_score_views failed ({rc}): {_lib.last_error()}")
+            prm = (_lib.Params * B)(*params[b0:b1])
+            vin = R._view_inputs([inputs] * B)
+
+            def launch(cap, flags, scratch, saved, notify_ptr, seq):
+                return lib.b200gsr_score_views(B, prm, vin, _lib.ptr(acc), _lib.ptr(scratch), scratch.numel(),
+                                               _lib.ptr(saved), saved.numel(), cap, flags, notify_ptr, seq, stream)
+
+            # `saved` holds no deterministic state in the score pass: the accumulator does
+            layout = (B * P, _lib.stacked_height(B, H, W), W, False, False)
+            _, slot, seq = R._issue_once(d, layout, flags, cap, launch, stream.value, False, "b200gsr_score_views")
             return slot, seq
 
         def settle(items):
@@ -139,22 +119,9 @@ def important_score(settings_list: Sequence[R.GaussianRasterizationSettings], me
         if not det:
             return acc
         score = torch.empty(P, dtype=torch.float32, device=dev)
-        _check(lib.b200gsr_score_finish(P, C.c_void_p(acc.data_ptr()), C.c_void_p(score.data_ptr()),
-                                        _lib.FWD_DETERMINISTIC, stream), "b200gsr_score_finish")
+        _lib.check(lib.b200gsr_score_finish(P, _lib.ptr(acc), _lib.ptr(score), _lib.FWD_DETERMINISTIC, stream),
+                   "b200gsr_score_finish")
         return score
-
-
-def _kth_smallest(v: torch.Tensor, k: int) -> torch.Tensor:
-    """-> device tensor [1]: the k-th smallest (0-based) element of v, without a sort or host sync."""
-    v = v.detach().float().contiguous()
-    out = torch.empty(1, dtype=torch.float32, device=v.device)
-    scratch = torch.empty(2048, dtype=torch.uint8, device=v.device)
-    with torch.cuda.device(v.device):
-        _check(_lib.load().b200gsr_kth_smallest(int(v.numel()), C.c_void_p(v.data_ptr()), int(k),
-                                                C.c_void_p(scratch.data_ptr()), C.c_void_p(out.data_ptr()),
-                                                C.c_void_p(torch.cuda.current_stream(v.device).cuda_stream)),
-               "b200gsr_kth_smallest")
-    return out
 
 
 def volume_weighted_score(score: torch.Tensor, scaling_raw: torch.Tensor, v_pow: float) -> torch.Tensor:
@@ -166,7 +133,7 @@ def volume_weighted_score(score: torch.Tensor, scaling_raw: torch.Tensor, v_pow:
     if n == 0:
         return torch.zeros_like(volume)
     index = int(n * 0.9)
-    kth = _kth_smallest(volume, n - 1 - index).reshape(())
+    kth = _densify.kth_smallest(volume, n - 1 - index).reshape(())
     v_list = torch.pow(volume / kth, v_pow)
     return v_list * score.detach()
 

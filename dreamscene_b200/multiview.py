@@ -22,7 +22,6 @@ sorted lists are the same lists, bit for bit - and gradients equal the sum over 
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import List, Optional, Sequence, Union
 
 import torch
@@ -37,16 +36,12 @@ _GRAD_FIELD = {"means3D": "d_means3D", "opacities": "d_opacities", "shs": "d_shs
                "scales": "d_scales", "rotations": "d_rotations", "cov3D_precomp": "d_cov3D"}
 
 
-def _ptr(t):
-    return None if t is None else t.data_ptr()
-
-
 class _RasterizeViews(torch.autograd.Function):
     @staticmethod
     def forward(ctx, settings, spec, B, *flat):
         # spec[name] = None | ("shared", idx) | ("list", [idx...]) into `flat`; flat also holds the B means2D ports last
         lib = _lib.load()
-        tensors = [R._f32c(t) for t in flat]
+        tensors = [_lib.prepare(t) for t in flat]
         get = lambda name, v: None if spec[name] is None else tensors[spec[name][1] if spec[name][0] == "shared" else spec[name][1][v]]
         m0 = get("means3D", 0)
         dev = m0.device
@@ -64,38 +59,25 @@ class _RasterizeViews(torch.autograd.Function):
             d.resolve()
         keep: list = []
         with torch.cuda.device(dev):
-            hs = C.c_int32(0)
-            lib.b200gsr_views_geometry(B, H, W, C.byref(hs))
-            Hs = int(hs.value)
+            Hs = _lib.stacked_height(B, H, W)
             bg_all = torch.stack([R._const(s.bg, dev).reshape(3) for s in settings]).contiguous()
-            keep.append(bg_all)
-            prm = (_lib.Params * B)()
-            vin = (_lib.ViewInputs * B)()
-            for v, s in enumerate(settings):
-                vm, pm, cp = R._const(s.viewmatrix, dev), R._const(s.projmatrix, dev), R._const(s.campos, dev)
-                keep.extend([vm, pm, cp])
-                prm[v] = _lib.Params(P, M, int(s.sh_degree), H, W, float(s.tanfovx), float(s.tanfovy), float(s.scale_modifier),
-                                     int(bool(s.prefiltered)), int(score_flag), bg_all.data_ptr() + 12 * v, vm.data_ptr(),
-                                     pm.data_ptr(), cp.data_ptr())
-                for name in _NAMES:
-                    setattr(vin[v], name, _ptr(get(name, v)))
+            prm = (_lib.Params * B)(*[R._make_params(s, P, M, keep, dev, bg_all, v) for v, s in enumerate(settings)])
+            vin = R._view_inputs([[get(name, v) for name in _NAMES] for v in range(B)])
             color = torch.empty(3, Hs, W, dtype=torch.float32, device=dev)
             depth_alpha = torch.empty(2, Hs, W, dtype=torch.float32, device=dev)
             radii = torch.empty(B, P, dtype=torch.int32, device=dev)
             score = torch.zeros(B, P, dtype=torch.float32, device=dev) if score_flag else None
-            stream_h = torch.cuda.current_stream(dev).cuda_stream
-            stream = C.c_void_p(stream_h)
+            stream = _lib.stream(dev)
             det = R.deterministic_mode()
-            flags = (0 if with_backward else _lib.FWD_NO_BACKWARD) | (_lib.FWD_DETERMINISTIC if det else 0)
+            ptr = _lib.ptr
 
-            def launch(cap, scratch, saved, notify_ptr, seq):
-                return lib.b200gsr_forward_views(B, prm, vin, C.c_void_p(color.data_ptr()), C.c_void_p(depth_alpha.data_ptr()),
-                                                 C.c_void_p(radii.data_ptr()), None if score is None else C.c_void_p(score.data_ptr()),
-                                                 C.c_void_p(scratch.data_ptr()), scratch.numel(), C.c_void_p(saved.data_ptr()),
-                                                 saved.numel(), cap, flags, notify_ptr, seq, stream)
+            def launch(cap, flags, scratch, saved, notify_ptr, seq):
+                return lib.b200gsr_forward_views(B, prm, vin, ptr(color), ptr(depth_alpha), ptr(radii), ptr(score),
+                                                 ptr(scratch), scratch.numel(), ptr(saved), saved.numel(), cap, flags,
+                                                 notify_ptr, seq, stream)
 
             saved, cap = R._issue_with_capacity(d, (B, P, H, W), B * P, Hs, W, with_backward, det, score, launch, capturing,
-                                                stream_h)
+                                                stream.value)
         ctx.meta = (spec, B, P, W, Hs, cap, with_backward, len(flat), det)
         ctx.views = (prm, vin)            # the backward reuses the arrays; `keep` holds their device constants
         ctx.keep = keep
@@ -119,8 +101,8 @@ class _RasterizeViews(torch.autograd.Function):
         if not with_backward:
             raise RuntimeError("b200gsr: backward through a forward that ran without gradient accumulators")
         get = lambda name, v: None if spec[name] is None else tensors[spec[name][1] if spec[name][0] == "shared" else spec[name][1][v]]
-        g_color = torch.zeros(3, Hs, W, device=dev) if g_color is None else R._f32c(g_color)
-        g_da = torch.zeros(2, Hs, W, device=dev) if g_da is None else R._f32c(g_da)
+        g_color = torch.zeros(3, Hs, W, device=dev) if g_color is None else _lib.prepare(g_color)
+        g_da = torch.zeros(2, Hs, W, device=dev) if g_da is None else _lib.prepare(g_da)
         grads: List[Optional[torch.Tensor]] = [None] * nflat
         m2d_base = nflat - B
         with torch.cuda.device(dev):
@@ -141,13 +123,11 @@ class _RasterizeViews(torch.autograd.Function):
                 grads[m2d_base + v] = g2
                 out[v].d_means2D = g2.data_ptr()
                 out[v].accumulate = acc
-            rc = lib.b200gsr_backward_views_ex(B, prm, vin, C.c_void_p(radii.data_ptr()), C.c_void_p(depth_alpha.data_ptr()),
-                                               C.c_void_p(g_color.data_ptr()), C.c_void_p(g_da.data_ptr()),
-                                               C.c_void_p(ctx.saved_buf.data_ptr()), ctx.saved_buf.numel(), cap, out,
-                                               _lib.BWD_DETERMINISTIC if det else 0,
-                                               C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        if rc:
-            raise RuntimeError(f"b200gsr_backward_views failed ({rc}): {_lib.last_error()}")
+            ptr = _lib.ptr
+            rc = lib.b200gsr_backward_views_ex(B, prm, vin, ptr(radii), ptr(depth_alpha), ptr(g_color), ptr(g_da),
+                                               ptr(ctx.saved_buf), ctx.saved_buf.numel(), cap, out,
+                                               _lib.BWD_DETERMINISTIC if det else 0, _lib.stream(dev))
+        _lib.check(rc, "b200gsr_backward_views")
         return (None, None, None) + tuple(grads)
 
 

@@ -17,7 +17,6 @@ the two classes.
 from __future__ import annotations
 
 import contextlib
-import ctypes as C
 from typing import List, Tuple
 
 import torch
@@ -135,10 +134,9 @@ class GaussianAdam(torch.optim.Adam):
                                  *adam_scalars(lr, beta1, beta2, eps, step_t.item()))
                  for p, g, m, v, lr, beta1, beta2, eps, step_t in records]
         lib = _lib.load()
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        stream = _lib.stream(dev)
         with contextlib.nullcontext() if dev.index == torch.cuda.current_device() else torch.cuda.device(dev):
             for part in launches(table):
-                rc = lib.b200gsr_adam_step(len(part), (_lib.AdamTensor * len(part))(*part), stream)
-                if rc:
-                    raise RuntimeError(f"b200gsr_adam_step failed ({rc}): {_lib.last_error()}")
+                _lib.check(lib.b200gsr_adam_step(len(part), (_lib.AdamTensor * len(part))(*part), stream),
+                           "b200gsr_adam_step")
         return loss

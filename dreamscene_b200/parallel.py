@@ -122,13 +122,10 @@ def exchange_factored(flat: torch.Tensor, dcol: torch.Tensor, P: int, M: int, sh
     for w in works:
         w.wait()
     d_sh = torch.empty(P, M, 3, dtype=torch.float32, device=dcol.device)
-    import ctypes as C
     with torch.cuda.device(dcol.device):
-        rc = _lib.load().b200gsr_sh_grad_expand(
-            P, M, int(sh_degree), world, C.c_void_p(means3D.data_ptr()), C.c_void_p(gathered.data_ptr()),
-            dcol.numel(), C.c_void_p(d_sh.data_ptr()), C.c_void_p(torch.cuda.current_stream(dcol.device).cuda_stream))
-    if rc:
-        raise RuntimeError(f"b200gsr_sh_grad_expand failed ({rc}): {_lib.last_error()}")
+        rc = _lib.load().b200gsr_sh_grad_expand(P, M, int(sh_degree), world, _lib.ptr(means3D), _lib.ptr(gathered),
+                                                dcol.numel(), _lib.ptr(d_sh), _lib.stream(dcol.device))
+    _lib.check(rc, "b200gsr_sh_grad_expand")
     return d_sh
 
 

@@ -15,8 +15,6 @@ including the paths through min_d and disp.max().
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import torch
 
 from . import _lib
@@ -25,18 +23,16 @@ from . import _lib
 class _Disparity(torch.autograd.Function):
     @staticmethod
     def forward(ctx, depth_alpha, focal):
-        da = depth_alpha.detach().float().contiguous()
+        da = _lib.prepare(depth_alpha.detach())
         B, _, H, W = da.shape
         dev = da.device
         out = torch.empty(B, 1, H, W, device=dev)
         stats = torch.empty(B, 8, dtype=torch.int32, device=dev)
         lib = _lib.load()
         with torch.cuda.device(dev):
-            rc = lib.b200gsr_disparity_forward(B, H * W, C.c_void_p(da.data_ptr()), C.c_void_p(focal.data_ptr()),
-                                               C.c_void_p(out.data_ptr()), C.c_void_p(stats.data_ptr()),
-                                               C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        if rc:
-            raise RuntimeError(f"b200gsr_disparity_forward failed ({rc}): {_lib.last_error()}")
+            rc = lib.b200gsr_disparity_forward(B, H * W, _lib.ptr(da), _lib.ptr(focal), _lib.ptr(out), _lib.ptr(stats),
+                                               _lib.stream(dev))
+        _lib.check(rc, "b200gsr_disparity_forward")
         alpha = da[:, 1:2].clone()
         ctx.deterministic = torch.are_deterministic_algorithms_enabled()   # the backward runs in the forward's mode
         ctx.save_for_backward(da, focal, stats)
@@ -47,20 +43,16 @@ class _Disparity(torch.autograd.Function):
         da, focal, stats = ctx.saved_tensors
         B, _, H, W = da.shape
         dev = da.device
-        g_disp = torch.zeros(B, 1, H, W, device=dev) if g_disp is None else g_disp.float().contiguous()
-        g_alpha = None if g_alpha is None else g_alpha.float().contiguous()
+        g_disp = torch.zeros(B, 1, H, W, device=dev) if g_disp is None else _lib.prepare(g_disp)
+        g_alpha = _lib.prepare(g_alpha)
         d_da = torch.empty_like(da)
         st = stats.clone()          # the backward accumulates into the record: keep the forward's pristine
-        lib = _lib.load()
+        lib, ptr = _lib.load(), _lib.ptr
         with torch.cuda.device(dev):
-            rc = lib.b200gsr_disparity_backward_ex(B, H * W, C.c_void_p(da.data_ptr()), C.c_void_p(focal.data_ptr()),
-                                                   C.c_void_p(g_disp.data_ptr()),
-                                                   None if g_alpha is None else C.c_void_p(g_alpha.data_ptr()),
-                                                   C.c_void_p(st.data_ptr()), C.c_void_p(d_da.data_ptr()),
-                                                   _lib.BWD_DETERMINISTIC if ctx.deterministic else 0,
-                                                   C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        if rc:
-            raise RuntimeError(f"b200gsr_disparity_backward failed ({rc}): {_lib.last_error()}")
+            rc = lib.b200gsr_disparity_backward_ex(B, H * W, ptr(da), ptr(focal), ptr(g_disp), ptr(g_alpha), ptr(st),
+                                                   ptr(d_da), _lib.BWD_DETERMINISTIC if ctx.deterministic else 0,
+                                                   _lib.stream(dev))
+        _lib.check(rc, "b200gsr_disparity_backward")
         return d_da, None
 
 

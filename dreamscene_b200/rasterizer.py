@@ -230,11 +230,6 @@ def _round_cap(n: int) -> int:
     return max(_MIN_CAPACITY, (int(n) + g - 1) // g * g)
 
 
-def _resolve_pending(d: _Device, block: bool = False) -> None:
-    """Read the pair counts the device has reported so far (never waits unless `block`)."""
-    d.resolve(block)
-
-
 def flush_checks(device=None) -> None:
     """Wait for every forward issued so far to report its pair count (raises on overflow)."""
     want = None
@@ -243,30 +238,15 @@ def flush_checks(device=None) -> None:
         want = dv.index if dv.index is not None else torch.cuda.current_device()
     for idx, d in list(_devices.items()):
         if want is None or idx == want:
-            _resolve_pending(d, block=True)
+            d.resolve(block=True)
 
 
 def last_pair_count(device=None) -> int:
     """Pair count D of the most recent forward on the device (waits for it to be reported)."""
     dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
     d = _device_state(dev)
-    _resolve_pending(d, block=True)
+    d.resolve(block=True)
     return d.last_pairs
-
-
-def _ptr(t: Optional[torch.Tensor]):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _f32c(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
-    if t is None:
-        return None
-    if t.dtype != torch.float32:
-        t = t.float()
-    t = t.contiguous()
-    if t.data_ptr() % 16:          # the kernels use 16-byte vector loads on rows
-        t = t.clone()
-    return t
 
 
 def _const(t: torch.Tensor, dev) -> torch.Tensor:
@@ -276,13 +256,26 @@ def _const(t: torch.Tensor, dev) -> torch.Tensor:
     return t
 
 
-def _make_params(rs: GaussianRasterizationSettings, P: int, M: int, keep: list, dev) -> _lib.Params:
-    bg, vm, pm, cp = _const(rs.bg, dev), _const(rs.viewmatrix, dev), _const(rs.projmatrix, dev), _const(rs.campos, dev)
+def _make_params(rs: GaussianRasterizationSettings, P: int, M: int, keep: list, dev,
+                 bg: Optional[torch.Tensor], view: int = 0) -> _lib.Params:
+    """The b200gsr_params of one view: the settings `rs` for P Gaussians with M SH coefficients per channel, with row
+    `view` of the contiguous device float32 backgrounds `bg` [*, 3] (None for the score pass, which reads none).  The
+    device constants are appended to `keep`, which must outlive every call that uses the struct."""
+    vm, pm, cp = _const(rs.viewmatrix, dev), _const(rs.projmatrix, dev), _const(rs.campos, dev)
     keep.extend([bg, vm, pm, cp])
     return _lib.Params(P, M, int(rs.sh_degree), int(rs.image_height), int(rs.image_width),
                        float(rs.tanfovx), float(rs.tanfovy), float(rs.scale_modifier),
                        int(bool(rs.prefiltered)), int(bool(rs.score_flag)),
-                       bg.data_ptr(), vm.data_ptr(), pm.data_ptr(), cp.data_ptr())
+                       None if bg is None else bg.data_ptr() + 12 * view, vm.data_ptr(), pm.data_ptr(), cp.data_ptr())
+
+
+def _view_inputs(views) -> C.Array:
+    """The b200gsr_view_inputs array of B views: `views` holds, per view, its seven input tensors (or None) in the
+    struct's order (means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp)."""
+    arr = (_lib.ViewInputs * len(views))()
+    for v, ts in enumerate(views):
+        arr[v] = _lib.ViewInputs(*[None if t is None else t.data_ptr() for t in ts])
+    return arr
 
 
 class _State:
@@ -312,30 +305,39 @@ def deterministic_mode() -> bool:
     return torch.are_deterministic_algorithms_enabled()
 
 
+def _issue_once(d: _Device, layout, flags: int, cap: int, launch, stream_h, capturing: bool, what: str, bad_arg=None):
+    """Enqueue one forward of any kind at pair capacity `cap`: size its scratch and `saved` buffers for `layout` =
+    (P, H, W, with_backward, deterministic) of _layouts, claim a notify slot (none while capturing) and call
+    `launch(cap, flags, scratch, saved, notify_ptr, seq)`, which returns the C return code.  A failed launch releases
+    its slot and raises through _lib.check(rc, what, bad_arg).  -> (saved, slot, seq)."""
+    P, H, W, with_backward, deterministic = layout
+    scratch_bytes, saved_bytes = _layouts(P, H, W, cap, with_backward, deterministic)
+    scratch = d.ensure_scratch(stream_h, scratch_bytes)
+    saved = torch.empty(saved_bytes, dtype=torch.uint8, device=d.device)
+    slot, seq, notify_ptr = d.claim() if not capturing else (-1, 0, None)
+    rc = launch(cap, flags, scratch, saved, notify_ptr, seq)
+    if rc:
+        if slot >= 0:
+            d.release(slot)
+        _lib.check(rc, what, bad_arg)
+    return saved, slot, seq
+
+
 def _issue_with_capacity(d: _Device, key, P_eff: int, H_eff: int, W: int, with_backward: bool, deterministic: bool,
-                         score, launch, capturing: bool, stream_h: int):
-    """The single- and multi-view forwards' side of the pair-capacity protocol.  `launch(cap, scratch, saved,
-    notify_ptr, seq)` enqueues the whole forward and returns the C return code; this helper sizes the buffers,
-    decides whether to wait for the device's pair count (sync mode / unknown capacity) and re-issues on overflow,
-    with `score` zeroed.  `capturing` and `stream_h` (the current stream's handle) come from the caller.
-    -> (saved tensor, capacity)."""
+                         score, launch, capturing: bool, stream_h):
+    """The single- and multi-view forwards' side of the pair-capacity protocol.  `launch` enqueues the whole forward
+    (see _issue_once); this helper sizes the buffers, decides whether to wait for the device's pair count (sync mode /
+    unknown capacity) and re-issues on overflow, with `score` zeroed.  `capturing` and `stream_h` (the current stream's
+    handle, which keys the scratch buffer) come from the caller.  Misused inputs (B200GSR_ERR_BAD_ARG) raise a bare
+    Exception, as the reference's checks do.  -> (saved tensor, capacity)."""
     cap, known = d.capacity_for(key, P_eff, capturing)
+    layout = (P_eff, H_eff, W, with_backward, deterministic)
+    flags = (0 if with_backward else _lib.FWD_NO_BACKWARD) | (_lib.FWD_DETERMINISTIC if deterministic else 0)
     saved = None
 
     def issue(cap):
         nonlocal saved
-        scratch_bytes, saved_bytes = _layouts(P_eff, H_eff, W, cap, with_backward, deterministic)
-        scratch = d.ensure_scratch(stream_h, scratch_bytes)
-        saved = torch.empty(saved_bytes, dtype=torch.uint8, device=d.device)
-        slot, seq, notify_ptr = d.claim() if not capturing else (-1, 0, None)
-        rc = launch(cap, scratch, saved, notify_ptr, seq)
-        if rc:
-            if slot >= 0:
-                d.release(slot)
-            msg = _lib.last_error()
-            if rc == -1:
-                raise Exception(msg)
-            raise RuntimeError(f"b200gsr_forward failed ({rc}): {msg}")
+        saved, slot, seq = _issue_once(d, layout, flags, cap, launch, stream_h, capturing, "b200gsr_forward", Exception)
         return slot, seq
 
     def reissue(cap):
@@ -368,24 +370,24 @@ def _forward_impl(rs, means3D, shs, colors, opac, scales, rots, cov3d, with_back
     if not capturing:
         d.resolve()                       # non-blocking: may raise PairCapacityOverflow for an earlier call
     keep: list = []
+    ptr = _lib.ptr
     with torch.cuda.device(dev):          # the library launches on the CURRENT device; restored on exit
-        prm = _make_params(rs, P, M, keep, dev)
+        prm = _make_params(rs, P, M, keep, dev, _const(rs.bg, dev))
         color = torch.empty(3, H, W, dtype=torch.float32, device=dev)
         depth_alpha = torch.empty(2, H, W, dtype=torch.float32, device=dev)
         radii = torch.empty(P, dtype=torch.int32, device=dev)
         score = torch.zeros(P, dtype=torch.float32, device=dev) if rs.score_flag else None
-        stream_h = torch.cuda.current_stream(dev).cuda_stream
-        stream = C.c_void_p(stream_h)
+        stream = _lib.stream(dev)
         det = deterministic_mode()
-        flags = (0 if with_backward else _lib.FWD_NO_BACKWARD) | (_lib.FWD_DETERMINISTIC if det else 0)
 
-        def launch(cap, scratch, saved, notify_ptr, seq):
-            return lib.b200gsr_forward(C.byref(prm), _ptr(means3D), _ptr(shs), _ptr(colors), _ptr(opac),
-                                       _ptr(scales), _ptr(rots), _ptr(cov3d), _ptr(color), _ptr(depth_alpha),
-                                       _ptr(radii), _ptr(score), _ptr(scratch), scratch.numel(), _ptr(saved),
+        def launch(cap, flags, scratch, saved, notify_ptr, seq):
+            return lib.b200gsr_forward(C.byref(prm), ptr(means3D), ptr(shs), ptr(colors), ptr(opac),
+                                       ptr(scales), ptr(rots), ptr(cov3d), ptr(color), ptr(depth_alpha),
+                                       ptr(radii), ptr(score), ptr(scratch), scratch.numel(), ptr(saved),
                                        saved.numel(), cap, flags, notify_ptr, seq, stream)
 
-        saved, cap = _issue_with_capacity(d, (P, H, W), P, H, W, with_backward, det, score, launch, capturing, stream_h)
+        saved, cap = _issue_with_capacity(d, (P, H, W), P, H, W, with_backward, det, score, launch, capturing,
+                                          stream.value)
     st = _State()
     st.params_keep = keep; st.P = P; st.M = M; st.capacity = cap; st.saved = saved; st.rs = rs
     st.with_backward = with_backward
@@ -411,9 +413,10 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                 cov3Ds_precomp, raster_settings):
-        means3D = _f32c(means3D); sh = _f32c(sh); colors_precomp = _f32c(colors_precomp)
-        opacities = _f32c(opacities); scales = _f32c(scales); rotations = _f32c(rotations)
-        cov3Ds_precomp = _f32c(cov3Ds_precomp)
+        prep = _lib.prepare
+        means3D = prep(means3D); sh = prep(sh); colors_precomp = prep(colors_precomp)
+        opacities = prep(opacities); scales = prep(scales); rotations = prep(rotations)
+        cov3Ds_precomp = prep(cov3Ds_precomp)
         # under torch.no_grad() / with frozen inputs no backward can follow: skip the accumulators
         with_backward = any(ctx.needs_input_grad)
         color, radii, depth_alpha, score, st = _forward_impl(
@@ -448,8 +451,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         dev = means3D.device
         P, M = st.P, st.M
         H, W = int(rs.image_height), int(rs.image_width)
-        g_color = torch.zeros(3, H, W, device=dev) if g_color is None else _f32c(g_color)
-        g_da = torch.zeros(2, H, W, device=dev) if g_da is None else _f32c(g_da)
+        g_color = torch.zeros(3, H, W, device=dev) if g_color is None else _lib.prepare(g_color)
+        g_da = torch.zeros(2, H, W, device=dev) if g_da is None else _lib.prepare(g_da)
 
         # one flat buffer for every parameter gradient.  Under view sharding (dreamscene_b200.parallel,
         # mode "backward") it is all-reduced chunk by chunk while later chunks are still being computed,
@@ -487,22 +490,21 @@ class _RasterizeGaussians(torch.autograd.Function):
             if not st.with_backward:
                 raise RuntimeError("b200gsr: backward through a forward that ran without gradient accumulators")
             if not torch.cuda.is_current_stream_capturing():
-                _resolve_pending(_device_state(dev))      # non-blocking overflow check of earlier forwards
+                _device_state(dev).resolve()      # non-blocking overflow check of earlier forwards
             with torch.cuda.device(dev):
                 prm = st.prm
-                stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+                stream = _lib.stream(dev)
                 det_bit = _lib.BWD_DETERMINISTIC if st.deterministic else 0
+                ptr = _lib.ptr
 
                 def launch(stages, g0, g1):
-                    rc = lib.b200gsr_backward_ex(
-                        C.byref(prm), _ptr(means3D), _ptr(sh), _ptr(colors), _ptr(opacities), _ptr(scales),
-                        _ptr(rots), _ptr(cov3d), _ptr(radii), _ptr(depth_alpha), _ptr(g_color), _ptr(g_da),
-                        _ptr(st.saved), st.saved.numel(), None, 0, st.capacity,
-                        _ptr(d_means3D), _ptr(d_means2D), _ptr(d_sh), _ptr(d_colors), _ptr(d_opac),
-                        _ptr(d_scales), _ptr(d_rots), _ptr(d_cov), stages | det_bit, g0, g1,
-                        -1 if factored else (ncoef if compact else 0), stream)
-                    if rc:
-                        raise RuntimeError(f"b200gsr_backward failed ({rc}): {_lib.last_error()}")
+                    _lib.check(lib.b200gsr_backward_ex(
+                        C.byref(prm), ptr(means3D), ptr(sh), ptr(colors), ptr(opacities), ptr(scales),
+                        ptr(rots), ptr(cov3d), ptr(radii), ptr(depth_alpha), ptr(g_color), ptr(g_da),
+                        ptr(st.saved), st.saved.numel(), None, 0, st.capacity,
+                        ptr(d_means3D), ptr(d_means2D), ptr(d_sh), ptr(d_colors), ptr(d_opac),
+                        ptr(d_scales), ptr(d_rots), ptr(d_cov), stages | det_bit, g0, g1,
+                        -1 if factored else (ncoef if compact else 0), stream), "b200gsr_backward")
 
                 bounds = _parallel.chunk_bounds(P) if reduce else []
                 if not reduce:
@@ -544,15 +546,13 @@ class GaussianRasterizer(nn.Module):
         """Frustum (near-plane) visibility mask; unused by DreamScene, kept for API parity."""
         rs = self.raster_settings
         with torch.no_grad():
-            pos = _f32c(positions)
+            pos = _lib.prepare(positions)
             vis = torch.empty(pos.shape[0], dtype=torch.uint8, device=pos.device)
             vm, pm = _const(rs.viewmatrix, pos.device), _const(rs.projmatrix, pos.device)
             with torch.cuda.device(pos.device):
-                rc = _lib.load().b200gsr_mark_visible(
-                    int(pos.shape[0]), _ptr(pos), _ptr(vm), _ptr(pm), _ptr(vis),
-                    C.c_void_p(torch.cuda.current_stream(pos.device).cuda_stream))
-            if rc:
-                raise RuntimeError(f"b200gsr_mark_visible failed ({rc}): {_lib.last_error()}")
+                rc = _lib.load().b200gsr_mark_visible(int(pos.shape[0]), _lib.ptr(pos), _lib.ptr(vm), _lib.ptr(pm),
+                                                      _lib.ptr(vis), _lib.stream(pos.device))
+            _lib.check(rc, "b200gsr_mark_visible")
         return vis.bool()
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None,

@@ -29,7 +29,6 @@ Noise modes
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Sequence
 
 import torch
@@ -44,16 +43,6 @@ def _get(group, name):
     return group[name] if isinstance(group, dict) else getattr(group, name)
 
 
-def _prep(t: torch.Tensor) -> torch.Tensor:
-    t = t.detach()
-    if t.dtype != torch.float32:
-        t = t.float()
-    t = t.contiguous()
-    if t.data_ptr() % 16:
-        t = t.clone()
-    return t
-
-
 def _group_table(raw: Sequence[Sequence[torch.Tensor]]):
     arr = (_lib.Group * len(raw))()
     for k, ts in enumerate(raw):
@@ -66,19 +55,16 @@ def _group_table(raw: Sequence[Sequence[torch.Tensor]]):
 class _Assemble(torch.autograd.Function):
     @staticmethod
     def forward(ctx, num_groups, M, B, c_shs, c_scale, z_shs, z_scales, seed, *flat):
-        raw = [[_prep(t) for t in flat[6 * k:6 * k + 6]] for k in range(num_groups)]
+        raw = [[_lib.prepare(t.detach()) for t in flat[6 * k:6 * k + 6]] for k in range(num_groups)]
         dev = raw[0][0].device
         P = sum(int(ts[0].shape[0]) for ts in raw)
         out = [torch.empty(P, 3, device=dev), torch.empty(P, 1, device=dev), torch.empty(B, P, 3, device=dev),
                torch.empty(P, 4, device=dev), torch.empty(B, P, M, 3, device=dev)]
-        lib = _lib.load()
-        ptr = lambda t: None if t is None else C.c_void_p(t.data_ptr())
+        lib, ptr = _lib.load(), _lib.ptr
         with torch.cuda.device(dev):
             rc = lib.b200gsr_assemble_forward(num_groups, _group_table(raw), M, B, c_shs, c_scale, ptr(z_shs), ptr(z_scales),
-                                              seed, *[ptr(o) for o in out],
-                                              C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        if rc:
-            raise RuntimeError(f"b200gsr_assemble_forward failed ({rc}): {_lib.last_error()}")
+                                              seed, *[ptr(o) for o in out], _lib.stream(dev))
+        _lib.check(rc, "b200gsr_assemble_forward")
         ctx.meta = (num_groups, M, B, c_shs, c_scale, seed)
         ctx.noise = (z_shs, z_scales)
         ctx.save_for_backward(*[t for ts in raw for t in ts])
@@ -93,20 +79,18 @@ class _Assemble(torch.autograd.Function):
         dev = raw[0][0].device
         P = sum(int(ts[0].shape[0]) for ts in raw)
         shapes = [(P, 3), (P, 1), (B, P, 3), (P, 4), (B, P, M, 3)]
-        gin = [torch.zeros(s, device=dev) if g is None else _prep(g) for g, s in zip((g_means, g_opac, g_scales, g_rots, g_shs), shapes)]
+        gin = [torch.zeros(s, device=dev) if g is None else _lib.prepare(g.detach())
+               for g, s in zip((g_means, g_opac, g_scales, g_rots, g_shs), shapes)]
         grads = [[torch.empty_like(t) for t in ts] for ts in raw]
         garr = (_lib.GroupGrad * num_groups)()
         for k, ts in enumerate(grads):
             for name, t in zip(("xyz", "opacity", "scaling", "rotation", "f_dc", "f_rest"), ts):
                 setattr(garr[k], name, t.data_ptr() if t.numel() else None)
-        lib = _lib.load()
-        ptr = lambda t: None if t is None else C.c_void_p(t.data_ptr())
+        lib, ptr = _lib.load(), _lib.ptr
         with torch.cuda.device(dev):
             rc = lib.b200gsr_assemble_backward(num_groups, _group_table(raw), garr, M, B, c_shs, c_scale, ptr(z_shs),
-                                               ptr(z_scales), seed, *[ptr(g) for g in gin],
-                                               C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        if rc:
-            raise RuntimeError(f"b200gsr_assemble_backward failed ({rc}): {_lib.last_error()}")
+                                               ptr(z_scales), seed, *[ptr(g) for g in gin], _lib.stream(dev))
+        _lib.check(rc, "b200gsr_assemble_backward")
         return (None,) * 8 + tuple(t for ts in grads for t in ts)
 
 
@@ -146,8 +130,8 @@ def assemble_scene(groups: Sequence, shs_aug: bool = True, scale_aug: bool = Tru
             z_shs = zs[0] if B == 1 else torch.stack(zs)
         if zc:
             z_scales = zc[0] if B == 1 else torch.stack(zc)
-        z_shs = _prep(z_shs) if shs_aug else None
-        z_scales = _prep(z_scales) if scale_aug else None
+        z_shs = _lib.prepare(z_shs.detach()) if shs_aug else None
+        z_scales = _lib.prepare(z_scales.detach()) if scale_aug else None
         if (z_shs is not None and z_shs.numel() != B * P * M * 3) or (z_scales is not None and z_scales.numel() != B * P * 3):
             raise ValueError("noise tensors must hold one draw per view and element")
         seed = 0

@@ -118,15 +118,15 @@ def test_deferred_overflow_check_reads_the_notify_ring_without_blocking():
     d.free_slots = list(range(R._NOTIFY_SLOTS - 1, -1, -1))
     s1, s2 = d.free_slots.pop(), d.free_slots.pop()
     d.pending = [(s1, 11, 1 << 20, (5, 16, 16)), (s2, 12, 1 << 20, (5, 16, 16))]
-    R._resolve_pending(d)                       # nothing reported yet: stays pending, no wait
+    d.resolve()                                 # nothing reported yet: stays pending, no wait
     assert len(d.pending) == 2
     d.notify_np[s1] = (11, 500_000, 0, 64)      # first forward reports 0.5M pairs
-    R._resolve_pending(d)
+    d.resolve()
     assert d.pending == [(s2, 12, 1 << 20, (5, 16, 16))] and d.last_pairs == 500_000 and s1 in d.free_slots
     assert d.capacity == R._round_cap(1_000_000) and d.caps[(5, 16, 16)] == R._round_cap(1_000_000)
     d.notify_np[s2] = (12, 3 << 20, 1, 64)      # second one overflowed its 1M-pair buffer
     with pytest.raises(R.PairCapacityOverflow):
-        R._resolve_pending(d)
+        d.resolve()
     assert not d.pending and d.capacity >= 6 << 20      # raised so that a retry fits
 
 
@@ -142,8 +142,8 @@ def _fake_device():
     calls = []
 
     def launch_with(pairs):
-        def launch(cap, scratch, saved, notify_ptr, seq):
-            calls.append((cap, saved.numel()))
+        def launch(cap, flags, scratch, saved, notify_ptr, seq):
+            calls.append((cap, saved.numel(), flags))
             if notify_ptr is not None:
                 d.notify_np[(notify_ptr.value - d.notify.data_ptr()) // 16, :2] = (seq, pairs)
             return 0
@@ -161,7 +161,7 @@ def test_sync_overflow_reissues_with_room_for_the_count_and_zeroes_the_score():
     R.set_pair_count_mode("sync")
     try:
         saved, cap = R._issue_with_capacity(d, (8, 64, 64), 8, 64, 64, True, False, score, launch_with(pairs), False, 0)
-        assert [c for c, _ in calls] == [R._round_cap(1 << 20), R._round_cap(2 * pairs)]
+        assert [c for c, _, _ in calls] == [R._round_cap(1 << 20), R._round_cap(2 * pairs)]
         assert cap == R._round_cap(2 * pairs) and saved.numel() == _lib.saved_layout(8, 64, 64, cap).total
         assert torch.equal(score, torch.zeros(8))              # the overflowed issue's partial score is dropped
         assert d.capacity == cap and d.caps == {} and d.last_pairs == pairs and not d.pending
@@ -189,6 +189,18 @@ def test_first_forward_of_a_shape_is_measured_then_later_ones_are_deferred():
                                True, 0)
 
 
+def test_forward_flags_and_saved_size_follow_with_backward_and_deterministic():
+    """_issue_with_capacity derives the forward flags and the `saved` layout from the same two arguments."""
+    from dreamscene_b200 import _lib, rasterizer as R
+    for with_backward in (True, False):
+        for det in (False, True):
+            d, calls, launch_with = _fake_device()
+            _, cap = R._issue_with_capacity(d, (100, 64, 64), 100, 64, 64, with_backward, det, None, launch_with(10),
+                                            False, 0)
+            want = (0 if with_backward else _lib.FWD_NO_BACKWARD) | (_lib.FWD_DETERMINISTIC if det else 0)
+            assert calls == [(cap, _lib.saved_layout(100, 64, 64, cap, with_backward, det).total, want)]
+
+
 def test_score_pass_settle_reissues_without_touching_the_accumulator():
     """The score pass adds into an accumulator that holds the earlier passes' sums; an overflowed pass adds nothing,
     so settling re-issues it as it is."""
@@ -204,12 +216,12 @@ def test_score_pass_settle_reissues_without_touching_the_accumulator():
 
     def issue(c):
         slot, seq, ptr = d.claim()
-        launch(c, torch.empty(0), torch.empty(0), ptr, seq)
+        launch(c, 0, torch.empty(0), torch.empty(0), ptr, seq)
         return slot, seq
 
     slot, seq = issue(cap)
     got = d.settle(key, cap, slot, seq, issue)
-    assert got == R._round_cap(2 * pairs) and [c for c, _ in calls] == [cap, got]
+    assert got == R._round_cap(2 * pairs) and [c for c, _, _ in calls] == [cap, got]
     assert torch.equal(acc, torch.full((4,), 7.0)) and d.capacity == got and d.caps == {}
 
 
