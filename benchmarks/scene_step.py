@@ -8,6 +8,7 @@ restated here: per view  torch.cat(env, floor, objects) -> SH/scale augmentation
 depth/alpha post-processing; 4 views per step (C_batch_size, config.py:163); one backward.
 
   python benchmarks/scene_step.py [--steps 10] [--views 4] [--size 512] [--optim none|torch|native]
+                                  [--glue torch|fused|fused_rng|views|scene]
 Prints a JSON line with the step time and the share spent inside the rasterizer.  --optim adds the optimizer step
 after the backward, one Adam per GaussianModel as the reference builds it: torch.optim.Adam's default path or
 dreamscene_b200.GaussianAdam (default none: no optimizer step, as before).
@@ -26,7 +27,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from dreamscene_b200 import GaussianRasterizationSettings, GaussianRasterizer  # noqa: E402
 from dreamscene_b200.multiview import rasterize_views  # noqa: E402
 from dreamscene_b200.postprocess import disparity_from_depth_alpha  # noqa: E402
-from dreamscene_b200.scene import assemble_scene  # noqa: E402
+from dreamscene_b200.scene import assemble_scene, render_scene  # noqa: E402
 from harness import cameras  # noqa: E402
 from harness.scene_ref import reference_assemble  # noqa: E402
 
@@ -123,21 +124,29 @@ def render(groups, cam, dev, bg, aug=True, glue="torch"):
     return dict(image=image, depth=disp, alpha=alpha, radii=radii, viewspace=screenspace, ev=(t0, t1))
 
 
-def render_views(groups, cams, dev, bg, aug=True):
+def render_views(groups, cams, dev, bg, aug=True, scene=False):
     """All views of the step in one rasterizer pass (dreamscene_b200.multiview): per-view augmented shs / scales
-    (in-kernel Philox noise), shared positions / opacities / rotations, batched fused disparity."""
+    (in-kernel Philox noise), shared positions / opacities / rotations, batched fused disparity.  scene=True:
+    dreamscene_b200.scene.render_scene renders them straight from the raw groups (the activations and the
+    augmentation happen inside the projection kernels; the rasterizer time then includes them)."""
     named = [{"_xyz": g["xyz"], "_opacity": g["opacity"], "_scaling": g["scaling"], "_rotation": g["rotation"],
               "_features_dc": g["f_dc"], "_features_rest": g["f_rest"]} for g in groups]
-    xyz, opacity, scales_v, rots, shs_v = assemble_scene(named, shs_aug=aug, scale_aug=aug, noise="fused", views=len(cams))
+    if not scene:
+        xyz, opacity, scales_v, rots, shs_v = assemble_scene(named, shs_aug=aug, scale_aug=aug, noise="fused",
+                                                             views=len(cams))
     S = [GaussianRasterizationSettings(
         image_height=c.image_height, image_width=c.image_width, tanfovx=c.tanfovx, tanfovy=c.tanfovy, bg=bg,
         scale_modifier=1.0, viewmatrix=c.world_view_transform, projmatrix=c.full_proj_transform, sh_degree=1,
         campos=c.camera_center, prefiltered=False, score_flag=False) for c in cams]
-    screens = [torch.zeros_like(xyz, requires_grad=True) for _ in cams]
+    P = sum(int(g["xyz"].shape[0]) for g in groups)
+    screens = [torch.zeros(P, 3, device=dev, requires_grad=True) for _ in cams]
     t0 = torch.cuda.Event(enable_timing=True); t1 = torch.cuda.Event(enable_timing=True)
     t0.record()
-    outs = rasterize_views(S, xyz, opacity, shs=list(shs_v.unbind(0)), scales=list(scales_v.unbind(0)), rotations=rots,
-                           means2D=screens)
+    if scene:
+        outs = render_scene(named, S, shs_aug=aug, scale_aug=aug, means2D=screens)
+    else:
+        outs = rasterize_views(S, xyz, opacity, shs=list(shs_v.unbind(0)), scales=list(scales_v.unbind(0)),
+                               rotations=rots, means2D=screens)
     t1.record()
     da = torch.stack([o[2] for o in outs])                                  # [B,2,H,W]
     focals = [1 / (2 * math.tan(c.FoVx / 2)) for c in cams]
@@ -152,7 +161,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--views", type=int, default=4)
     ap.add_argument("--size", type=int, default=512)
-    ap.add_argument("--glue", default="torch", choices=["torch", "fused", "fused_rng", "views"])
+    ap.add_argument("--glue", default="torch", choices=["torch", "fused", "fused_rng", "views", "scene"])
     ap.add_argument("--optim", default="none", choices=["none", "torch", "native"])
     a = ap.parse_args()
     dev = torch.device("cuda", 0)
@@ -178,7 +187,7 @@ def main():
             p.grad = None
         torch.cuda.synchronize(); t0 = time.perf_counter()
         cams = all_cams[it]
-        outs = render_views(groups, cams, dev, bg) if a.glue == "views" else [render(groups, c, dev, bg, glue=a.glue) for c in cams]
+        outs = render_views(groups, cams, dev, bg, scene=a.glue == "scene") if a.glue in ("views", "scene") else [render(groups, c, dev, bg, glue=a.glue) for c in cams]
         images = torch.stack([o["image"] for o in outs]); depths = torch.stack([o["depth"] for o in outs])
         loss = ((images - target) ** 2).mean() * 100 + depths.mean() * 0.1      # SDS -> L2 stub (+ depth path)
         loss.backward()
@@ -196,7 +205,7 @@ def main():
         for p in params:
             p.grad = None
         cams = all_cams[it]
-        outs = render_views(groups, cams, dev, bg) if a.glue == "views" else [render(groups, c, dev, bg, glue=a.glue) for c in cams]
+        outs = render_views(groups, cams, dev, bg, scene=a.glue == "scene") if a.glue in ("views", "scene") else [render(groups, c, dev, bg, glue=a.glue) for c in cams]
         images = torch.stack([o["image"] for o in outs]); depths = torch.stack([o["depth"] for o in outs])
         (((images - target) ** 2).mean() * 100 + depths.mean() * 0.1).backward()
         for o in opts:

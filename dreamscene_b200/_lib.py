@@ -1,4 +1,4 @@
-"""ctypes binding of libb200gsr.so (include/b200gsr.h).  Fails loudly if the library is missing:
+"""ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h).  Fails loudly if the library is missing:
 there is NO CPU or PyTorch fallback in the product path."""
 from __future__ import annotations
 
@@ -106,6 +106,14 @@ SIGNATURES = {
 }
 EXPORTS = list(SIGNATURES)
 
+# The scene-render entry points of include/b200gsr_scene.h (same library), in that header's order.
+SCENE_SIGNATURES = {
+    "b200gsr_forward_scene": (C.c_int, [i32, _P(Params), i32, _P(Group), vp, vp, u64] + [vp] * 5 +
+                              [sz, vp, sz, u64, u32, vp, u32, vp]),
+    "b200gsr_backward_scene": (C.c_int, [i32, _P(Params), i32, _P(Group), _P(GroupGrad), vp, vp, u64] + [vp] * 6 +
+                               [sz, u64, vp, u32, vp]),
+}
+
 _lib = None
 ABI_VERSION = 3
 ERR_BAD_ARG = -1
@@ -134,7 +142,7 @@ def load():
                 f"{LIB_PATH} is missing and could not be built ({err}). Build it with "
                 "`python -m dreamscene_b200._build` (needs nvcc; sm_90a only). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in SIGNATURES.items():
+    for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:

@@ -1,5 +1,6 @@
-// C ABI (include/b200gsr.h): argument validation, buffer layouts, launch sequencing.
+// C ABI (include/b200gsr.h, include/b200gsr_scene.h): argument validation, buffer layouts, launch sequencing.
 #include "common.cuh"
+#include "../../include/b200gsr_scene.h"
 
 #include <cstdarg>
 #include <cstdio>
@@ -160,7 +161,9 @@ int check_det_size(int32_t H, int32_t W) {
 //   kViews  b200gsr_forward_views: the layouts describe the stacked image (even for B = 1); no profiling events.
 //   kScore  b200gsr_score_views: stacked; geometry-only projection and score-only compositing into the caller's
 //           accumulator, which holds the deterministic sum itself, so `saved` carries no deterministic state.
-enum class Pass { kImage, kViews, kScore };
+//   kScene  b200gsr_forward_scene: stacked; the projection reads the raw leaves of `scene` (in == null); records the
+//           profiling events.
+enum class Pass { kImage, kViews, kScore, kScene };
 
 // Everything a forward does after its entry point's validation, for B views stacked vertically.  Every size and
 // workspace refusal comes before device_state(), the first CUDA call.  `score` is the float [B*P] score of a
@@ -168,7 +171,7 @@ enum class Pass { kImage, kViews, kScore };
 int run_forward(Pass pass, int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, float* out_color,
                 float* out_depth_alpha, int32_t* radii, void* score, void* scratch, size_t scratch_bytes, void* saved,
                 size_t saved_bytes, uint64_t max_pairs, uint32_t flags, uint32_t* host_notify, uint32_t notify_seq,
-                void* stream) {
+                void* stream, const GsrScene* scene = nullptr) {
     const bool score_pass = pass == Pass::kScore;
     const int P = prm[0].P, H = prm[0].image_height, W = prm[0].image_width;
     const GsrTileGrid g1 = gsr_grid(H, W);
@@ -198,6 +201,7 @@ int run_forward(Pass pass, int32_t B, const b200gsr_params* prm, const b200gsr_v
     a.flags = flags; a.num_sms = ds->num_sms; a.stats = score_pass ? nullptr : g_stats;
     a.num_views = B; a.P_view = P; a.gy_view = g1.gy;
     a.stream = static_cast<cudaStream_t>(stream);
+    a.scene = scene;
     const bool profile = pass != Pass::kViews;
 
     // The counters at the start of scratch must be zero before the count kernel runs.  On the main path
@@ -212,8 +216,10 @@ int run_forward(Pass pass, int32_t B, const b200gsr_params* prm, const b200gsr_v
     GSR_RANGE_PUSH("b200gsr.project+count");
     for (int v = 0; v < B && !rc; ++v) {
         a.prm = prm[v]; a.view = v;
-        a.means3D = in[v].means3D; a.shs = in[v].shs; a.colors = in[v].colors_precomp; a.opac = in[v].opacities;
-        a.scales = in[v].scales; a.rots = in[v].rotations; a.cov3d = in[v].cov3D_precomp;
+        if (in) {
+            a.means3D = in[v].means3D; a.shs = in[v].shs; a.colors = in[v].colors_precomp; a.opac = in[v].opacities;
+            a.scales = in[v].scales; a.rots = in[v].rotations; a.cov3d = in[v].cov3D_precomp;
+        }
         rc = check_cuda(gsr_launch_project(a, score_pass), score_pass ? "project_geo" : "project_sh");
     }
     a.prm = prm[0]; a.view = 0;     // per-view constants are not used past this point (bg is indexed by tile row)
@@ -751,6 +757,97 @@ int b200gsr_sh_grad_expand(int32_t P, int32_t M, int32_t sh_degree, int32_t num_
         return fail(B200GSR_ERR_BAD_ARG, "bad sh_grad_expand arguments");
     return check_cuda(gsr_launch_sh_grad_expand(P, M, sh_degree, num_views, means3D, dcol, view_stride, d_shs,
                                                 static_cast<cudaStream_t>(stream)), "sh_grad_expand");
+}
+
+// ---------------------------------------------------------------------------------------------
+// Scene renders (include/b200gsr_scene.h): the views of a training step rendered straight from the raw parameter
+// groups.  The forward is run_forward's kScene pass; the backward is the multi-view backward with the raw-leaf
+// mode of project_bwd, views in order.
+// ---------------------------------------------------------------------------------------------
+static int check_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
+                       const float* shs_noise, const float* scale_noise) {
+    if (B < 1 || B > B200GSR_MAX_VIEWS) return fail(B200GSR_ERR_UNSUPPORTED, "number of views %d not in 1..%d", B, B200GSR_MAX_VIEWS);
+    if (!prm) return fail(B200GSR_ERR_BAD_ARG, "null view array");
+    if (!shs_noise || !scale_noise) return fail(B200GSR_ERR_BAD_ARG, "shs_noise / scale_noise must be host arrays of B coefficients");
+    int rc = check_groups(num_groups, groups, prm[0].M);
+    if (rc) return rc;
+    long long total = 0;
+    for (int g = 0; g < num_groups; ++g) total += groups[g].n;
+    for (int v = 0; v < B; ++v) {
+        const b200gsr_params& p = prm[v];
+        if ((rc = check_size(p, v))) return rc;
+        if (!p.bg || !p.viewmatrix || !p.projmatrix || !p.campos)
+            return fail(B200GSR_ERR_BAD_ARG, "view %d: bg/viewmatrix/projmatrix/campos must be device pointers", v);
+        if (p.P != total) return fail(B200GSR_ERR_BAD_ARG, "view %d: P = %d but the groups hold %lld rows", v, p.P, total);
+        if (p.M != prm[0].M || p.image_height != prm[0].image_height || p.image_width != prm[0].image_width)
+            return fail(B200GSR_ERR_BAD_ARG, "view %d: M and image size must equal view 0's", v);
+        if (p.score_flag) return fail(B200GSR_ERR_UNSUPPORTED, "view %d: score_flag is not supported by the scene render", v);
+        if (p.bg != prm[0].bg + 3 * v)
+            return fail(B200GSR_ERR_BAD_ARG, "view %d: backgrounds must be one contiguous device array [B,3] (prm[v].bg = prm[0].bg + 3 v)", v);
+        if (p.sh_degree < 0 || p.sh_degree > 3) return fail(B200GSR_ERR_UNSUPPORTED, "view %d: sh_degree %d not in 0..3", v, p.sh_degree);
+        if (p.M < (p.sh_degree + 1) * (p.sh_degree + 1))
+            return fail(B200GSR_ERR_BAD_ARG, "view %d: M=%d inconsistent with sh_degree=%d (need (deg+1)^2 <= M)", v, p.M, p.sh_degree);
+    }
+    if ((long long)B * total > 0x3fffffffLL) return fail(B200GSR_ERR_UNSUPPORTED, "B * P too large");
+    return B200GSR_OK;
+}
+
+int b200gsr_forward_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
+                          const float* shs_noise, const float* scale_noise, uint64_t seed, float* out_scales,
+                          float* out_color, float* out_depth_alpha, int32_t* radii, void* scratch, size_t scratch_bytes,
+                          void* saved, size_t saved_bytes, uint64_t max_pairs, uint32_t flags, uint32_t* host_notify,
+                          uint32_t notify_seq, void* stream) {
+    int rc = check_scene(B, prm, num_groups, groups, shs_noise, scale_noise);
+    if (rc) return rc;
+    if (flags & ~(B200GSR_FWD_NO_BACKWARD | B200GSR_FWD_DETERMINISTIC)) return fail(B200GSR_ERR_BAD_ARG, "unknown flags 0x%x", flags);
+    if (!out_color || !out_depth_alpha || (prm[0].P > 0 && !radii) || !scratch || !saved)
+        return fail(B200GSR_ERR_BAD_ARG, "null output/workspace pointer");
+    const GsrScene sc = {num_groups, groups, nullptr, shs_noise, scale_noise, seed, out_scales, nullptr};
+    return run_forward(Pass::kScene, B, prm, nullptr, out_color, out_depth_alpha, radii, nullptr, scratch, scratch_bytes,
+                       saved, saved_bytes, max_pairs, flags, host_notify, notify_seq, stream, &sc);
+}
+
+int b200gsr_backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
+                           const b200gsr_group_grad* grads, const float* shs_noise, const float* scale_noise,
+                           uint64_t seed, const float* d_scales, const int32_t* radii, const float* out_depth_alpha,
+                           const float* dL_dcolor, const float* dL_ddepth_alpha, void* saved, size_t saved_bytes,
+                           uint64_t max_pairs, float* d_means2D, uint32_t flags, void* stream) {
+    int rc = check_scene(B, prm, num_groups, groups, shs_noise, scale_noise);
+    if (rc) return rc;
+    if (flags & ~B200GSR_BWD_DETERMINISTIC) return fail(B200GSR_ERR_BAD_ARG, "unknown flags 0x%x", flags);
+    if (num_groups > 0 && !grads) return fail(B200GSR_ERR_BAD_ARG, "grads is null");
+    for (int g = 0; g < num_groups; ++g)
+        if (groups[g].n > 0 && (!grads[g].xyz || !grads[g].opacity || !grads[g].scaling || !grads[g].rotation ||
+                                !grads[g].f_dc || (prm[0].M > 1 && !grads[g].f_rest)))
+            return fail(B200GSR_ERR_BAD_ARG, "group %d: null gradient pointer", g);
+    const int P = prm[0].P;
+    if (P == 0) return B200GSR_OK;
+    if (!radii || !out_depth_alpha || !dL_dcolor || !dL_ddepth_alpha || !saved || !d_means2D)
+        return fail(B200GSR_ERR_BAD_ARG, "null saved-state/gradient pointer");
+    GsrBwdArgs a;
+    if ((rc = setup_backward(true, B, prm, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes,
+                             max_pairs, (flags & B200GSR_BWD_DETERMINISTIC) != 0, stream, a)))
+        return rc;
+    const GsrScene sc = {num_groups, groups, grads, shs_noise, scale_noise, seed, nullptr, d_scales};
+    a.scene = &sc;
+    a.g_begin = 0; a.g_end = P;
+    prof_mark_bwd(0, a.stream);
+    GSR_RANGE_PUSH("b200gsr.scene.composite_bwd");
+    rc = check_cuda(gsr_launch_composite_bwd(a), "composite_bwd");
+    GSR_RANGE_POP();
+    if (rc) return rc;
+    prof_mark_bwd(1, a.stream);
+    GSR_RANGE_PUSH("b200gsr.scene.project_bwd");
+    for (int v = 0; v < B && !rc; ++v) {      // in view order: view 0 writes the leaf gradients, later views add
+        a.prm = prm[v]; a.view = v;
+        a.d_means2D = d_means2D + 3 * (size_t)P * v;
+        rc = check_cuda(gsr_launch_project_bwd(a), "project_bwd");
+    }
+    GSR_RANGE_POP();
+    if (rc) return rc;
+    prof_mark_bwd(2, a.stream);
+    if (g_prof.max_calls > 0 && g_prof.nbwd < g_prof.max_calls) ++g_prof.nbwd;
+    return B200GSR_OK;
 }
 
 int b200gsr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix,

@@ -20,72 +20,9 @@
 // torch.randn in the reference's order and the random stream matches the reference's), or - z == NULL
 // and seed given - a counter-based Philox4x32-10 generator evaluated in the kernel (no noise tensor
 // is ever written or read; the backward regenerates the same numbers from (seed, element index)).
-#include "common.cuh"
-#include <cstring>
+#include "scene_math.cuh"
 
 namespace {
-
-constexpr int kMaxGroups = B200GSR_MAX_GROUPS;
-
-struct GroupTable {
-    const float* xyz[kMaxGroups];
-    const float* opacity[kMaxGroups];
-    const float* scaling[kMaxGroups];
-    const float* rotation[kMaxGroups];
-    const float* f_dc[kMaxGroups];
-    const float* f_rest[kMaxGroups];
-    int start[kMaxGroups + 1];     // first packed row of group g; start[num] = P
-    int num;
-};
-struct GroupGradTable {
-    float* xyz[kMaxGroups];
-    float* opacity[kMaxGroups];
-    float* scaling[kMaxGroups];
-    float* rotation[kMaxGroups];
-    float* f_dc[kMaxGroups];
-    float* f_rest[kMaxGroups];
-};
-
-__device__ __forceinline__ int find_group(const GroupTable& t, int row) {
-    int g = 0;
-#pragma unroll 1
-    while (g + 1 < t.num && row >= t.start[g + 1]) ++g;
-    return g;
-}
-
-// ---- Philox4x32-10 (Salmon et al. 2011), counter = (lo, hi, stream, 0), key = seed ------------
-__device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
-    constexpr uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        const uint32_t hi0 = __umulhi(M0, ctr.x), lo0 = M0 * ctr.x;
-        const uint32_t hi1 = __umulhi(M1, ctr.z), lo1 = M1 * ctr.z;
-        ctr = make_uint4(hi1 ^ ctr.y ^ key.x, lo1, hi0 ^ ctr.w ^ key.y, lo0);
-        key.x += W0; key.y += W1;
-    }
-    return ctr;
-}
-// four standard normals for quad index q of stream s (Box-Muller on the four 32-bit outputs)
-__device__ __forceinline__ float4 normal4(unsigned long long seed, uint32_t stream, unsigned long long q) {
-    const uint4 r = philox4x32_10(make_uint4((uint32_t)q, (uint32_t)(q >> 32), stream, 0u),
-                                  make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
-    const float u0 = ((float)r.x + 0.5f) * 2.3283064365386963e-10f;   // (0, 1)
-    const float u1 = ((float)r.y + 0.5f) * 2.3283064365386963e-10f;
-    const float u2 = ((float)r.z + 0.5f) * 2.3283064365386963e-10f;
-    const float u3 = ((float)r.w + 0.5f) * 2.3283064365386963e-10f;
-    const float ra = sqrtf(-2.0f * __logf(u0)), rb = sqrtf(-2.0f * __logf(u2));
-    float s0, c0, s1, c1;
-    __sincosf(6.283185307179586f * u1, &s0, &c0);
-    __sincosf(6.283185307179586f * u3, &s1, &c1);
-    return make_float4(ra * c0, ra * s0, rb * c1, rb * s1);
-}
-enum { kStreamShs = 1u, kStreamScales = 2u };    // + 2 * view
-
-// noise factor helpers: value v, standard normal z, coefficient c (0.2**0.5), divisor d (1 or 4):
-// reference order  v + z * ((c * v) / d)
-__device__ __forceinline__ float aug(float v, float z, float c, float d) {
-    return __fadd_rn(v, __fmul_rn(z, __fdiv_rn(__fmul_rn(c, v), d)));
-}
 
 constexpr int kAsmBlock = 128;
 
@@ -113,9 +50,9 @@ assemble_kernel(GroupTable tab, GroupGradTable gtab, int P, int M, int B, float 
         const float sx = tab.scaling[g][3 * (size_t)l], sy = tab.scaling[g][3 * (size_t)l + 1], sz = tab.scaling[g][3 * (size_t)l + 2];
         const float4 q = *reinterpret_cast<const float4*>(tab.rotation[g] + 4 * (size_t)l);
         const float o = tab.opacity[g][l];
-        const float e[3] = {expf(sx), expf(sy), expf(sz)};
-        const float sig = __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-o)));
-        const float nrm = fmaxf(sqrtf(__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(q.x, q.x), __fmul_rn(q.y, q.y)), __fmul_rn(q.z, q.z)), __fmul_rn(q.w, q.w))), 1e-12f);
+        const float e[3] = {act_scale(sx), act_scale(sy), act_scale(sz)};
+        const float sig = act_opacity(o);
+        const float nrm = quat_norm(q);
         float dsum[3] = {0.f, 0.f, 0.f};
         for (int v = 0; v < B; ++v) {
             float zs[3] = {0.f, 0.f, 0.f};
@@ -132,14 +69,10 @@ assemble_kernel(GroupTable tab, GroupGradTable gtab, int P, int M, int B, float 
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
                 if (!BACKWARD) {
-                    sv[k] = (c_scale != 0.0f) ? fmaxf(aug(e[k], zs[k], c_scale, 4.0f), 0.0f) : e[k];
+                    sv[k] = (c_scale != 0.0f) ? aug_scale(e[k], zs[k], c_scale) : e[k];
                 } else {
                     float d = sv[k];
-                    if (c_scale != 0.0f) {
-                        // y = clamp(e + z*((c*e)/4), 0): dy/de = 1 + z*c/4 where the clamp is inactive
-                        const float y = aug(e[k], zs[k], c_scale, 4.0f);
-                        d = (y > 0.0f) ? d * (1.0f + zs[k] * (c_scale * 0.25f)) : 0.0f;
-                    }
+                    if (c_scale != 0.0f) d = aug_scale_grad(d, e[k], zs[k], c_scale);
                     dsum[k] += d;
                 }
             }
@@ -149,8 +82,7 @@ assemble_kernel(GroupTable tab, GroupGradTable gtab, int P, int M, int B, float 
             means3D[3 * (size_t)i + 1] = tab.xyz[g][3 * (size_t)l + 1];
             means3D[3 * (size_t)i + 2] = tab.xyz[g][3 * (size_t)l + 2];
             opac[i] = sig;
-            *reinterpret_cast<float4*>(rots + 4 * (size_t)i) =
-                make_float4(__fdiv_rn(q.x, nrm), __fdiv_rn(q.y, nrm), __fdiv_rn(q.z, nrm), __fdiv_rn(q.w, nrm));
+            *reinterpret_cast<float4*>(rots + 4 * (size_t)i) = quat_normalize(q, nrm);
         } else {
             // incoming gradients live in the packed arrays; outputs are the per-group leaf gradients
             gtab.xyz[g][3 * (size_t)l] = means3D[3 * (size_t)i];
@@ -160,12 +92,7 @@ assemble_kernel(GroupTable tab, GroupGradTable gtab, int P, int M, int B, float 
 #pragma unroll
             for (int k = 0; k < 3; ++k) gtab.scaling[g][3 * (size_t)l + k] = dsum[k] * e[k];
             const float4 gq = *reinterpret_cast<const float4*>(rots + 4 * (size_t)i);
-            const float inv = 1.0f / nrm;
-            const float4 u = make_float4(q.x * inv, q.y * inv, q.z * inv, q.w * inv);
-            const float dot = u.x * gq.x + u.y * gq.y + u.z * gq.z + u.w * gq.w;
-            // d normalize: (g - u (u.g)) / |q|   (the eps clamp is inactive for any usable quaternion)
-            *reinterpret_cast<float4*>(gtab.rotation[g] + 4 * (size_t)l) =
-                make_float4((gq.x - u.x * dot) * inv, (gq.y - u.y * dot) * inv, (gq.z - u.z * dot) * inv, (gq.w - u.w * dot) * inv);
+            *reinterpret_cast<float4*>(gtab.rotation[g] + 4 * (size_t)l) = quat_normalize_grad(q, nrm, gq);
         }
     }
     // ---- phase B: SH rows of the block as a flat span ----------------------------------------
@@ -241,21 +168,7 @@ cudaError_t gsr_launch_assemble(bool backward, int num_groups, const b200gsr_gro
                                 float* means3D, float* opac, float* scales, float* rots, float* shs, cudaStream_t s) {
     GroupTable tab;
     GroupGradTable gtab;
-    memset(&tab, 0, sizeof(tab));
-    memset(&gtab, 0, sizeof(gtab));
-    int P = 0;
-    for (int g = 0; g < num_groups; ++g) {
-        tab.xyz[g] = groups[g].xyz; tab.opacity[g] = groups[g].opacity; tab.scaling[g] = groups[g].scaling;
-        tab.rotation[g] = groups[g].rotation; tab.f_dc[g] = groups[g].f_dc; tab.f_rest[g] = groups[g].f_rest;
-        tab.start[g] = P;
-        P += groups[g].n;
-        if (backward) {
-            gtab.xyz[g] = grads[g].xyz; gtab.opacity[g] = grads[g].opacity; gtab.scaling[g] = grads[g].scaling;
-            gtab.rotation[g] = grads[g].rotation; gtab.f_dc[g] = grads[g].f_dc; gtab.f_rest[g] = grads[g].f_rest;
-        }
-    }
-    tab.start[num_groups] = P;
-    tab.num = num_groups;
+    const int P = gsr_group_tables(num_groups, groups, backward ? grads : nullptr, tab, gtab);
     if (P == 0) return cudaSuccess;
     const int nblocks = (P + kAsmBlock - 1) / kAsmBlock;
     if (backward)

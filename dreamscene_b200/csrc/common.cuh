@@ -203,6 +203,19 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 #endif  // __CUDACC__
 
 // ---- kernel launchers (defined in the .cu files, called from api.cu) ---------------------
+// Scene renders (b200gsr_forward_scene / b200gsr_backward_scene): the projection reads each group's raw leaves and
+// applies the activations and the view's augmentation itself instead of reading packed per-view arrays.
+struct GsrScene {
+    int num_groups;
+    const b200gsr_group* groups;         // host array of num_groups records
+    const b200gsr_group_grad* grads;     // host array (backward): leaf gradient destinations
+    const float* shs_noise;              // host [B]: per-view SH noise coefficient (0 = off)
+    const float* scale_noise;            // host [B]: per-view scale noise coefficient (0 = off)
+    unsigned long long seed;
+    float* out_scales;                   // forward: [B,P,3] augmented scales, or null
+    const float* d_scales;               // backward: [B,P,3] incoming gradient of those scales, or null
+};
+
 struct GsrFwdArgs {
     b200gsr_params prm;
     const float *means3D, *shs, *colors, *opac, *scales, *rots, *cov3d;
@@ -224,6 +237,7 @@ struct GsrFwdArgs {
     int num_sms;           // of the current device (cached per device in api.cu)
     unsigned long long* stats;
     cudaStream_t stream;
+    const GsrScene* scene; // scene render: the raw leaves replace means3D .. cov3d (null otherwise)
 };
 
 struct GsrBwdArgs {
@@ -244,6 +258,7 @@ struct GsrBwdArgs {
     int num_sms;
     unsigned long long* stats;   // optional device counters (b200gsr_debug_counters); selects the STATS kernels
     cudaStream_t stream;
+    const GsrScene* scene;       // scene render: leaf gradients of the raw parameters (null otherwise)
 };
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device) instead of on every

@@ -8,8 +8,9 @@
 // Numerics contract: everything that decides an integer (depth bits, radius, tile rect) uses
 // individually rounded fp32 ops (__fmul_rn/__fadd_rn/... are never FMA-contracted) in the order
 // written in the oracle, so those integers are bit-exact against it.
-#include "common.cuh"
+#include "scene_math.cuh"
 #include <cuda_fp16.h>
+#include <type_traits>
 
 #define MUL(a, b) __fmul_rn((a), (b))
 #define ADD(a, b) __fadd_rn((a), (b))
@@ -235,6 +236,93 @@ __device__ __forceinline__ void stage_sh_rows(const float* __restrict__ shs, int
     else asm volatile("cp.async.commit_group;" ::: "memory");
 }
 
+// ---- raw-parameter mode (RAW: b200gsr_forward_scene / b200gsr_backward_scene) ---------------------------------
+// The kernels read each group's raw leaves and form the rasterizer inputs themselves with the helpers of
+// scene_math.cuh, in assemble_kernel's statements, so the values are bit for bit those assemble_kernel writes for
+// the same seed and view.  The default instantiations take the empty NoScene in the last parameter slot.
+struct NoScene {};
+struct SceneFwd {
+    GroupTable tab;
+    unsigned long long seed;
+    float c_shs, c_scale;        // this view's noise coefficients (0 = no augmentation)
+    uint32_t view;               // Philox streams 2 view + 1 (SH) and 2 view + 2 (scales)
+    float* out_scales;           // this view's [P,3] augmented scales, or null
+};
+struct SceneBwd {
+    GroupTable tab;
+    GroupGradTable gtab;
+    unsigned long long seed;
+    float c_shs, c_scale;
+    uint32_t view;               // view 0 writes every leaf gradient row, later views add into the rows they touch
+    const float* d_scales;       // incoming gradient of this view's augmented scales [P,3], or null
+};
+
+// A row's shape leaves and what the chain rule needs of them.
+struct RawLeaf {
+    float e[3], z[3];            // exp(_scaling), the scale noise
+    float4 q;                    // _rotation
+    float nrm;                   // its clamped norm
+};
+__device__ __forceinline__ void raw_shape(const GroupTable& t, int grp, size_t loc, int i, unsigned long long seed,
+                                          float c_scale, uint32_t view, RawLeaf& lf, RawShape& r) {
+    const float* sp = t.scaling[grp] + 3 * loc;
+    lf.e[0] = act_scale(__ldg(sp)); lf.e[1] = act_scale(__ldg(sp + 1)); lf.e[2] = act_scale(__ldg(sp + 2));
+    lf.z[0] = lf.z[1] = lf.z[2] = 0.0f;
+    if (c_scale != 0.0f) {
+        const float4 n = normal4(seed, kStreamScales + 2u * view, (unsigned long long)i);
+        lf.z[0] = n.x; lf.z[1] = n.y; lf.z[2] = n.z;
+    }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) r.s[k] = (c_scale != 0.0f) ? aug_scale(lf.e[k], lf.z[k], c_scale) : lf.e[k];
+    lf.q = __ldg(reinterpret_cast<const float4*>(t.rotation[grp]) + loc);
+    lf.nrm = quat_norm(lf.q);
+    r.q = quat_normalize(lf.q, lf.nrm);
+}
+
+// SH rows of the block's visible rows from f_dc [n,1,3] and f_rest [n,M-1,3]: 12- and 12(M-1)-byte rows that are
+// not 16-byte aligned, so half a warp copies one row with 4-byte cp.async (coalesced within the row).
+template <bool WAIT>
+__device__ __forceinline__ void stage_raw_rows(const GroupTable& t, int M, int nf, int g0, int P, const uint8_t* vis,
+                                               float* buf, int stride) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int hl = lane & 15, hsel = lane >> 4;
+    const size_t nrest = 3 * (size_t)M - 3;
+    for (int it = 0; it < kBlock / 8; ++it) {
+        const int row = it * 8 + w * 2 + hsel;          // 4 warps x 2 rows per iteration
+        if (g0 + row < P && vis[row]) {
+            const int grp = find_group(t, g0 + row);
+            const size_t loc = (size_t)(g0 + row - t.start[grp]);
+            const float* dc = t.f_dc[grp] + 3 * loc;
+            const float* fr = t.f_rest[grp] + nrest * loc;
+            float* dst = buf + row * stride;
+            for (int col = hl; col < nf; col += 16) cp_async4(dst + col, col < 3 ? dc + col : fr + (col - 3));
+        }
+    }
+    if (WAIT) cp_async_wait_all();
+    else asm volatile("cp.async.commit_group;" ::: "memory");
+}
+
+// A staged row of nf coefficients, whose first element has the flat index e0 in the view's packed [P, M, 3] array,
+// augmented in place: v + z * (c * v) with z = component e & 3 of quad e >> 2 of `stream` (assemble_kernel's draw
+// for element e).  FACTOR: multiplied by the derivative 1 + z c instead.
+template <bool FACTOR>
+__device__ __forceinline__ void raw_sh_noise(float* row, int nf, size_t e0, unsigned long long seed, uint32_t stream,
+                                             float c) {
+    const size_t e_end = e0 + nf;
+    for (unsigned long long q = e0 >> 2; 4 * q < e_end; ++q) {
+        const float4 n = normal4(seed, stream, q);
+        const float z[4] = {n.x, n.y, n.z, n.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const size_t e = 4 * q + k;
+            if (e >= e0 && e < e_end) {
+                float& v = row[e - e0];
+                v = FACTOR ? v * (1.0f + z[k] * c) : aug(v, z[k], c, 1.0f);
+            }
+        }
+    }
+}
+
 // basis values for degree <= 3 at unit direction (x,y,z): utils/sh_utils.py:73-102
 __device__ __forceinline__ void sh_basis(int deg, float x, float y, float z, float (&B)[16]) {
     B[0] = SH_C0;
@@ -287,7 +375,11 @@ __device__ __forceinline__ void sh_color(const float (&B)[16], const float* row,
 // Gaussian); record part 2 carries only the index.  The cull, radius, tile rect, depth bits and record parts 0/1 are
 // the default mode's statements, so the tile lists are those of a score_flag render.  No backward state is written and
 // `radii` may be null.  Every GEO difference is a compile-time guard, so the other instantiations carry no trace of it.
-template <int MT, bool DET = false, bool GEO = false>
+// RAW: the scene render (b200gsr_forward_scene).  The inputs are the raw leaves of `sc.tab`: mean, sigmoid opacity,
+// augmented exp scale and normalized rotation are formed per row, the visible rows' SH coefficients are staged from
+// f_dc / f_rest and augmented in shared memory before the colour is evaluated, and with sc.out_scales every row's
+// augmented scales are written out.  The packed input pointers are null.  Compile-time guards only, as for GEO.
+template <int MT, bool DET = false, bool GEO = false, bool RAW = false>
 __global__ void __launch_bounds__(kBlock)
 project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
                   const float* __restrict__ shs, const float* __restrict__ colors,
@@ -298,7 +390,8 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
                   uint32_t* __restrict__ zero_words, int num_zero_words, float* __restrict__ dgeom,
                   int rec_base, int tile_row_off, int ntiles_total,
                   uint32_t* __restrict__ det_max, unsigned long long* __restrict__ det_fx,
-                  unsigned long long* __restrict__ score_fx, uint32_t* __restrict__ det_queue) {
+                  unsigned long long* __restrict__ score_fx, uint32_t* __restrict__ det_queue,
+                  const std::conditional_t<RAW, SceneFwd, NoScene> sc) {
     extern __shared__ __align__(16) float sh_buf[];
     __shared__ uint8_t vis_s[kBlock];
     const int g0 = blockIdx.x * kBlock;
@@ -317,16 +410,37 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
     int minx = 0, maxx = 0, miny = 0, maxy = 0;
     uint4 rd = make_uint4(0u, 0u, 0u, 0u);
     bool vis = false;
+    int grp = 0;                 // RAW: the row's group and its row inside the group
+    size_t loc = 0;
+    RawShape rs;                 // RAW: the row's rasterizer shape inputs
     if (active) {
-        x = __ldg(means3D + 3 * (size_t)i); y = __ldg(means3D + 3 * (size_t)i + 1);
-        z = __ldg(means3D + 3 * (size_t)i + 2);
+        if constexpr (RAW) {
+            grp = find_group(sc.tab, i);
+            loc = (size_t)(i - sc.tab.start[grp]);
+            const float* xp = sc.tab.xyz[grp] + 3 * loc;
+            x = __ldg(xp); y = __ldg(xp + 1); z = __ldg(xp + 2);
+        } else {
+            x = __ldg(means3D + 3 * (size_t)i); y = __ldg(means3D + 3 * (size_t)i + 1);
+            z = __ldg(means3D + 3 * (size_t)i + 2);
+        }
         geo_view(C, x, y, z, g);
         rd.z = __float_as_uint(g.tz);
+        if constexpr (RAW) {
+            if (g.tz > GSR_NEAR_Z || sc.out_scales != nullptr) {
+                RawLeaf lf;
+                raw_shape(sc.tab, grp, loc, i, sc.seed, sc.c_scale, sc.view, lf, rs);
+                if (sc.out_scales != nullptr) {      // every row, culled ones included (the scale loss reads them all)
+                    float* so = sc.out_scales + 3 * (size_t)i;
+                    so[0] = rs.s[0]; so[1] = rs.s[1]; so[2] = rs.s[2];
+                }
+            }
+        }
         if (g.tz > GSR_NEAR_Z) {
             // (hoisting these loads above the depth cull was measured: no gain)
             RawShape raw;
-            load_shape(scales, rots, cov3d, i, raw);
-            geo_rest(C, p, x, y, z, cov3d != nullptr, raw, g);
+            if constexpr (RAW) raw = rs;
+            else load_shape(scales, rots, cov3d, i, raw);
+            geo_rest(C, p, x, y, z, !RAW && cov3d != nullptr, raw, g);
             if (g.det != 0.0f) {
                 const float mid = MUL(0.5f, ADD(g.a, g.c));
                 const float sq = SQRT(fmaxf(SUB(MUL(mid, mid), g.det), 0.1f));
@@ -370,10 +484,11 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
     }
     const int stride = sh_row_stride(p.M);
     const int ncoef = (p.sh_degree + 1) * (p.sh_degree + 1);
-    if (!GEO && shs != nullptr) {
+    if (!GEO && (RAW || shs != nullptr)) {
         vis_s[threadIdx.x] = vis;
         __syncthreads();
-        stage_sh_rows<MT>(shs, p.M, 3 * ncoef, g0, p.P, vis_s, sh_buf, stride);
+        if constexpr (RAW) stage_raw_rows<true>(sc.tab, p.M, 3 * ncoef, g0, p.P, vis_s, sh_buf, stride);
+        else stage_sh_rows<MT>(shs, p.M, 3 * ncoef, g0, p.P, vis_s, sh_buf, stride);
         __syncthreads();
     }
     if (!vis) return;
@@ -389,7 +504,12 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
     float rgb[3];
     if constexpr (GEO) {
         rgb[0] = rgb[1] = rgb[2] = 0.0f;
-    } else if (shs != nullptr) {
+    } else if (RAW || shs != nullptr) {
+        if constexpr (RAW) {     // this thread's own row: no barrier needed
+            if (sc.c_shs != 0.0f)
+                raw_sh_noise<false>(sh_buf + threadIdx.x * stride, 3 * ncoef, (size_t)i * 3 * p.M, sc.seed,
+                                    kStreamShs + 2u * sc.view, sc.c_shs);
+        }
         float dx = x - C.cam[0], dy = y - C.cam[1], dz = z - C.cam[2];
         float dn = sqrtf(dx * dx + dy * dy + dz * dz);
         if (dn == 0.0f) dn = 1.0f;
@@ -402,7 +522,9 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
         rgb[0] = __ldg(colors + 3 * (size_t)i); rgb[1] = __ldg(colors + 3 * (size_t)i + 1);
         rgb[2] = __ldg(colors + 3 * (size_t)i + 2);
     }
-    const float o = __ldg(opac + i);
+    float o;
+    if constexpr (RAW) o = act_opacity(__ldg(sc.tab.opacity[grp] + loc));
+    else o = __ldg(opac + i);
     // conservative half extents of the region where alpha can reach 1/255
     float ex = -1.0f, ey = -1.0f;
     if (o * 255.0f > 1.0f) {
@@ -444,8 +566,12 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
 //   5: sum G*dL/dalpha (dL/dopacity)   6..8: dL/drgb   9: dL/ddepth   10,11: unused
 // =========================================================================================
 // 6 CTAs/SM (80 registers): with the parameter loads hoisted above the SH wait, 8 CTAs/SM (64 registers) spills heavily.
-template <int MT>
-__global__ void __launch_bounds__(kBlock, 6)
+// RAW: the scene render's backward (b200gsr_backward_scene).  The activations and noise factors are recomputed from
+// the raw leaves of `sc.tab` and the view's parameter gradients are chained straight to the leaf gradients of
+// `sc.gtab`; view 0 writes every row (zeros on culled rows), later views add into the rows they touched only.  It
+// carries more live state (the leaf values and noise of the row), hence 5 CTAs/SM.
+template <int MT, bool RAW = false>
+__global__ void __launch_bounds__(kBlock, RAW ? 5 : 6)
 project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
                    const float* __restrict__ shs, const float* __restrict__ colors,
                    const float* __restrict__ scales, const float* __restrict__ rots,
@@ -455,7 +581,8 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
                    float* __restrict__ d_means3D, float* __restrict__ d_means2D,
                    float* __restrict__ d_shs, float* __restrict__ d_colors,
                    float* __restrict__ d_opac, float* __restrict__ d_scales,
-                   float* __restrict__ d_rots, float* __restrict__ d_cov3d) {
+                   float* __restrict__ d_rots, float* __restrict__ d_cov3d,
+                   const std::conditional_t<RAW, SceneBwd, NoScene> sc) {
     extern __shared__ __align__(16) float sh_buf[];
     __shared__ uint8_t vis_s[kBlock];
     // this launch covers Gaussians [g_base, g_end) (the whole range, or one chunk when the host
@@ -468,25 +595,46 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
     const int stride = sh_row_stride(p.M);
     const int deg = p.sh_degree;
     const int ncoef = (deg + 1) * (deg + 1);
-    if (shs != nullptr) {
+    if (RAW || shs != nullptr) {
         vis_s[threadIdx.x] = vis;
         __syncthreads();
-        stage_sh_rows<MT, false>(shs, p.M, 3 * ncoef, g0, g_end, vis_s, sh_buf, stride);   // issue only
+        if constexpr (RAW) stage_raw_rows<false>(sc.tab, p.M, 3 * ncoef, g0, g_end, vis_s, sh_buf, stride);
+        else stage_sh_rows<MT, false>(shs, p.M, 3 * ncoef, g0, g_end, vis_s, sh_buf, stride);   // issue only
     }
     // every other global load of this thread is issued while the SH rows are still in flight
     float x = 0.f, y = 0.f, z = 0.f;
     RawShape raw;
     float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), a1 = a0, a2 = a0;
     float4* dg = nullptr;
+    int grp = 0;                 // RAW: the row's group, its row inside the group and its shape leaves
+    size_t loc = 0;
+    RawLeaf lf;
+    if constexpr (RAW) {
+        if (active) {
+            grp = find_group(sc.tab, i);
+            loc = (size_t)(i - sc.tab.start[grp]);
+            if (vis || sc.d_scales != nullptr) raw_shape(sc.tab, grp, loc, i, sc.seed, sc.c_scale, sc.view, lf, raw);
+        }
+    }
     if (vis) {
-        x = __ldg(means3D + 3 * (size_t)i); y = __ldg(means3D + 3 * (size_t)i + 1); z = __ldg(means3D + 3 * (size_t)i + 2);
-        load_shape(scales, rots, cov3d, i, raw);
+        if constexpr (RAW) {
+            const float* xp = sc.tab.xyz[grp] + 3 * loc;
+            x = __ldg(xp); y = __ldg(xp + 1); z = __ldg(xp + 2);
+        } else {
+            x = __ldg(means3D + 3 * (size_t)i); y = __ldg(means3D + 3 * (size_t)i + 1); z = __ldg(means3D + 3 * (size_t)i + 2);
+            load_shape(scales, rots, cov3d, i, raw);
+        }
         dg = reinterpret_cast<float4*>(dgeom + 12 * (size_t)(rec_base + i));
         a0 = dg[0]; a1 = dg[1]; a2 = dg[2];
     }
-    if (shs != nullptr) {
+    if (RAW || shs != nullptr) {
         cp_async_wait_all();
         __syncthreads();
+    }
+    if constexpr (RAW) {         // the visible rows' SH coefficients as the forward augmented them (own row)
+        if (vis && sc.c_shs != 0.0f)
+            raw_sh_noise<false>(sh_buf + threadIdx.x * stride, 3 * ncoef, (size_t)i * 3 * p.M, sc.seed,
+                                kStreamShs + 2u * sc.view, sc.c_shs);
     }
     float dmean[3] = {0.f, 0.f, 0.f};
     float dm2[2] = {0.f, 0.f};
@@ -505,7 +653,7 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
         load_cam(p, C);
         Geo g;
         geo_view(C, x, y, z, g);
-        geo_rest(C, p, x, y, z, cov3d != nullptr, raw, g);
+        geo_rest(C, p, x, y, z, !RAW && cov3d != nullptr, raw, g);
         // read-and-clear: the accumulators are zero again for the next backward over this `saved`
         const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
         dg[0] = z4; dg[1] = z4; dg[2] = z4;
@@ -568,7 +716,7 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
         dmean[1] += C.V[4] * dtx + C.V[5] * dty + C.V[6] * dtz;
         dmean[2] += C.V[8] * dtx + C.V[9] * dty + C.V[10] * dtz;
 
-        if (cov3d != nullptr) {
+        if (!RAW && cov3d != nullptr) {
             dcov[0] = Gs[0]; dcov[1] = Gs[1] + Gs[3]; dcov[2] = Gs[2] + Gs[6];
             dcov[3] = Gs[4]; dcov[4] = Gs[5] + Gs[7]; dcov[5] = Gs[8];
         } else {
@@ -607,7 +755,7 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
         }
 
         // ---- colour -> SH (coefficients live in this thread's shared-memory row) -------------
-        if (shs != nullptr) {
+        if (RAW || shs != nullptr) {
             float vx = x - C.cam[0], vy = y - C.cam[1], vz = z - C.cam[2];
             float dn = sqrtf(vx * vx + vy * vy + vz * vz);
             if (dn == 0.0f) dn = 1.0f;
@@ -673,6 +821,105 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
         } else {
             dcol[0] = drgb[0]; dcol[1] = drgb[1]; dcol[2] = drgb[2];
         }
+    }
+
+    if constexpr (RAW) {
+        // ---- leaf gradients.  View 0 writes every row (zeros on culled rows); a later view adds into the rows it
+        // touched: its visible rows, and every row's _scaling when the augmented scales have an incoming gradient.
+        const bool first = sc.view == 0;
+        const bool has_ds = sc.d_scales != nullptr;
+        if (active) {
+            d_means2D[3 * (size_t)i] = dm2[0]; d_means2D[3 * (size_t)i + 1] = dm2[1]; d_means2D[3 * (size_t)i + 2] = 0.f;
+            // this view's contribution to the row's 11 leaf floats; a later view loads all old values before it
+            // stores any (the five leaf arrays may alias as far as the compiler knows: load/store pairs would
+            // serialise on the load latency)
+            float gm[3] = {dmean[0], dmean[1], dmean[2]}, go = 0.0f, gs[3] = {0.f, 0.f, 0.f};
+            float4 gq = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (vis) {
+                const float sig = act_opacity(__ldg(sc.tab.opacity[grp] + loc));
+                go = dop * sig * (1.0f - sig);
+                gq = quat_normalize_grad(lf.q, lf.nrm, make_float4(drot[0], drot[1], drot[2], drot[3]));
+            }
+            if (vis || has_ds) {
+#pragma unroll
+                for (int k = 0; k < 3; ++k) {
+                    float d = dsc[k] + (has_ds ? __ldg(sc.d_scales + 3 * (size_t)i + k) : 0.0f);
+                    if (sc.c_scale != 0.0f) d = aug_scale_grad(d, lf.e[k], lf.z[k], sc.c_scale);
+                    gs[k] = d * lf.e[k];
+                }
+            }
+            float* px = sc.gtab.xyz[grp] + 3 * loc;
+            float* po = sc.gtab.opacity[grp] + loc;
+            float* ps = sc.gtab.scaling[grp] + 3 * loc;
+            float4* pq = reinterpret_cast<float4*>(sc.gtab.rotation[grp]) + loc;
+            const bool rows_touched = first || vis, scale_touched = first || vis || has_ds;
+            if (!first) {
+                if (rows_touched) {
+                    const float4 oq = *pq;
+                    const float ox = px[0], oy = px[1], oz = px[2], oo = *po;
+                    gm[0] += ox; gm[1] += oy; gm[2] += oz; go += oo;
+                    gq.x += oq.x; gq.y += oq.y; gq.z += oq.z; gq.w += oq.w;
+                }
+                if (scale_touched) {
+                    const float s0 = ps[0], s1 = ps[1], s2 = ps[2];
+                    gs[0] += s0; gs[1] += s1; gs[2] += s2;
+                }
+            }
+            if (rows_touched) {
+                px[0] = gm[0]; px[1] = gm[1]; px[2] = gm[2]; *po = go; *pq = gq;
+            }
+            if (scale_touched) { ps[0] = gs[0]; ps[1] = gs[1]; ps[2] = gs[2]; }
+        }
+        // SH: the row holds dL/d(augmented coefficient); times 1 + z c it is the leaf gradient.  Then the rows drain
+        // to f_dc / f_rest, half a warp per row (the leaves' rows are not 16-byte aligned).
+        const int nf = 3 * ncoef, nrow = 3 * p.M;
+        if (vis && sc.c_shs != 0.0f)
+            raw_sh_noise<true>(sh_buf + threadIdx.x * stride, nf, (size_t)i * nrow, sc.seed, kStreamShs + 2u * sc.view,
+                               sc.c_shs);
+        __syncthreads();
+        // Half a warp per row, four rows per thread at a time: a later view loads the old values of all of them
+        // before it stores, so twelve loads are in flight instead of one.
+        const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+        const int hl = lane & 15, hsel = lane >> 4;
+        const int lim = first ? nrow : nf;                 // view 0 also writes the zeros above the degree
+#pragma unroll 1
+        for (int it0 = 0; it0 < kBlock / 8; it0 += 4) {
+            float* dst[4][3];
+            float val[4][3];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const int row = (it0 + u) * 8 + w * 2 + hsel;
+                const int gi = g0 + row;
+                const bool v = gi < g_end && vis_s[row];
+                const bool on = gi < g_end && (first || v);
+                int gg = 0;
+                if (on) gg = find_group(sc.tab, gi);
+                const size_t ll = on ? (size_t)(gi - sc.tab.start[gg]) : 0;
+#pragma unroll
+                for (int j = 0; j < 3; ++j) {
+                    const int col = hl + 16 * j;
+                    dst[u][j] = nullptr;
+                    val[u][j] = 0.0f;
+                    if (on && col < lim) {
+                        dst[u][j] = col < 3 ? sc.gtab.f_dc[gg] + 3 * ll + col : sc.gtab.f_rest[gg] + (size_t)(nrow - 3) * ll + (col - 3);
+                        if (v && col < nf) val[u][j] = sh_buf[row * stride + col];
+                    }
+                }
+            }
+            if (!first) {
+#pragma unroll
+                for (int u = 0; u < 4; ++u)
+#pragma unroll
+                    for (int j = 0; j < 3; ++j)
+                        if (dst[u][j]) val[u][j] += *dst[u][j];
+            }
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+#pragma unroll
+                for (int j = 0; j < 3; ++j)
+                    if (dst[u][j]) *dst[u][j] = val[u][j];
+        }
+        return;
     }
 
     // ---- dense writes (zeros for culled Gaussians).  `accumulate` (bit per output: 1 means3D, 2 opacity,
@@ -781,7 +1028,20 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D,
 
 }  // namespace
 
-template <int MT, bool DET, bool GEO = false>
+// The raw-parameter mode's kernel argument for view a.view of a scene render.
+static SceneFwd scene_fwd(const GsrFwdArgs& a) {
+    SceneFwd sc;
+    GroupGradTable unused;
+    gsr_group_tables(a.scene->num_groups, a.scene->groups, nullptr, sc.tab, unused);
+    sc.seed = a.scene->seed;
+    sc.c_shs = a.scene->shs_noise[a.view];
+    sc.c_scale = a.scene->scale_noise[a.view];
+    sc.view = (uint32_t)a.view;
+    sc.out_scales = a.scene->out_scales ? a.scene->out_scales + 3 * (size_t)a.P_view * a.view : nullptr;
+    return sc;
+}
+
+template <int MT, bool DET, bool GEO = false, bool RAW = false>
 static void launch_project_sh(const GsrFwdArgs& a, int P, size_t smem) {
     // multisplit path: counters + the single per-tile counter array are zeroed in the prologue
     // (api.cu issues a memset instead on the large-grid fallback, where this kernel counts itself)
@@ -789,7 +1049,9 @@ static void launch_project_sh(const GsrFwdArgs& a, int P, size_t smem) {
     tg.gy = a.num_views * a.gy_view; tg.ntiles = tg.gx * tg.gy;      // the stacked image
     const int nzero = gsr_use_multisplit(tg.ntiles) ? (int)gsr_counter_words(a.sl, tg.ntiles) : 0;
     const bool bwd = !(a.flags & B200GSR_FWD_NO_BACKWARD);
-    project_sh_kernel<MT, DET, GEO><<<(P + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
+    std::conditional_t<RAW, SceneFwd, NoScene> sc{};
+    if constexpr (RAW) sc = scene_fwd(a);
+    project_sh_kernel<MT, DET, GEO, RAW><<<(P + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
         a.prm, a.means3D, a.shs, a.colors, a.opac, a.scales, a.rots, a.cov3d, a.radii,
         reinterpret_cast<uint4*>(a.scratch + a.sl.rectdepth),
         reinterpret_cast<GsrRec*>(a.saved + a.vl.geom),
@@ -800,16 +1062,20 @@ static void launch_project_sh(const GsrFwdArgs& a, int P, size_t smem) {
         DET && bwd ? reinterpret_cast<uint32_t*>(a.saved + a.dl.dmax) : nullptr,
         DET && bwd ? reinterpret_cast<unsigned long long*>(a.saved + a.dl.dfx) : nullptr,
         DET && a.prm.score_flag ? reinterpret_cast<unsigned long long*>(a.saved + a.dl.score_fx) : nullptr,
-        DET && bwd && a.view == 0 ? reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE_DET : nullptr);
+        DET && bwd && a.view == 0 ? reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE_DET : nullptr, sc);
 }
 
 cudaError_t gsr_launch_project(const GsrFwdArgs& a, bool geo) {
     const int P = a.prm.P;
     if (P == 0) return cudaSuccess;
-    const size_t smem = a.shs ? (size_t)kBlock * sh_row_stride(a.prm.M) * sizeof(float) : 0;
+    const size_t smem = (a.shs || a.scene) ? (size_t)kBlock * sh_row_stride(a.prm.M) * sizeof(float) : 0;
     if (geo) {
         // the score pass accumulates into the caller's buffer, deterministic or not: no DET instantiation
         launch_project_sh<0, false, true>(a, P, 0);
+    } else if (a.scene) {
+        // the raw rows are staged with 4-byte copies whatever M is: no per-M instantiation
+        if (a.det) launch_project_sh<0, true, false, true>(a, P, smem);
+        else launch_project_sh<0, false, false, true>(a, P, smem);
     } else if (a.det) {
         if (a.shs && a.prm.M == 16) launch_project_sh<16, true>(a, P, smem);
         else if (a.shs && a.prm.M == 4) launch_project_sh<4, true>(a, P, smem);
@@ -822,22 +1088,36 @@ cudaError_t gsr_launch_project(const GsrFwdArgs& a, bool geo) {
     return cudaGetLastError();
 }
 
-template <int MT>
+static SceneBwd scene_bwd(const GsrBwdArgs& a) {
+    SceneBwd sc;
+    gsr_group_tables(a.scene->num_groups, a.scene->groups, a.scene->grads, sc.tab, sc.gtab);
+    sc.seed = a.scene->seed;
+    sc.c_shs = a.scene->shs_noise[a.view];
+    sc.c_scale = a.scene->scale_noise[a.view];
+    sc.view = (uint32_t)a.view;
+    sc.d_scales = a.scene->d_scales ? a.scene->d_scales + 3 * (size_t)a.P_view * a.view : nullptr;
+    return sc;
+}
+
+template <int MT, bool RAW = false>
 static void launch_project_bwd(const GsrBwdArgs& a, int g_begin, int g_end, size_t smem) {
-    project_bwd_kernel<MT><<<(g_end - g_begin + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
+    std::conditional_t<RAW, SceneBwd, NoScene> sc{};
+    if constexpr (RAW) sc = scene_bwd(a);
+    project_bwd_kernel<MT, RAW><<<(g_end - g_begin + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
         a.prm, a.means3D, a.shs, a.colors, a.scales, a.rots, a.cov3d, a.radii,
         reinterpret_cast<float*>(a.saved + a.vl.dgeom),
         reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE, g_begin, g_end,
         a.dsh_coefs > 0 ? a.dsh_coefs : (a.dsh_coefs < 0 ? -1 : a.prm.M), a.view * a.P_view, a.accumulate, a.d_means3D,
         a.d_means2D, a.d_shs,
-        a.d_colors, a.d_opac, a.d_scales, a.d_rots, a.d_cov3d);
+        a.d_colors, a.d_opac, a.d_scales, a.d_rots, a.d_cov3d, sc);
 }
 
 cudaError_t gsr_launch_project_bwd(const GsrBwdArgs& a) {
     const int g_begin = a.g_begin, g_end = a.g_end;
     if (g_end <= g_begin) return cudaSuccess;
-    const size_t smem = a.shs ? (size_t)kBlock * sh_row_stride(a.prm.M) * sizeof(float) : 0;
-    if (a.shs && a.prm.M == 16) launch_project_bwd<16>(a, g_begin, g_end, smem);
+    const size_t smem = (a.shs || a.scene) ? (size_t)kBlock * sh_row_stride(a.prm.M) * sizeof(float) : 0;
+    if (a.scene) launch_project_bwd<0, true>(a, g_begin, g_end, smem);
+    else if (a.shs && a.prm.M == 16) launch_project_bwd<16>(a, g_begin, g_end, smem);
     else if (a.shs && a.prm.M == 4) launch_project_bwd<4>(a, g_begin, g_end, smem);
     else launch_project_bwd<0>(a, g_begin, g_end, smem);
     return cudaGetLastError();

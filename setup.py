@@ -24,7 +24,7 @@ setup(
     version="0.1.0",
     description="H100-native differentiable 3D-Gaussian rasterizer (drop-in for DreamScene's diff_gaussian_rasterization)",
     packages=["dreamscene_b200", "diff_gaussian_rasterization", "simple_knn"],
-    package_data={"dreamscene_b200": ["libb200gsr.so", "csrc/*", "../include/b200gsr.h"]},
+    package_data={"dreamscene_b200": ["libb200gsr.so", "csrc/*", "../include/b200gsr.h", "../include/b200gsr_scene.h"]},
     cmdclass={"build_py": BuildWithCuda},
     python_requires=">=3.9",
 )
