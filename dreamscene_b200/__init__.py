@@ -8,7 +8,8 @@ from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer, Pair
                          set_workspace_capacity)
 from . import parallel
 from .optim import GaussianAdam
+from .graph import StepGraph
 
 __all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians",
            "set_workspace_capacity", "set_pair_count_mode", "flush_checks", "last_pair_count",
-           "PairCapacityOverflow", "parallel", "GaussianAdam"]
+           "PairCapacityOverflow", "parallel", "GaussianAdam", "StepGraph"]

@@ -1,4 +1,4 @@
-"""ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h).  Fails loudly if the library is missing:
+"""ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h).  Fails loudly if the library is missing:
 there is NO CPU or PyTorch fallback in the product path."""
 from __future__ import annotations
 
@@ -114,6 +114,22 @@ SCENE_SIGNATURES = {
                                [sz, u64, vp, u32, vp]),
 }
 
+
+class StepView(C.Structure):        # == b200gsr_step_view (include/b200gsr_step.h)
+    _fields_ = [("tanfovx", C.c_float), ("tanfovy", C.c_float), ("shs_noise", C.c_float), ("scale_noise", C.c_float),
+                ("sh_degree", C.c_int32), ("reserved", C.c_int32 * 3)]
+
+
+# The graph-replay entry points of include/b200gsr_step.h (same library), in that header's order.
+STEP_SIGNATURES = {
+    "b200gsr_forward_scene_dyn": (C.c_int, [i32, _P(Params), i32, _P(Group), vp, vp] + [vp] * 5 +
+                                  [sz, vp, sz, u64, u32, vp, u32, vp]),
+    "b200gsr_backward_scene_dyn": (C.c_int, [i32, _P(Params), i32, _P(Group), _P(GroupGrad), vp, vp] + [vp] * 6 +
+                                   [sz, u64, vp, u32, vp]),
+    "b200gsr_adam_step_dyn": (C.c_int, [i32, _P(AdamTensor), vp, vp]),
+    "b200gsr_pair_report": (C.c_int, [vp, vp, vp]),
+}
+
 _lib = None
 ABI_VERSION = 3
 ERR_BAD_ARG = -1
@@ -142,7 +158,7 @@ def load():
                 f"{LIB_PATH} is missing and could not be built ({err}). Build it with "
                 "`python -m dreamscene_b200._build` (needs nvcc; sm_90a only). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES}.items():
+    for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES, **STEP_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:

@@ -1,6 +1,7 @@
-// C ABI (include/b200gsr.h, include/b200gsr_scene.h): argument validation, buffer layouts, launch sequencing.
+// C ABI (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h): argument validation, buffer layouts,
+// launch sequencing.
 #include "common.cuh"
-#include "../../include/b200gsr_scene.h"
+#include "../../include/b200gsr_step.h"
 
 #include <cstdarg>
 #include <cstdio>
@@ -719,7 +720,7 @@ int b200gsr_kth_smallest(int32_t n, const float* v, uint32_t k, void* scratch, f
     return check_cuda(gsr_kth_smallest(n, v, k, scratch, out, ds->num_sms, GSR_ST(stream)), "kth_smallest");
 }
 
-int b200gsr_adam_step(int32_t n_tensors, const b200gsr_adam_tensor* tensors, void* stream) {
+static int check_adam(int32_t n_tensors, const b200gsr_adam_tensor* tensors) {
     if (n_tensors < 0 || (n_tensors > 0 && !tensors)) return fail(B200GSR_ERR_BAD_ARG, "bad adam_step arguments");
     if (n_tensors > B200GSR_ADAM_MAX_TENSORS)
         return fail(B200GSR_ERR_UNSUPPORTED, "adam_step: %d tensors, at most %d per call", n_tensors, B200GSR_ADAM_MAX_TENSORS);
@@ -729,7 +730,25 @@ int b200gsr_adam_step(int32_t n_tensors, const b200gsr_adam_tensor* tensors, voi
         if (t.n > 0 && (!t.param || !t.grad || !t.exp_avg || !t.exp_avg_sq))
             return fail(B200GSR_ERR_BAD_ARG, "adam_step: tensor %d has a null pointer", i);
     }
+    return B200GSR_OK;
+}
+
+int b200gsr_adam_step(int32_t n_tensors, const b200gsr_adam_tensor* tensors, void* stream) {
+    int rc = check_adam(n_tensors, tensors);
+    if (rc) return rc;
     return check_cuda(gsr_launch_adam(n_tensors, tensors, GSR_ST(stream)), "adam_step");
+}
+
+int b200gsr_adam_step_dyn(int32_t n_tensors, const b200gsr_adam_tensor* tensors, const float* scalars, void* stream) {
+    int rc = check_adam(n_tensors, tensors);
+    if (rc) return rc;
+    if (n_tensors > 0 && !scalars) return fail(B200GSR_ERR_BAD_ARG, "adam_step_dyn: scalars must be a device array [n, 6]");
+    return check_cuda(gsr_launch_adam_dyn(n_tensors, tensors, scalars, GSR_ST(stream)), "adam_step_dyn");
+}
+
+int b200gsr_pair_report(const void* saved, uint32_t* report, void* stream) {
+    if (!saved || !report) return fail(B200GSR_ERR_BAD_ARG, "pair_report: saved and report must be device pointers");
+    return check_cuda(gsr_launch_pair_report(static_cast<const uint32_t*>(saved), report, GSR_ST(stream)), "pair_report");
 }
 
 int b200gsr_debug_counters(unsigned long long* device_counters) {
@@ -764,11 +783,16 @@ int b200gsr_sh_grad_expand(int32_t P, int32_t M, int32_t sh_degree, int32_t num_
 // groups.  The forward is run_forward's kScene pass; the backward is the multi-view backward with the raw-leaf
 // mode of project_bwd, views in order.
 // ---------------------------------------------------------------------------------------------
+// `sc` carries either the host noise arrays or (the _dyn entry points, `dyn`) the device records and seed, whose
+// values the kernels trust; the host's tanfovx / tanfovy / sh_degree are not checked then, since they are not read.
 static int check_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
-                       const float* shs_noise, const float* scale_noise) {
+                       const GsrScene& sc, bool dyn) {
     if (B < 1 || B > B200GSR_MAX_VIEWS) return fail(B200GSR_ERR_UNSUPPORTED, "number of views %d not in 1..%d", B, B200GSR_MAX_VIEWS);
     if (!prm) return fail(B200GSR_ERR_BAD_ARG, "null view array");
-    if (!shs_noise || !scale_noise) return fail(B200GSR_ERR_BAD_ARG, "shs_noise / scale_noise must be host arrays of B coefficients");
+    if (dyn && (!sc.dyn_views || !sc.dyn_seed))
+        return fail(B200GSR_ERR_BAD_ARG, "views / seed must be device pointers to B step records and the seed");
+    if (!dyn && (!sc.shs_noise || !sc.scale_noise))
+        return fail(B200GSR_ERR_BAD_ARG, "shs_noise / scale_noise must be host arrays of B coefficients");
     int rc = check_groups(num_groups, groups, prm[0].M);
     if (rc) return rc;
     long long total = 0;
@@ -784,6 +808,7 @@ static int check_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups,
         if (p.score_flag) return fail(B200GSR_ERR_UNSUPPORTED, "view %d: score_flag is not supported by the scene render", v);
         if (p.bg != prm[0].bg + 3 * v)
             return fail(B200GSR_ERR_BAD_ARG, "view %d: backgrounds must be one contiguous device array [B,3] (prm[v].bg = prm[0].bg + 3 v)", v);
+        if (dyn) continue;
         if (p.sh_degree < 0 || p.sh_degree > 3) return fail(B200GSR_ERR_UNSUPPORTED, "view %d: sh_degree %d not in 0..3", v, p.sh_degree);
         if (p.M < (p.sh_degree + 1) * (p.sh_degree + 1))
             return fail(B200GSR_ERR_BAD_ARG, "view %d: M=%d inconsistent with sh_degree=%d (need (deg+1)^2 <= M)", v, p.M, p.sh_degree);
@@ -792,27 +817,50 @@ static int check_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups,
     return B200GSR_OK;
 }
 
+// b200gsr_forward_scene and b200gsr_forward_scene_dyn: `sc` as check_scene's, completed with the outputs here
+static int forward_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
+                         GsrScene sc, bool dyn, float* out_scales, float* out_color, float* out_depth_alpha,
+                         int32_t* radii, void* scratch, size_t scratch_bytes, void* saved, size_t saved_bytes,
+                         uint64_t max_pairs, uint32_t flags, uint32_t* host_notify, uint32_t notify_seq, void* stream) {
+    int rc = check_scene(B, prm, num_groups, groups, sc, dyn);
+    if (rc) return rc;
+    if (flags & ~(B200GSR_FWD_NO_BACKWARD | B200GSR_FWD_DETERMINISTIC)) return fail(B200GSR_ERR_BAD_ARG, "unknown flags 0x%x", flags);
+    if (!out_color || !out_depth_alpha || (prm[0].P > 0 && !radii) || !scratch || !saved)
+        return fail(B200GSR_ERR_BAD_ARG, "null output/workspace pointer");
+    sc.num_groups = num_groups; sc.groups = groups; sc.out_scales = out_scales;
+    return run_forward(Pass::kScene, B, prm, nullptr, out_color, out_depth_alpha, radii, nullptr, scratch, scratch_bytes,
+                       saved, saved_bytes, max_pairs, flags, host_notify, notify_seq, stream, &sc);
+}
+
 int b200gsr_forward_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
                           const float* shs_noise, const float* scale_noise, uint64_t seed, float* out_scales,
                           float* out_color, float* out_depth_alpha, int32_t* radii, void* scratch, size_t scratch_bytes,
                           void* saved, size_t saved_bytes, uint64_t max_pairs, uint32_t flags, uint32_t* host_notify,
                           uint32_t notify_seq, void* stream) {
-    int rc = check_scene(B, prm, num_groups, groups, shs_noise, scale_noise);
-    if (rc) return rc;
-    if (flags & ~(B200GSR_FWD_NO_BACKWARD | B200GSR_FWD_DETERMINISTIC)) return fail(B200GSR_ERR_BAD_ARG, "unknown flags 0x%x", flags);
-    if (!out_color || !out_depth_alpha || (prm[0].P > 0 && !radii) || !scratch || !saved)
-        return fail(B200GSR_ERR_BAD_ARG, "null output/workspace pointer");
-    const GsrScene sc = {num_groups, groups, nullptr, shs_noise, scale_noise, seed, out_scales, nullptr};
-    return run_forward(Pass::kScene, B, prm, nullptr, out_color, out_depth_alpha, radii, nullptr, scratch, scratch_bytes,
-                       saved, saved_bytes, max_pairs, flags, host_notify, notify_seq, stream, &sc);
+    GsrScene sc{};
+    sc.shs_noise = shs_noise; sc.scale_noise = scale_noise; sc.seed = seed;
+    return forward_scene(B, prm, num_groups, groups, sc, false, out_scales, out_color, out_depth_alpha, radii, scratch,
+                         scratch_bytes, saved, saved_bytes, max_pairs, flags, host_notify, notify_seq, stream);
 }
 
-int b200gsr_backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
-                           const b200gsr_group_grad* grads, const float* shs_noise, const float* scale_noise,
-                           uint64_t seed, const float* d_scales, const int32_t* radii, const float* out_depth_alpha,
-                           const float* dL_dcolor, const float* dL_ddepth_alpha, void* saved, size_t saved_bytes,
-                           uint64_t max_pairs, float* d_means2D, uint32_t flags, void* stream) {
-    int rc = check_scene(B, prm, num_groups, groups, shs_noise, scale_noise);
+int b200gsr_forward_scene_dyn(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
+                              const b200gsr_step_view* views, const uint64_t* seed, float* out_scales,
+                              float* out_color, float* out_depth_alpha, int32_t* radii, void* scratch,
+                              size_t scratch_bytes, void* saved, size_t saved_bytes, uint64_t max_pairs, uint32_t flags,
+                              uint32_t* host_notify, uint32_t notify_seq, void* stream) {
+    GsrScene sc{};
+    sc.dyn_views = views; sc.dyn_seed = reinterpret_cast<const unsigned long long*>(seed);
+    return forward_scene(B, prm, num_groups, groups, sc, true, out_scales, out_color, out_depth_alpha, radii, scratch,
+                         scratch_bytes, saved, saved_bytes, max_pairs, flags, host_notify, notify_seq, stream);
+}
+
+// b200gsr_backward_scene and b200gsr_backward_scene_dyn
+static int backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
+                          const b200gsr_group_grad* grads, GsrScene sc, bool dyn, const float* d_scales,
+                          const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
+                          const float* dL_ddepth_alpha, void* saved, size_t saved_bytes, uint64_t max_pairs,
+                          float* d_means2D, uint32_t flags, void* stream) {
+    int rc = check_scene(B, prm, num_groups, groups, sc, dyn);
     if (rc) return rc;
     if (flags & ~B200GSR_BWD_DETERMINISTIC) return fail(B200GSR_ERR_BAD_ARG, "unknown flags 0x%x", flags);
     if (num_groups > 0 && !grads) return fail(B200GSR_ERR_BAD_ARG, "grads is null");
@@ -828,7 +876,7 @@ int b200gsr_backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_gro
     if ((rc = setup_backward(true, B, prm, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes,
                              max_pairs, (flags & B200GSR_BWD_DETERMINISTIC) != 0, stream, a)))
         return rc;
-    const GsrScene sc = {num_groups, groups, grads, shs_noise, scale_noise, seed, nullptr, d_scales};
+    sc.num_groups = num_groups; sc.groups = groups; sc.grads = grads; sc.d_scales = d_scales;
     a.scene = &sc;
     a.g_begin = 0; a.g_end = P;
     prof_mark_bwd(0, a.stream);
@@ -848,6 +896,28 @@ int b200gsr_backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_gro
     prof_mark_bwd(2, a.stream);
     if (g_prof.max_calls > 0 && g_prof.nbwd < g_prof.max_calls) ++g_prof.nbwd;
     return B200GSR_OK;
+}
+
+int b200gsr_backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
+                           const b200gsr_group_grad* grads, const float* shs_noise, const float* scale_noise,
+                           uint64_t seed, const float* d_scales, const int32_t* radii, const float* out_depth_alpha,
+                           const float* dL_dcolor, const float* dL_ddepth_alpha, void* saved, size_t saved_bytes,
+                           uint64_t max_pairs, float* d_means2D, uint32_t flags, void* stream) {
+    GsrScene sc{};
+    sc.shs_noise = shs_noise; sc.scale_noise = scale_noise; sc.seed = seed;
+    return backward_scene(B, prm, num_groups, groups, grads, sc, false, d_scales, radii, out_depth_alpha, dL_dcolor,
+                          dL_ddepth_alpha, saved, saved_bytes, max_pairs, d_means2D, flags, stream);
+}
+
+int b200gsr_backward_scene_dyn(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
+                               const b200gsr_group_grad* grads, const b200gsr_step_view* views, const uint64_t* seed,
+                               const float* d_scales, const int32_t* radii, const float* out_depth_alpha,
+                               const float* dL_dcolor, const float* dL_ddepth_alpha, void* saved, size_t saved_bytes,
+                               uint64_t max_pairs, float* d_means2D, uint32_t flags, void* stream) {
+    GsrScene sc{};
+    sc.dyn_views = views; sc.dyn_seed = reinterpret_cast<const unsigned long long*>(seed);
+    return backward_scene(B, prm, num_groups, groups, grads, sc, true, d_scales, radii, out_depth_alpha, dL_dcolor,
+                          dL_ddepth_alpha, saved, saved_bytes, max_pairs, d_means2D, flags, stream);
 }
 
 int b200gsr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix,

@@ -811,3 +811,18 @@ cudaError_t gsr_launch_sort(const GsrFwdArgs& a, cudaStream_t side, cudaEvent_t 
     }
     return cudaGetLastError();
 }
+
+// b200gsr_pair_report: a forward captured into a CUDA graph has no host notify slot, so this one-thread kernel,
+// enqueued after it, folds the pair count and overflow flag the scan wrote into its header into a device report:
+// report[0] = the largest pair count seen, report[1] = the number of forwards that overflowed their key buffer.
+namespace {
+__global__ void pair_report_kernel(const uint32_t* __restrict__ header, uint32_t* __restrict__ report) {
+    report[0] = max(report[0], header[GSR_H_NUM_PAIRS]);
+    report[1] += header[GSR_H_OVERFLOW] != 0u ? 1u : 0u;
+}
+}  // namespace
+
+cudaError_t gsr_launch_pair_report(const uint32_t* header, uint32_t* report, cudaStream_t s) {
+    pair_report_kernel<<<1, 1, 0, s>>>(header, report);
+    return cudaGetLastError();
+}

@@ -4,7 +4,7 @@
 #include <stdint.h>
 #include <atomic>
 
-#include "../../include/b200gsr.h"
+#include "../../include/b200gsr_step.h"
 
 #define GSR_TILE 16
 #define GSR_NEAR_Z 0.2f
@@ -214,6 +214,10 @@ struct GsrScene {
     unsigned long long seed;
     float* out_scales;                   // forward: [B,P,3] augmented scales, or null
     const float* d_scales;               // backward: [B,P,3] incoming gradient of those scales, or null
+    // b200gsr_*_scene_dyn: device [B] per-view records and the device seed, read by the kernels in place of
+    // shs_noise / scale_noise / seed and the views' tanfovx / tanfovy / sh_degree (both null otherwise)
+    const b200gsr_step_view* dyn_views;
+    const unsigned long long* dyn_seed;
 };
 
 struct GsrFwdArgs {
@@ -389,3 +393,7 @@ __host__ __device__ inline GsrAdamChunk gsr_adam_chunk(const GsrAdamEntry& e, lo
     return c;
 }
 cudaError_t gsr_launch_adam(int n, const b200gsr_adam_tensor* t, cudaStream_t s);
+// b200gsr_adam_step_dyn: the scalars of record i are read from scalars[6 i ..] in device memory
+cudaError_t gsr_launch_adam_dyn(int n, const b200gsr_adam_tensor* t, const float* scalars, cudaStream_t s);
+// b200gsr_pair_report: fold a forward's pair count and overflow flag (its saved header) into report[2]
+cudaError_t gsr_launch_pair_report(const uint32_t* header, uint32_t* report, cudaStream_t s);

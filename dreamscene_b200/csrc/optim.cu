@@ -12,6 +12,7 @@
 //   addcdiv  fma(step_size, m / d, p)
 // Non-finite values go through the same instructions and so come out as the same bit patterns.
 #include "common.cuh"
+#include <type_traits>
 
 namespace {
 
@@ -31,11 +32,17 @@ __device__ __forceinline__ void adam_update4(float4& p, const float4& g, float4&
     adam_update(p.w, g.w, m.w, v.w, e);
 }
 
+// DYN (b200gsr_adam_step_dyn): the table of b200gsr_adam_step plus, per entry, the row of the device scalar array
+// [n, 6] that holds its six scalars, so that a CUDA graph replays with the step's learning rate and bias corrections.
+struct GsrAdamDynTable {
+    GsrAdamTable t;
+    const float* scalars;
+    int row[B200GSR_ADAM_MAX_TENSORS];   // entries skip empty tensors, rows do not
+};
+
 // One CTA = one GSR_ADAM_CHUNK-element chunk of one tensor.  The vector path issues all of a thread's loads
 // (4 x 4 float4) before the first use, so each thread keeps 256 bytes in flight.
-__global__ void __launch_bounds__(GSR_ADAM_THREADS)
-adam_step_kernel(const __grid_constant__ GsrAdamTable tab) {
-    const GsrAdamEntry& e = tab.e[gsr_adam_find(tab, blockIdx.x)];
+__device__ __forceinline__ void adam_chunk(const GsrAdamEntry& e) {
     const GsrAdamChunk c = gsr_adam_chunk(e, blockIdx.x);
     if (c.vend > c.start) {
         const int nv = (int)((c.vend - c.start) >> 2);
@@ -65,6 +72,22 @@ adam_step_kernel(const __grid_constant__ GsrAdamTable tab) {
     }
 }
 
+// DYN: each CTA loads its entry's six scalars from device memory once, in place of the table's.
+template <bool DYN = false>
+__global__ void __launch_bounds__(GSR_ADAM_THREADS)
+adam_step_kernel(const __grid_constant__ std::conditional_t<DYN, GsrAdamDynTable, GsrAdamTable> tab) {
+    if constexpr (DYN) {
+        const int k = gsr_adam_find(tab.t, blockIdx.x);
+        GsrAdamEntry e = tab.t.e[k];
+        const float* s = tab.scalars + 6 * (size_t)tab.row[k];
+        e.w = __ldg(s); e.beta2 = __ldg(s + 1); e.omb2 = __ldg(s + 2); e.eps = __ldg(s + 3);
+        e.step_size = __ldg(s + 4); e.bc2_sqrt = __ldg(s + 5);
+        adam_chunk(e);
+    } else {
+        adam_chunk(tab.e[gsr_adam_find(tab, blockIdx.x)]);
+    }
+}
+
 }  // namespace
 
 cudaError_t gsr_launch_adam(int n, const b200gsr_adam_tensor* t, cudaStream_t s) {
@@ -73,5 +96,17 @@ cudaError_t gsr_launch_adam(int n, const b200gsr_adam_tensor* t, cudaStream_t s)
     if (blocks == 0) return cudaSuccess;
     if (blocks > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
     adam_step_kernel<<<(unsigned)blocks, GSR_ADAM_THREADS, 0, s>>>(tab);
+    return cudaGetLastError();
+}
+
+cudaError_t gsr_launch_adam_dyn(int n, const b200gsr_adam_tensor* t, const float* scalars, cudaStream_t s) {
+    GsrAdamDynTable tab;
+    const long long blocks = gsr_adam_plan(n, t, &tab.t);
+    if (blocks == 0) return cudaSuccess;
+    if (blocks > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+    tab.scalars = scalars;
+    for (int i = 0, k = 0; i < n; ++i)
+        if (t[i].n > 0) tab.row[k++] = i;
+    adam_step_kernel<true><<<(unsigned)blocks, GSR_ADAM_THREADS, 0, s>>>(tab);
     return cudaGetLastError();
 }

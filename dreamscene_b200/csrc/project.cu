@@ -257,6 +257,46 @@ struct SceneBwd {
     const float* d_scales;       // incoming gradient of this view's augmented scales [P,3], or null
 };
 
+// DYN (b200gsr_forward_scene_dyn / b200gsr_backward_scene_dyn, RAW only): the view's per-step values - tanfovx,
+// tanfovy, sh_degree, the two noise coefficients and the seed - are read from device memory once at kernel entry, in
+// place of the by-value fields, so that a CUDA graph replays with the values of the step.  Compile-time guards only.
+struct SceneDyn {
+    const b200gsr_step_view* views;      // [B]; record `view` is this launch's
+    const unsigned long long* seed;
+};
+struct SceneFwdDyn : SceneFwd { SceneDyn dyn; };
+struct SceneBwdDyn : SceneBwd { SceneDyn dyn; };
+template <bool RAW, bool DYN>
+using FwdScene = std::conditional_t<RAW, std::conditional_t<DYN, SceneFwdDyn, SceneFwd>, NoScene>;
+template <bool RAW, bool DYN>
+using BwdScene = std::conditional_t<RAW, std::conditional_t<DYN, SceneBwdDyn, SceneBwd>, NoScene>;
+
+struct ViewNoise {
+    unsigned long long seed;
+    float c_shs, c_scale;
+};
+// DYN: the view's seed and noise coefficients from its device record, which also overwrites the view's tanfovx /
+// tanfovy / sh_degree in `p`.  Zeros (unused) otherwise.
+template <bool DYN, typename S>
+__device__ __forceinline__ ViewNoise view_noise(const S& sc, b200gsr_params& p) {
+    ViewNoise n{0ull, 0.0f, 0.0f};
+    if constexpr (DYN) {
+        const b200gsr_step_view* v = sc.dyn.views + sc.view;
+        p.tanfovx = __ldg(&v->tanfovx);
+        p.tanfovy = __ldg(&v->tanfovy);
+        p.sh_degree = __ldg(&v->sh_degree);
+        n.seed = __ldg(sc.dyn.seed);
+        n.c_shs = __ldg(&v->shs_noise);
+        n.c_scale = __ldg(&v->scale_noise);
+    }
+    return n;
+}
+// The RAW paths' seed and noise coefficients: the values loaded at entry under DYN, else the kernel argument's fields
+// read where they are used (as the by-value instantiations always have, so their code is unchanged).
+#define GSR_SEED (DYN ? nz.seed : sc.seed)
+#define GSR_C_SHS (DYN ? nz.c_shs : sc.c_shs)
+#define GSR_C_SCALE (DYN ? nz.c_scale : sc.c_scale)
+
 // A row's shape leaves and what the chain rule needs of them.
 struct RawLeaf {
     float e[3], z[3];            // exp(_scaling), the scale noise
@@ -379,7 +419,8 @@ __device__ __forceinline__ void sh_color(const float (&B)[16], const float* row,
 // augmented exp scale and normalized rotation are formed per row, the visible rows' SH coefficients are staged from
 // f_dc / f_rest and augmented in shared memory before the colour is evaluated, and with sc.out_scales every row's
 // augmented scales are written out.  The packed input pointers are null.  Compile-time guards only, as for GEO.
-template <int MT, bool DET = false, bool GEO = false, bool RAW = false>
+// DYN (with RAW): the view's per-step values come from device memory (view_noise).
+template <int MT, bool DET = false, bool GEO = false, bool RAW = false, bool DYN = false>
 __global__ void __launch_bounds__(kBlock)
 project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
                   const float* __restrict__ shs, const float* __restrict__ colors,
@@ -391,9 +432,10 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
                   int rec_base, int tile_row_off, int ntiles_total,
                   uint32_t* __restrict__ det_max, unsigned long long* __restrict__ det_fx,
                   unsigned long long* __restrict__ score_fx, uint32_t* __restrict__ det_queue,
-                  const std::conditional_t<RAW, SceneFwd, NoScene> sc) {
+                  const FwdScene<RAW, DYN> sc) {
     extern __shared__ __align__(16) float sh_buf[];
     __shared__ uint8_t vis_s[kBlock];
+    const ViewNoise nz = view_noise<DYN>(sc, p);
     const int g0 = blockIdx.x * kBlock;
     const int i = g0 + threadIdx.x;
     const bool active = i < p.P;
@@ -428,7 +470,7 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
         if constexpr (RAW) {
             if (g.tz > GSR_NEAR_Z || sc.out_scales != nullptr) {
                 RawLeaf lf;
-                raw_shape(sc.tab, grp, loc, i, sc.seed, sc.c_scale, sc.view, lf, rs);
+                raw_shape(sc.tab, grp, loc, i, GSR_SEED, GSR_C_SCALE, sc.view, lf, rs);
                 if (sc.out_scales != nullptr) {      // every row, culled ones included (the scale loss reads them all)
                     float* so = sc.out_scales + 3 * (size_t)i;
                     so[0] = rs.s[0]; so[1] = rs.s[1]; so[2] = rs.s[2];
@@ -506,9 +548,9 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
         rgb[0] = rgb[1] = rgb[2] = 0.0f;
     } else if (RAW || shs != nullptr) {
         if constexpr (RAW) {     // this thread's own row: no barrier needed
-            if (sc.c_shs != 0.0f)
-                raw_sh_noise<false>(sh_buf + threadIdx.x * stride, 3 * ncoef, (size_t)i * 3 * p.M, sc.seed,
-                                    kStreamShs + 2u * sc.view, sc.c_shs);
+            if (GSR_C_SHS != 0.0f)
+                raw_sh_noise<false>(sh_buf + threadIdx.x * stride, 3 * ncoef, (size_t)i * 3 * p.M, GSR_SEED,
+                                    kStreamShs + 2u * sc.view, GSR_C_SHS);
         }
         float dx = x - C.cam[0], dy = y - C.cam[1], dz = z - C.cam[2];
         float dn = sqrtf(dx * dx + dy * dy + dz * dz);
@@ -569,8 +611,9 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
 // RAW: the scene render's backward (b200gsr_backward_scene).  The activations and noise factors are recomputed from
 // the raw leaves of `sc.tab` and the view's parameter gradients are chained straight to the leaf gradients of
 // `sc.gtab`; view 0 writes every row (zeros on culled rows), later views add into the rows they touched only.  It
-// carries more live state (the leaf values and noise of the row), hence 5 CTAs/SM.
-template <int MT, bool RAW = false>
+// carries more live state (the leaf values and noise of the row), hence 5 CTAs/SM.  DYN (with RAW): the view's
+// per-step values come from device memory (view_noise).
+template <int MT, bool RAW = false, bool DYN = false>
 __global__ void __launch_bounds__(kBlock, RAW ? 5 : 6)
 project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
                    const float* __restrict__ shs, const float* __restrict__ colors,
@@ -582,9 +625,10 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
                    float* __restrict__ d_shs, float* __restrict__ d_colors,
                    float* __restrict__ d_opac, float* __restrict__ d_scales,
                    float* __restrict__ d_rots, float* __restrict__ d_cov3d,
-                   const std::conditional_t<RAW, SceneBwd, NoScene> sc) {
+                   const BwdScene<RAW, DYN> sc) {
     extern __shared__ __align__(16) float sh_buf[];
     __shared__ uint8_t vis_s[kBlock];
+    const ViewNoise nz = view_noise<DYN>(sc, p);
     // this launch covers Gaussians [g_base, g_end) (the whole range, or one chunk when the host
     // overlaps the gradient all-reduce of finished chunks with the remaining ones)
     const int g0 = g_base + blockIdx.x * kBlock;
@@ -613,7 +657,7 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
         if (active) {
             grp = find_group(sc.tab, i);
             loc = (size_t)(i - sc.tab.start[grp]);
-            if (vis || sc.d_scales != nullptr) raw_shape(sc.tab, grp, loc, i, sc.seed, sc.c_scale, sc.view, lf, raw);
+            if (vis || sc.d_scales != nullptr) raw_shape(sc.tab, grp, loc, i, GSR_SEED, GSR_C_SCALE, sc.view, lf, raw);
         }
     }
     if (vis) {
@@ -632,9 +676,9 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
         __syncthreads();
     }
     if constexpr (RAW) {         // the visible rows' SH coefficients as the forward augmented them (own row)
-        if (vis && sc.c_shs != 0.0f)
-            raw_sh_noise<false>(sh_buf + threadIdx.x * stride, 3 * ncoef, (size_t)i * 3 * p.M, sc.seed,
-                                kStreamShs + 2u * sc.view, sc.c_shs);
+        if (vis && GSR_C_SHS != 0.0f)
+            raw_sh_noise<false>(sh_buf + threadIdx.x * stride, 3 * ncoef, (size_t)i * 3 * p.M, GSR_SEED,
+                                kStreamShs + 2u * sc.view, GSR_C_SHS);
     }
     float dmean[3] = {0.f, 0.f, 0.f};
     float dm2[2] = {0.f, 0.f};
@@ -844,7 +888,7 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
 #pragma unroll
                 for (int k = 0; k < 3; ++k) {
                     float d = dsc[k] + (has_ds ? __ldg(sc.d_scales + 3 * (size_t)i + k) : 0.0f);
-                    if (sc.c_scale != 0.0f) d = aug_scale_grad(d, lf.e[k], lf.z[k], sc.c_scale);
+                    if (GSR_C_SCALE != 0.0f) d = aug_scale_grad(d, lf.e[k], lf.z[k], GSR_C_SCALE);
                     gs[k] = d * lf.e[k];
                 }
             }
@@ -873,9 +917,9 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
         // SH: the row holds dL/d(augmented coefficient); times 1 + z c it is the leaf gradient.  Then the rows drain
         // to f_dc / f_rest, half a warp per row (the leaves' rows are not 16-byte aligned).
         const int nf = 3 * ncoef, nrow = 3 * p.M;
-        if (vis && sc.c_shs != 0.0f)
-            raw_sh_noise<true>(sh_buf + threadIdx.x * stride, nf, (size_t)i * nrow, sc.seed, kStreamShs + 2u * sc.view,
-                               sc.c_shs);
+        if (vis && GSR_C_SHS != 0.0f)
+            raw_sh_noise<true>(sh_buf + threadIdx.x * stride, nf, (size_t)i * nrow, GSR_SEED, kStreamShs + 2u * sc.view,
+                               GSR_C_SHS);
         __syncthreads();
         // Half a warp per row, four rows per thread at a time: a later view loads the old values of all of them
         // before it stores, so twelve loads are in flight instead of one.
@@ -1028,20 +1072,21 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D,
 
 }  // namespace
 
-// The raw-parameter mode's kernel argument for view a.view of a scene render.
+// The raw-parameter mode's kernel argument for view a.view of a scene render (the noise fields stay zero under DYN,
+// whose kernels read them from device memory).
 static SceneFwd scene_fwd(const GsrFwdArgs& a) {
     SceneFwd sc;
     GroupGradTable unused;
     gsr_group_tables(a.scene->num_groups, a.scene->groups, nullptr, sc.tab, unused);
     sc.seed = a.scene->seed;
-    sc.c_shs = a.scene->shs_noise[a.view];
-    sc.c_scale = a.scene->scale_noise[a.view];
+    sc.c_shs = a.scene->shs_noise ? a.scene->shs_noise[a.view] : 0.0f;
+    sc.c_scale = a.scene->scale_noise ? a.scene->scale_noise[a.view] : 0.0f;
     sc.view = (uint32_t)a.view;
     sc.out_scales = a.scene->out_scales ? a.scene->out_scales + 3 * (size_t)a.P_view * a.view : nullptr;
     return sc;
 }
 
-template <int MT, bool DET, bool GEO = false, bool RAW = false>
+template <int MT, bool DET, bool GEO = false, bool RAW = false, bool DYN = false>
 static void launch_project_sh(const GsrFwdArgs& a, int P, size_t smem) {
     // multisplit path: counters + the single per-tile counter array are zeroed in the prologue
     // (api.cu issues a memset instead on the large-grid fallback, where this kernel counts itself)
@@ -1049,9 +1094,10 @@ static void launch_project_sh(const GsrFwdArgs& a, int P, size_t smem) {
     tg.gy = a.num_views * a.gy_view; tg.ntiles = tg.gx * tg.gy;      // the stacked image
     const int nzero = gsr_use_multisplit(tg.ntiles) ? (int)gsr_counter_words(a.sl, tg.ntiles) : 0;
     const bool bwd = !(a.flags & B200GSR_FWD_NO_BACKWARD);
-    std::conditional_t<RAW, SceneFwd, NoScene> sc{};
-    if constexpr (RAW) sc = scene_fwd(a);
-    project_sh_kernel<MT, DET, GEO, RAW><<<(P + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
+    FwdScene<RAW, DYN> sc{};
+    if constexpr (RAW) static_cast<SceneFwd&>(sc) = scene_fwd(a);
+    if constexpr (DYN) sc.dyn = SceneDyn{a.scene->dyn_views, a.scene->dyn_seed};
+    project_sh_kernel<MT, DET, GEO, RAW, DYN><<<(P + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
         a.prm, a.means3D, a.shs, a.colors, a.opac, a.scales, a.rots, a.cov3d, a.radii,
         reinterpret_cast<uint4*>(a.scratch + a.sl.rectdepth),
         reinterpret_cast<GsrRec*>(a.saved + a.vl.geom),
@@ -1074,7 +1120,10 @@ cudaError_t gsr_launch_project(const GsrFwdArgs& a, bool geo) {
         launch_project_sh<0, false, true>(a, P, 0);
     } else if (a.scene) {
         // the raw rows are staged with 4-byte copies whatever M is: no per-M instantiation
-        if (a.det) launch_project_sh<0, true, false, true>(a, P, smem);
+        const bool dyn = a.scene->dyn_views != nullptr;
+        if (dyn && a.det) launch_project_sh<0, true, false, true, true>(a, P, smem);
+        else if (dyn) launch_project_sh<0, false, false, true, true>(a, P, smem);
+        else if (a.det) launch_project_sh<0, true, false, true>(a, P, smem);
         else launch_project_sh<0, false, false, true>(a, P, smem);
     } else if (a.det) {
         if (a.shs && a.prm.M == 16) launch_project_sh<16, true>(a, P, smem);
@@ -1092,18 +1141,19 @@ static SceneBwd scene_bwd(const GsrBwdArgs& a) {
     SceneBwd sc;
     gsr_group_tables(a.scene->num_groups, a.scene->groups, a.scene->grads, sc.tab, sc.gtab);
     sc.seed = a.scene->seed;
-    sc.c_shs = a.scene->shs_noise[a.view];
-    sc.c_scale = a.scene->scale_noise[a.view];
+    sc.c_shs = a.scene->shs_noise ? a.scene->shs_noise[a.view] : 0.0f;
+    sc.c_scale = a.scene->scale_noise ? a.scene->scale_noise[a.view] : 0.0f;
     sc.view = (uint32_t)a.view;
     sc.d_scales = a.scene->d_scales ? a.scene->d_scales + 3 * (size_t)a.P_view * a.view : nullptr;
     return sc;
 }
 
-template <int MT, bool RAW = false>
+template <int MT, bool RAW = false, bool DYN = false>
 static void launch_project_bwd(const GsrBwdArgs& a, int g_begin, int g_end, size_t smem) {
-    std::conditional_t<RAW, SceneBwd, NoScene> sc{};
-    if constexpr (RAW) sc = scene_bwd(a);
-    project_bwd_kernel<MT, RAW><<<(g_end - g_begin + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
+    BwdScene<RAW, DYN> sc{};
+    if constexpr (RAW) static_cast<SceneBwd&>(sc) = scene_bwd(a);
+    if constexpr (DYN) sc.dyn = SceneDyn{a.scene->dyn_views, a.scene->dyn_seed};
+    project_bwd_kernel<MT, RAW, DYN><<<(g_end - g_begin + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
         a.prm, a.means3D, a.shs, a.colors, a.scales, a.rots, a.cov3d, a.radii,
         reinterpret_cast<float*>(a.saved + a.vl.dgeom),
         reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE, g_begin, g_end,
@@ -1116,7 +1166,8 @@ cudaError_t gsr_launch_project_bwd(const GsrBwdArgs& a) {
     const int g_begin = a.g_begin, g_end = a.g_end;
     if (g_end <= g_begin) return cudaSuccess;
     const size_t smem = (a.shs || a.scene) ? (size_t)kBlock * sh_row_stride(a.prm.M) * sizeof(float) : 0;
-    if (a.scene) launch_project_bwd<0, true>(a, g_begin, g_end, smem);
+    if (a.scene && a.scene->dyn_views) launch_project_bwd<0, true, true>(a, g_begin, g_end, smem);
+    else if (a.scene) launch_project_bwd<0, true>(a, g_begin, g_end, smem);
     else if (a.shs && a.prm.M == 16) launch_project_bwd<16>(a, g_begin, g_end, smem);
     else if (a.shs && a.prm.M == 4) launch_project_bwd<4>(a, g_begin, g_end, smem);
     else launch_project_bwd<0>(a, g_begin, g_end, smem);
