@@ -1,4 +1,5 @@
-"""ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h).  Fails loudly if the library is missing:
+"""ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h,
+include/b200gsr_loss.h).  Fails loudly if the library is missing:
 there is NO CPU or PyTorch fallback in the product path."""
 from __future__ import annotations
 
@@ -130,6 +131,12 @@ STEP_SIGNATURES = {
     "b200gsr_pair_report": (C.c_int, [vp, vp, vp]),
 }
 
+# The reconstruction-loss entry points of include/b200gsr_loss.h (same library), in that header's order.
+LOSS_SIGNATURES = {
+    "b200gsr_recon_l2_scratch_bytes": (C.c_size_t, [i32, i32]),
+    "b200gsr_recon_l2": (C.c_int, [i32, i32, vp, vp, i32, i32, vp, f32, vp, vp, vp, vp, sz, vp]),
+}
+
 _lib = None
 ABI_VERSION = 3
 ERR_BAD_ARG = -1
@@ -158,7 +165,7 @@ def load():
                 f"{LIB_PATH} is missing and could not be built ({err}). Build it with "
                 "`python -m dreamscene_b200._build` (needs nvcc; sm_90a only). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES, **STEP_SIGNATURES}.items():
+    for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES, **STEP_SIGNATURES, **LOSS_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:

@@ -1,7 +1,8 @@
-// C ABI (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h): argument validation, buffer layouts,
-// launch sequencing.
+// C ABI (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h, include/b200gsr_loss.h): argument
+// validation, buffer layouts, launch sequencing.
 #include "common.cuh"
 #include "../../include/b200gsr_step.h"
+#include "../../include/b200gsr_loss.h"
 
 #include <cstdarg>
 #include <cstdio>
@@ -749,6 +750,33 @@ int b200gsr_adam_step_dyn(int32_t n_tensors, const b200gsr_adam_tensor* tensors,
 int b200gsr_pair_report(const void* saved, uint32_t* report, void* stream) {
     if (!saved || !report) return fail(B200GSR_ERR_BAD_ARG, "pair_report: saved and report must be device pointers");
     return check_cuda(gsr_launch_pair_report(static_cast<const uint32_t*>(saved), report, GSR_ST(stream)), "pair_report");
+}
+
+size_t b200gsr_recon_l2_scratch_bytes(int32_t B, int32_t N) {
+    return B < 1 || N < 1 ? 0 : (size_t)B * (size_t)gsr_l2_blocks(N) * sizeof(double);
+}
+
+int b200gsr_recon_l2(int32_t B, int32_t N, const float* image, const void* target, int32_t target_is_half,
+                     int32_t n_targets, const int32_t* target_index, float weight, const void* grad_out,
+                     void* loss_out, float* d_image, void* scratch, size_t scratch_bytes, void* stream) {
+    if (B < 1 || N < 1 || n_targets < 1) return fail(B200GSR_ERR_BAD_ARG, "recon_l2: B %d, N %d and n_targets %d must be >= 1", B, N, n_targets);
+    if (B > 65535) return fail(B200GSR_ERR_UNSUPPORTED, "recon_l2: at most 65535 views, got %d", B);
+    if (target_is_half != 0 && target_is_half != 1) return fail(B200GSR_ERR_BAD_ARG, "recon_l2: target_is_half must be 0 or 1");
+    if (!image || !target) return fail(B200GSR_ERR_BAD_ARG, "recon_l2: image and target must be device pointers");
+    if (!loss_out && !d_image) return fail(B200GSR_ERR_BAD_ARG, "recon_l2: nothing to compute (loss_out and d_image are null)");
+    if (d_image && !grad_out) return fail(B200GSR_ERR_BAD_ARG, "recon_l2: d_image needs grad_out");
+    if (!target_index && B > n_targets)
+        return fail(B200GSR_ERR_BAD_ARG, "recon_l2: without target_index view v uses target v, but B %d > n_targets %d", B, n_targets);
+    if (loss_out && (!scratch || scratch_bytes < b200gsr_recon_l2_scratch_bytes(B, N) || (uintptr_t)scratch % 8))
+        return fail(B200GSR_ERR_WORKSPACE, "recon_l2: scratch must be 8-byte aligned and hold %zu bytes (got %zu)",
+                    b200gsr_recon_l2_scratch_bytes(B, N), scratch ? scratch_bytes : (size_t)0);
+    GsrL2Args a;
+    a.B = B; a.N = N; a.n_targets = n_targets;
+    a.weight = weight;
+    a.inv_n = 1.0f / (float)N;
+    a.image = image; a.target = target; a.target_index = target_index; a.grad_out = grad_out;
+    a.loss_out = loss_out; a.d_image = d_image; a.partials = static_cast<double*>(scratch);
+    return check_cuda(gsr_launch_recon_l2(a, target_is_half != 0, GSR_ST(stream)), "recon_l2");
 }
 
 int b200gsr_debug_counters(unsigned long long* device_counters) {

@@ -397,3 +397,22 @@ cudaError_t gsr_launch_adam(int n, const b200gsr_adam_tensor* t, cudaStream_t s)
 cudaError_t gsr_launch_adam_dyn(int n, const b200gsr_adam_tensor* t, const float* scalars, cudaStream_t s);
 // b200gsr_pair_report: fold a forward's pair count and overflow flag (its saved header) into report[2]
 cudaError_t gsr_launch_pair_report(const uint32_t* header, uint32_t* report, cudaStream_t s);
+
+// ---- b200gsr_recon_l2 (include/b200gsr_loss.h, csrc/loss.cu) ------------------------------------------------------
+// One CTA per GSR_L2_CHUNK elements of one view (16 per thread); with a loss, each CTA writes one double partial to
+// scratch[v * gsr_l2_blocks(N) + b] and a second launch sums a view's partials in a fixed order.
+constexpr int GSR_L2_THREADS = 256;
+constexpr int GSR_L2_CHUNK = GSR_L2_THREADS * 16;
+inline long long gsr_l2_blocks(int32_t N) { return ((long long)N + GSR_L2_CHUNK - 1) / GSR_L2_CHUNK; }
+struct GsrL2Args {
+    int32_t B, N, n_targets;
+    float weight, inv_n;           // inv_n = fp32(1 / fp32(N)), the reciprocal torch's mean backward multiplies by
+    const float* image;
+    const void* target;
+    const int32_t* target_index;   // NULL: view v uses target v
+    const void* grad_out;          // with d_image
+    void* loss_out;                // NULL: no loss
+    float* d_image;                // NULL: no gradient
+    double* partials;              // with loss_out
+};
+cudaError_t gsr_launch_recon_l2(const GsrL2Args& a, bool half_target, cudaStream_t s);

@@ -16,10 +16,20 @@ disparity focal lengths and the Adam scalars - live in static device buffers tha
 before each replay (include/b200gsr_step.h).  A step equals render_scene + disparity_from_depth_alpha + backward +
 GaussianAdam.step() for the same values; in deterministic mode bit for bit.
 
+Target mode (the refine stages' reconstruction step, f9) puts the loss into the render graph as well:
+
+    sg = StepGraph(groups, optimizers, views=1, height=H, width=W, target=gt, target_weight=100.0)   # gt [G,3,H,W]
+    sg.render(settings_list, shs_aug=False, scale_aug=False, target_index=[i])   # render + recon_l2 loss + gradient
+    sg.step()       # no eager loss, no .grad hand-off; sg.loss [B] holds each view's loss
+
+``step(optimize=False)`` replays the backward only (``grads`` and ``d_means2D``), leaving parameters, moments and
+step counters as they are: the reference's densify step, whose optimizer.step() follows densify_and_prune and so
+updates nothing.
+
 The first ``render()`` of a layout runs one eager forward and backward (which measure the pair capacity and set up
 the library) and then captures.  The layout - P, the group tensors, the optimizer state tensors, the per-view
-scale_modifier and deterministic mode - is compared on the host at every ``render()``; a change (densify / prune)
-re-captures.
+scale_modifier, deterministic mode and the target tensor and weight - is compared on the host at every ``render()``;
+a change (densify / prune) re-captures.
 """
 from __future__ import annotations
 
@@ -39,8 +49,8 @@ _VIEW_WORDS = 8             # sizeof(b200gsr_step_view) / 4
 
 
 class StepOutputs(NamedTuple):
-    """Static tensors, overwritten by the next render().  image / disp / alpha / scales are leaves that require grad:
-    the loss's gradients reach step() through their .grad."""
+    """Static tensors, overwritten by the next render().  image / disp / alpha / scales are leaves that require grad
+    (except in target mode): the loss's gradients reach step() through their .grad."""
     image: torch.Tensor     # [B,3,H,W]
     disp: torch.Tensor      # [B,1,H,W]
     alpha: torch.Tensor     # [B,1,H,W]
@@ -50,9 +60,14 @@ class StepOutputs(NamedTuple):
 
 class StepGraph:
     """One training step of `views` views of height x width over the parameter groups `groups` (as render_scene),
-    with the GaussianAdam optimizers `optimizers` over their leaves, replayed from CUDA graphs."""
+    with the GaussianAdam optimizers `optimizers` over their leaves, replayed from CUDA graphs.
 
-    def __init__(self, groups: Sequence, optimizers: Sequence, *, views: int, height: int, width: int):
+    target: a CUDA [G,3,H,W] float16 / float32 contiguous tensor of pseudo ground truths, read in place at every
+    replay.  The render graph then also computes view v's loss target_weight * mean((fp16(image_v) - target[i_v])^2)
+    (dreamscene_b200.losses.recon_l2_loss) into `loss` and its image gradient; the step minimises the views' sum."""
+
+    def __init__(self, groups: Sequence, optimizers: Sequence, *, views: int, height: int, width: int,
+                 target: torch.Tensor | None = None, target_weight: float = 100.0):
         self.groups = list(groups)
         self.optimizers = list(optimizers)
         self.B, self.H, self.W = int(views), int(height), int(width)
@@ -61,11 +76,45 @@ class StepGraph:
         for opt in self.optimizers:
             if not isinstance(opt, O.GaussianAdam):
                 raise TypeError(f"StepGraph: only GaussianAdam optimizers can be replayed, got {type(opt).__name__}")
+        self.target, self.target_weight = target, float(target_weight)
+        self._target_key()
         self._key = None
         self._report = None         # device [2]: max pair count, overflowed replays; kept across re-captures
         self._scratch_key = None
         self.d_means2D = None       # [B,P,3] per-view screen-space gradients of the last step (densification stats)
-        self.grads = None           # per group {leaf name: its gradient of the last step} (the update graph's buffers)
+        self.grads = None           # per group {leaf name: its gradient of the last step} (the backward graph's buffers)
+        self.loss = None            # target mode: [B] each view's loss of the last render(), in the target's dtype
+
+    def _target_key(self):
+        """Host checks of `target` (its device is checked in render()) -> its part of the layout key, None without."""
+        t = self.target
+        if t is None:
+            return None
+        if not torch.is_tensor(t) or t.dtype not in (torch.float16, torch.float32):
+            raise TypeError("StepGraph: target must be a float16 or float32 tensor")
+        if t.dim() != 4 or t.shape[0] < 1 or tuple(t.shape[1:]) != (3, self.H, self.W):
+            raise ValueError(f"StepGraph: target must be [G,3,{self.H},{self.W}] with G >= 1, got {tuple(t.shape)}")
+        if not t.is_contiguous():
+            raise ValueError("StepGraph: target must be contiguous (it is read in place at every replay)")
+        if 3 * self.H * self.W >= 2 ** 31:
+            raise ValueError("StepGraph: target mode needs 3 H W < 2^31")
+        return t.data_ptr(), t.dtype, tuple(t.shape), self.target_weight
+
+    def _target_indices(self, target_index):
+        """-> the B validated target indices, or None without a target."""
+        if self._target_key() is None:
+            if target_index is not None:
+                raise ValueError("StepGraph: target_index needs a StepGraph built with target=")
+            return None
+        if target_index is None:
+            raise ValueError("StepGraph: a StepGraph with a target needs render(..., target_index=[one per view])")
+        idx = [int(i) for i in target_index]
+        G = int(self.target.shape[0])
+        if len(idx) != self.B:
+            raise ValueError(f"StepGraph: expected {self.B} target indices, got {len(idx)}")
+        if not all(0 <= i < G for i in idx):
+            raise ValueError(f"StepGraph: target indices must be in 0..{G - 1}, got {idx}")
+        return idx
 
     # ---- per-step values -----------------------------------------------------------------------------------------
     def _views(self, settings, shs_aug, scale_aug, M):
@@ -92,9 +141,9 @@ class StepGraph:
                 for p in group["params"]:
                     st = opt.state.get(p, {})
                     states.append((id(p), st["exp_avg"].data_ptr() if st else 0, st["exp_avg_sq"].data_ptr() if st else 0))
-        return (P, M, ptrs, tuple(states), tuple(float(s.scale_modifier) for s in settings), det)
+        return (P, M, ptrs, tuple(states), tuple(float(s.scale_modifier) for s in settings), det, self._target_key())
 
-    def _upload(self, settings, rec, seed, focal):
+    def _upload(self, settings, rec, seed, focal, tidx):
         """One pinned staging tensor, one non_blocking copy of it (plus one device concatenation when the cameras
         are CUDA tensors).  The caching host allocator keeps the staging buffer alive until its copy has run."""
         B, dev = self.B, self._dev.device
@@ -105,6 +154,7 @@ class StepGraph:
         views[:, 4:].view(torch.int32)[:, 0] = torch.tensor([r[4] for r in rec], dtype=torch.int32)
         f0 = _SEED_WORDS + _VIEW_WORDS * B
         stage[f0:f0 + B] = torch.tensor([float(f) for f in focal], dtype=torch.float64)
+        stage[f0 + B:f0 + 2 * B].view(torch.int32)[:] = torch.tensor(tidx or [0] * B, dtype=torch.int32)
         cams = ([s.viewmatrix for s in settings] + [s.projmatrix for s in settings] + [s.campos for s in settings] +
                 [s.bg for s in settings])
         c0 = self._cam0
@@ -145,8 +195,9 @@ class StepGraph:
 
     # ---- capture -------------------------------------------------------------------------------------------------
     def _capture(self, flat, P, M, settings, det, values):
-        """Allocate the static buffers, upload this step's `values` = (records, seed, focal), run the step's render
-        and backward eagerly once (measuring the pair capacity), then capture both graphs."""
+        """Allocate the static buffers, upload this step's `values` = (records, seed, focal, target indices), run the
+        step's render and backward eagerly once (measuring the pair capacity), then capture the render, backward and
+        Adam graphs."""
         B, H, W = self.B, self.H, self.W
         dev = flat[0].device
         lib, ptr = _lib.load(), _lib.ptr
@@ -158,12 +209,14 @@ class StepGraph:
                              "(a copy would freeze their values into the graph)")
         Hs = _lib.stacked_height(B, H, W)
         Hp = Hs // B
-        self._cam0 = c0 = (_SEED_WORDS + _VIEW_WORDS * B + B + 63) // 64 * 64
-        # [seed | B view records | B focal lengths | pad | B viewmatrix, B projmatrix, B campos, B bg]
+        f0 = _SEED_WORDS + _VIEW_WORDS * B
+        self._cam0 = c0 = (f0 + 2 * B + 63) // 64 * 64
+        # [seed | B view records | B focal lengths | B target indices | pad | B viewmatrix, B projmatrix, B campos, B bg]
         self._dev = torch.zeros(c0 + B * 38, dtype=torch.float32, device=dev)
         seed_t = self._dev[:2].view(torch.int64)
-        views_t = self._dev[_SEED_WORDS:_SEED_WORDS + _VIEW_WORDS * B]
-        focal = self._dev[_SEED_WORDS + _VIEW_WORDS * B:_SEED_WORDS + _VIEW_WORDS * B + B]
+        views_t = self._dev[_SEED_WORDS:f0]
+        focal = self._dev[f0:f0 + B]
+        tidx_t = self._dev[f0 + B:f0 + 2 * B].view(torch.int32)
         cam = self._dev[c0:]
         vm, pm = cam[:16 * B].view(B, 16), cam[16 * B:32 * B].view(B, 16)
         cp, bg = cam[32 * B:35 * B].view(B, 3), cam[35 * B:38 * B].view(B, 3)
@@ -212,6 +265,14 @@ class StepGraph:
         fwd_flags = _lib.FWD_DETERMINISTIC if det else 0
         bwd_flags = _lib.BWD_DETERMINISTIC if det else 0
         views_p, seed_p = ptr(views_t), ptr(seed_t)
+        target = self.target
+        loss = None
+        if target is not None:
+            # the views' loss and its image gradient into g_image, for an incoming gradient of 1 per view
+            loss = torch.zeros(B, dtype=target.dtype, device=dev)
+            ones = torch.ones(B, dtype=target.dtype, device=dev)
+            l2_scratch = torch.empty(lib.b200gsr_recon_l2_scratch_bytes(B, 3 * H * W), dtype=torch.uint8, device=dev)
+            keep.append((ones, l2_scratch))
 
         def launch(cap, flags, scratch, saved, notify_ptr, seq):
             return lib.b200gsr_forward_scene_dyn(B, prm, ng, table, views_p, seed_p, ptr(scales), ptr(color), ptr(da),
@@ -224,6 +285,12 @@ class StepGraph:
             _lib.check(lib.b200gsr_disparity_forward(B, H * W, ptr(da4), ptr(focal), ptr(disp), ptr(stats),
                                                      _lib.stream(dev)), "b200gsr_disparity_forward")
             alpha.copy_(da4[:, 1:2])
+            if target is not None:
+                _lib.check(lib.b200gsr_recon_l2(B, 3 * H * W, ptr(image), ptr(target),
+                                                int(target.dtype == torch.float16), target.shape[0], ptr(tidx_t),
+                                                self.target_weight, ptr(ones), ptr(loss), ptr(g_image),
+                                                ptr(l2_scratch), l2_scratch.numel(), _lib.stream(dev)),
+                           "b200gsr_recon_l2")
 
         def backward(saved, cap):
             g_color.view(3, B, Hp, W)[:, :, :H].copy_(g_image.permute(1, 0, 2, 3))
@@ -260,20 +327,26 @@ class StepGraph:
             d.ensure_scratch(skey, scratch_bytes)
             torch.cuda.current_stream(dev).synchronize()
             pool = torch.cuda.graph_pool_handle()
-            g_render, g_update = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+            g_render, g_backward = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+            g_adam = torch.cuda.CUDAGraph() if tables else None     # an empty graph cannot be replayed
             with torch.cuda.graph(g_render, pool=pool):
                 saved, _, _ = R._issue_once(d, layout, fwd_flags, cap, launch, skey, True,
                                             "b200gsr_forward_scene_dyn", Exception)
                 _lib.check(lib.b200gsr_pair_report(ptr(saved), ptr(report), _lib.stream(dev)), "b200gsr_pair_report")
                 render(saved)
-            with torch.cuda.graph(g_update, pool=pool):
+            with torch.cuda.graph(g_backward, pool=pool):
                 backward(saved, cap)
-                for i0, arr in tables:
-                    _lib.check(lib.b200gsr_adam_step_dyn(len(arr), arr, C.c_void_p(self._scalars.data_ptr() + 24 * i0),
-                                                         _lib.stream(dev)), "b200gsr_adam_step_dyn")
-        for t in (image, disp, alpha, scales):
-            t.requires_grad_(True)
-        self._graphs = (g_render, g_update)
+            if g_adam is not None:
+                with torch.cuda.graph(g_adam, pool=pool):
+                    for i0, arr in tables:
+                        _lib.check(lib.b200gsr_adam_step_dyn(len(arr), arr,
+                                                             C.c_void_p(self._scalars.data_ptr() + 24 * i0),
+                                                             _lib.stream(dev)), "b200gsr_adam_step_dyn")
+        if target is None:
+            for t in (image, disp, alpha, scales):
+                t.requires_grad_(True)
+        self._graphs = (g_render, g_backward, g_adam)
+        self.loss = loss
         self._keep = (keep, prm, table, garr, tables, raw, saved, color, da, da4, stats, stats_bwd, g_color, g_da, d_da4)
         self._static_grads = (g_image, g_disp, g_alpha, g_scales)
         self._leaves = list(flat)
@@ -285,15 +358,19 @@ class StepGraph:
 
     # ---- the step ------------------------------------------------------------------------------------------------
     def render(self, settings_list: Sequence, *, shs_aug=True, scale_aug=True, seed: int | None = None,
-               generator: torch.Generator | None = None, focal=None) -> StepOutputs:
+               generator: torch.Generator | None = None, focal=None, target_index=None) -> StepOutputs:
         """Replay the render graph for this step's cameras and values (as render_scene + disparity_from_depth_alpha
-        on the stacked views).  focal: B floats, default 1 / (2 tanfovx) per view."""
+        on the stacked views).  focal: B floats, default 1 / (2 tanfovx) per view.  target_index: in target mode (only
+        there), B indices into the target, view v's pseudo ground truth; the graph also computes `loss`."""
         from . import parallel
         if parallel.reduction_active():
             raise RuntimeError("StepGraph does not reduce gradients over ranks; view sharding cannot be replayed")
         flat, M, P = S._scene_groups(self.groups)
         S._check_device(flat)
         rec = self._views(settings_list, shs_aug, scale_aug, M)
+        tidx = self._target_indices(target_index)
+        if tidx is not None and (self.target.device.type != "cuda" or self.target.device != flat[0].device):
+            raise ValueError("StepGraph: target must be a CUDA tensor on the groups' device")
         if seed is None:
             cpu_gen = generator if generator is not None and generator.device.type == "cpu" else None
             seed = int(torch.randint(0, 2 ** 62, (1,), generator=cpu_gen).item())
@@ -303,20 +380,26 @@ class StepGraph:
             raise ValueError(f"StepGraph: expected {self.B} focal lengths")
         det = R.deterministic_mode()
         if self._key is None or self._layout(flat, P, M, settings_list, det) != self._key:
-            self._capture(flat, P, M, settings_list, det, (rec, seed, focal))
+            self._capture(flat, P, M, settings_list, det, (rec, seed, focal, tidx))
         else:
-            self._upload(settings_list, rec, seed, focal)
+            self._upload(settings_list, rec, seed, focal, tidx)
         self._graphs[0].replay()
         for t in (self.out.image, self.out.disp, self.out.alpha, self.out.scales):
             t.grad = None
         return self.out
 
-    def step(self) -> None:
-        """Replay the update graph: the render backward with the .grad of image / disp / alpha / scales (a missing
-        grad counts as zeros), the disparity backward and every optimizer's step.  The leaf gradients come from out.*
+    def step(self, optimize: bool = True) -> None:
+        """Replay the backward graph: the render backward with the .grad of image / disp / alpha / scales (a missing
+        grad counts as zeros; in target mode the loss's image gradient from the render graph instead), the disparity
+        backward; then, with `optimize`, the Adam graph: every optimizer's step.  The leaf gradients come from out.*
         only: a leaf that holds a .grad of its own (a loss term that reaches it directly, or a gradient not cleared
         since an eager step) is refused rather than dropped.  Afterwards `grads` holds the leaf gradients and
-        d_means2D the per-view screen-space gradients."""
+        d_means2D the per-view screen-space gradients.
+
+        optimize=False leaves parameters, moments and step counters untouched, as the reference's optimizer.step()
+        after densify_and_prune (whose new leaves have no gradient) does.  A step where only some leaves skip Adam
+        (reset_opacity replaces the opacity leaf only) is step(optimize=False) followed by an eager
+        GaussianAdam.step() over the others' `grads` (INTEGRATION.md section 4c)."""
         if self._key is None:
             raise RuntimeError("StepGraph.step() needs a render() first")
         for t in self._leaves:
@@ -325,19 +408,23 @@ class StepGraph:
                                    "the leaf gradients from out.image / disp / alpha / scales only and would discard "
                                    "it. Clear the leaves' gradients (optimizer.zero_grad()) and route every loss term "
                                    "through the outputs")
-        for t, g in zip((self.out.image, self.out.disp, self.out.alpha, self.out.scales), self._static_grads):
-            if t.grad is None:
-                g.zero_()
-            else:
-                g.copy_(t.grad)
-            t.grad = None
-        records = self._adam_records()      # this step's lr / betas / eps; same tensors as at capture (the layout)
-        if records:
-            torch._foreach_add_([r[8] for r in records], O._ONE, alpha=1.0)   # as GaussianAdam.step(): counters first
-            stage = torch.tensor([O.adam_scalars(lr, b1, b2, eps, st.item())
-                                  for _, _, _, _, lr, b1, b2, eps, st in records], dtype=torch.float32).pin_memory()
-            self._scalars[:len(records)].copy_(stage, non_blocking=True)
+        if self.loss is None:
+            for t, g in zip((self.out.image, self.out.disp, self.out.alpha, self.out.scales), self._static_grads):
+                if t.grad is None:
+                    g.zero_()
+                else:
+                    g.copy_(t.grad)
+                t.grad = None
+        if optimize:
+            records = self._adam_records()      # this step's lr / betas / eps; same tensors as at capture (the layout)
+            if records:
+                torch._foreach_add_([r[8] for r in records], O._ONE, alpha=1.0)   # as GaussianAdam.step(): counters first
+                stage = torch.tensor([O.adam_scalars(lr, b1, b2, eps, st.item())
+                                      for _, _, _, _, lr, b1, b2, eps, st in records], dtype=torch.float32).pin_memory()
+                self._scalars[:len(records)].copy_(stage, non_blocking=True)
         self._graphs[1].replay()
+        if optimize and self._graphs[2] is not None:
+            self._graphs[2].replay()
 
     def check(self) -> None:
         """Raise PairCapacityOverflow if a render replayed since the last check - under this capture or an earlier
