@@ -131,10 +131,14 @@ STEP_SIGNATURES = {
     "b200gsr_pair_report": (C.c_int, [vp, vp, vp]),
 }
 
-# The reconstruction-loss entry points of include/b200gsr_loss.h (same library), in that header's order.
+# The loss entry points of include/b200gsr_loss.h (same library), in that header's order.
 LOSS_SIGNATURES = {
     "b200gsr_recon_l2_scratch_bytes": (C.c_size_t, [i32, i32]),
     "b200gsr_recon_l2": (C.c_int, [i32, i32, vp, vp, i32, i32, vp, f32, vp, vp, vp, vp, sz, vp]),
+    "b200gsr_tv_loss_scratch_bytes": (C.c_size_t, [i32, i32, i32, i32]),
+    "b200gsr_tv_loss": (C.c_int, [i32, i32, i32, i32, vp, vp, vp, vp, i32, vp, sz, vp]),
+    "b200gsr_scale_loss_scratch_bytes": (C.c_size_t, [i32]),
+    "b200gsr_scale_loss": (C.c_int, [i32, vp, vp, vp, vp, i32, vp, sz, vp]),
 }
 
 _lib = None

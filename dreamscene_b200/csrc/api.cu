@@ -779,6 +779,60 @@ int b200gsr_recon_l2(int32_t B, int32_t N, const float* image, const void* targe
     return check_cuda(gsr_launch_recon_l2(a, target_is_half != 0, GSR_ST(stream)), "recon_l2");
 }
 
+size_t b200gsr_tv_loss_scratch_bytes(int32_t B, int32_t C, int32_t H, int32_t W) {
+    if (B < 1 || C < 1 || H < 2 || W < 2 || (long long)B * C * H * W > INT32_MAX) return 0;
+    return (size_t)gsr_tv_blocks((long long)B * C, H, W, 1) * 2 * sizeof(double);      // the scalar path's grid
+}
+
+int b200gsr_tv_loss(int32_t B, int32_t C, int32_t H, int32_t W, const float* x, const float* grad_out, float* loss_out,
+                    float* d_x, int32_t accumulate, void* scratch, size_t scratch_bytes, void* stream) {
+    if (B < 1 || C < 1) return fail(B200GSR_ERR_BAD_ARG, "tv_loss: B %d and C %d must be >= 1", B, C);
+    if (H < 2 || W < 2) return fail(B200GSR_ERR_BAD_ARG, "tv_loss: H %d and W %d must be >= 2", H, W);
+    if ((long long)B * C * H * W > INT32_MAX)
+        return fail(B200GSR_ERR_UNSUPPORTED, "tv_loss: at most 2^31 - 1 elements, got %lld", (long long)B * C * H * W);
+    if (accumulate != 0 && accumulate != 1) return fail(B200GSR_ERR_BAD_ARG, "tv_loss: accumulate must be 0 or 1");
+    if (!x) return fail(B200GSR_ERR_BAD_ARG, "tv_loss: x must be a device pointer");
+    if (!loss_out && !d_x) return fail(B200GSR_ERR_BAD_ARG, "tv_loss: nothing to compute (loss_out and d_x are null)");
+    if (d_x && !grad_out) return fail(B200GSR_ERR_BAD_ARG, "tv_loss: d_x needs grad_out");
+    if (loss_out && (!scratch || scratch_bytes < b200gsr_tv_loss_scratch_bytes(B, C, H, W) || (uintptr_t)scratch % 8))
+        return fail(B200GSR_ERR_WORKSPACE, "tv_loss: scratch must be 8-byte aligned and hold %zu bytes (got %zu)",
+                    b200gsr_tv_loss_scratch_bytes(B, C, H, W), scratch ? scratch_bytes : (size_t)0);
+    GsrTvArgs a;
+    a.B = B; a.planes = B * C; a.H = H; a.W = W;
+    const long long ch = (long long)C * (H - 1) * W, cw = (long long)C * H * (W - 1);
+    a.inv_b = 1.0f / (float)B;              // torch's div by a CPU scalar: fp32(1 / fp32(n))
+    a.inv_h = 1.0f / (float)ch;
+    a.inv_w = 1.0f / (float)cw;
+    a.count_h = (double)ch; a.count_w = (double)cw;
+    a.x = x; a.grad_out = grad_out; a.loss_out = loss_out; a.d_x = d_x; a.accumulate = accumulate;
+    a.partials = static_cast<double*>(scratch);
+    return check_cuda(gsr_launch_tv_loss(a, GSR_ST(stream)), "tv_loss");
+}
+
+size_t b200gsr_scale_loss_scratch_bytes(int32_t rows) {
+    return rows < 1 || 3LL * rows > INT32_MAX ? 0 : (size_t)gsr_l2_blocks(3 * rows) * sizeof(double);
+}
+
+int b200gsr_scale_loss(int32_t rows, const float* scales, const float* grad_out, float* loss_out, float* d_scales,
+                       int32_t accumulate, void* scratch, size_t scratch_bytes, void* stream) {
+    if (rows < 1) return fail(B200GSR_ERR_BAD_ARG, "scale_loss: rows %d must be >= 1", rows);
+    if (3LL * rows > INT32_MAX) return fail(B200GSR_ERR_UNSUPPORTED, "scale_loss: at most 2^31 - 1 elements, got %lld", 3LL * rows);
+    if (accumulate != 0 && accumulate != 1) return fail(B200GSR_ERR_BAD_ARG, "scale_loss: accumulate must be 0 or 1");
+    if (!scales) return fail(B200GSR_ERR_BAD_ARG, "scale_loss: scales must be a device pointer");
+    if (!loss_out && !d_scales) return fail(B200GSR_ERR_BAD_ARG, "scale_loss: nothing to compute (loss_out and d_scales are null)");
+    if (d_scales && !grad_out) return fail(B200GSR_ERR_BAD_ARG, "scale_loss: d_scales needs grad_out");
+    if (loss_out && (!scratch || scratch_bytes < b200gsr_scale_loss_scratch_bytes(rows) || (uintptr_t)scratch % 8))
+        return fail(B200GSR_ERR_WORKSPACE, "scale_loss: scratch must be 8-byte aligned and hold %zu bytes (got %zu)",
+                    b200gsr_scale_loss_scratch_bytes(rows), scratch ? scratch_bytes : (size_t)0);
+    GsrScaleArgs a;
+    a.rows = rows;
+    a.inv_rows = 1.0f / (float)rows;        // MeanBackward0 / MeanBackward1: div by a CPU scalar
+    a.inv_3 = 1.0f / 3.0f;
+    a.scales = scales; a.grad_out = grad_out; a.loss_out = loss_out; a.d_scales = d_scales; a.accumulate = accumulate;
+    a.partials = static_cast<double*>(scratch);
+    return check_cuda(gsr_launch_scale_loss(a, GSR_ST(stream)), "scale_loss");
+}
+
 int b200gsr_debug_counters(unsigned long long* device_counters) {
     g_stats = device_counters;
     return B200GSR_OK;

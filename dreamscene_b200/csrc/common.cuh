@@ -416,3 +416,36 @@ struct GsrL2Args {
     double* partials;              // with loss_out
 };
 cudaError_t gsr_launch_recon_l2(const GsrL2Args& a, bool half_target, cudaStream_t s);
+
+// ---- b200gsr_tv_loss / b200gsr_scale_loss (include/b200gsr_loss.h, csrc/loss.cu) ------------------------------------
+// Total variation: a warp task is GSR_TV_ROWS rows x 32 lanes x V columns of one plane (V = 4 on the float4 path, 1 on
+// the scalar one), GSR_L2_THREADS / 32 tasks per CTA; with a loss each CTA writes one (h, w) pair of double partials.
+constexpr int GSR_TV_ROWS = 8;
+inline long long gsr_tv_blocks(long long planes, int32_t H, int32_t W, int V) {
+    const long long tasks = planes * ((H + GSR_TV_ROWS - 1) / GSR_TV_ROWS) * ((W + 32LL * V - 1) / (32LL * V));
+    return (tasks + GSR_L2_THREADS / 32 - 1) / (GSR_L2_THREADS / 32);
+}
+struct GsrTvArgs {
+    int32_t B, planes, H, W;        // planes = B C
+    float inv_b, inv_h, inv_w;      // fp32(1 / B), fp32(1 / (C (H-1) W)), fp32(1 / (C H (W-1))): torch's reciprocals
+    double count_h, count_w;        // C (H-1) W, C H (W-1)
+    const float* x;
+    const float* grad_out;          // with d_x
+    float* loss_out;                // NULL: no loss
+    float* d_x;                     // NULL: no gradient
+    int32_t accumulate;
+    double* partials;               // with loss_out: 2 per CTA of the scalar path's grid (the larger one)
+};
+cudaError_t gsr_launch_tv_loss(const GsrTvArgs& a, cudaStream_t s);
+// Scale loss over n = 3 rows elements: CTA b owns elements [b GSR_L2_CHUNK, (b + 1) GSR_L2_CHUNK) as recon_l2 does.
+struct GsrScaleArgs {
+    int32_t rows;
+    float inv_rows, inv_3;          // fp32(1 / rows), fp32(1 / 3)
+    const float* scales;
+    const float* grad_out;
+    float* loss_out;
+    float* d_scales;
+    int32_t accumulate;
+    double* partials;               // with loss_out: gsr_l2_blocks(3 rows)
+};
+cudaError_t gsr_launch_scale_loss(const GsrScaleArgs& a, cudaStream_t s);

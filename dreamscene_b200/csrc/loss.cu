@@ -157,3 +157,212 @@ cudaError_t launch(const GsrL2Args& a, cudaStream_t s) {
 cudaError_t gsr_launch_recon_l2(const GsrL2Args& a, bool half_target, cudaStream_t s) {
     return half_target ? launch<true>(a, s) : launch<false>(a, s);
 }
+
+// ---- the guidance stages' regularisers (DESIGN.md §0 f10) ----------------------------------------------------------
+// Total variation, tv(x) = 2 (h_tv / (C (H-1) W) + w_tv / (C H (W-1))) / B, and its gradient as torch's CUDA autograd
+// computes it for an incoming g:
+//   DivBackward (/ B), MulBackward (2 *)      g2 = 2 fp32(g * fp32(1 / B))       div by a CPU scalar: reciprocal multiply
+//   DivBackward (/ count), PowBackward        ch = fp32(fp32(g2 * fp32(1 / count_h)) * fp32(2 dh)), cw likewise
+//   SubBackward, SliceBackward                +c at the minuend, -c at the subtrahend, zero padded (+0)
+//   the input's gradient buffer               ((w+ + w-) + h-) + h+, autograd's arrival order
+// with w+ = +cw at [..., 1:], w- = -cw at [..., :-1], h+ / h- likewise along H.
+// Scale loss, mean(mean(scales, -1)): MeanBackward0 then MeanBackward1 give every element fp32(fp32(g * fp32(1 / rows))
+// * fp32(1 / 3)).
+namespace {
+
+// Fixed-order sums of two doubles per thread; the results are valid in thread 0.
+__device__ __forceinline__ void block_sum2(double& a, double& b) {
+    __shared__ double2 warp_sum[GSR_L2_THREADS / 32];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        a += __shfl_down_sync(0xffffffffu, a, o);
+        b += __shfl_down_sync(0xffffffffu, b, o);
+    }
+    if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = make_double2(a, b);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        a = 0.0; b = 0.0;
+        for (int w = 0; w < GSR_L2_THREADS / 32; ++w) { a += warp_sum[w].x; b += warp_sum[w].y; }
+    }
+}
+
+// V consecutive elements of row i starting at column j (zeros for an inactive lane)
+template <int V>
+__device__ __forceinline__ void load_row(const float* p, float (&v)[V], bool act) {
+    if constexpr (V == 4) {
+        const float4 q = act ? __ldg(reinterpret_cast<const float4*>(p)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
+    } else {
+        v[0] = act ? __ldg(p) : 0.0f;
+    }
+}
+
+// c = fp32(gs * fp32(2 (hi - lo))), one term of the gradient
+__device__ __forceinline__ float tv_term(float gs, float hi, float lo) {
+    return __fmul_rn(gs, __fmul_rn(2.0f, __fsub_rn(hi, lo)));
+}
+
+// grid gsr_tv_blocks(planes, H, W, V): warp task t covers rows [band 8, band 8 + 8) and columns [(chunk 32 + lane) V,
+// + V) of one plane, with the band's rows and a halo row above and below loaded into registers first; the left /
+// right neighbours come from the adjacent lanes, or from memory at the warp's edges.  V = 4 needs W % 4 == 0 and x, d_x 16-byte aligned.
+template <int V>
+__global__ void __launch_bounds__(GSR_L2_THREADS) tv_kernel(const GsrTvArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int H = a.H, W = a.W;
+    const int nchunk = (W + 32 * V - 1) / (32 * V);
+    const int nband = (H + GSR_TV_ROWS - 1) / GSR_TV_ROWS;
+    const long long task = (long long)blockIdx.x * (GSR_L2_THREADS / 32) + (threadIdx.x >> 5);
+    double sh = 0.0, sw = 0.0;
+    if (task < (long long)a.planes * nband * nchunk) {          // warp-uniform
+        const int chunk = (int)(task % nchunk);
+        const int band = (int)((task / nchunk) % nband);
+        const long long plane = task / ((long long)nchunk * nband);
+        const int j0 = (chunk * 32 + lane) * V;
+        const bool act = j0 < W;
+        const float* xp = a.x + plane * H * W;
+        float* dp = a.d_x ? a.d_x + plane * H * W : nullptr;
+        float gh = 0.0f, gw = 0.0f;
+        if (dp) {
+            const float g2 = __fmul_rn(2.0f, __fmul_rn(__ldg(a.grad_out), a.inv_b));
+            gh = __fmul_rn(g2, a.inv_h);
+            gw = __fmul_rn(g2, a.inv_w);
+        }
+        const int r0 = band * GSR_TV_ROWS;
+        float xs[GSR_TV_ROWS + 2][V];       // rows r0 - 1 .. r0 + GSR_TV_ROWS, all loads in flight at once
+#pragma unroll
+        for (int r = 0; r < GSR_TV_ROWS + 2; ++r) {
+            const int i = r0 - 1 + r;
+            load_row<V>(xp + (long long)min(max(i, 0), H - 1) * W + j0, xs[r], act && i >= 0 && i < H);
+        }
+#pragma unroll
+        for (int r = 1; r <= GSR_TV_ROWS; ++r) {
+            const int i = r0 - 1 + r;
+            if (i >= H) break;                                  // warp-uniform
+            const float(&up)[V] = xs[r - 1];
+            const float(&cur)[V] = xs[r];
+            const float(&dn)[V] = xs[r + 1];
+            const float* row = xp + (long long)i * W;
+            float xl = __shfl_up_sync(0xffffffffu, cur[V - 1], 1);
+            float xr = __shfl_down_sync(0xffffffffu, cur[0], 1);
+            if (lane == 0 && act && j0 > 0) xl = __ldg(row + j0 - 1);
+            if (lane == 31 && j0 + V < W) xr = __ldg(row + j0 + V);
+            if (act) {
+                float d[V];
+#pragma unroll
+                for (int k = 0; k < V; ++k) {
+                    const int j = j0 + k;
+                    const float left = k > 0 ? cur[k - 1] : xl;
+                    const float right = k < V - 1 ? cur[k + 1] : xr;
+                    if (a.loss_out) {
+                        if (i + 1 < H) { const float e = __fsub_rn(dn[k], cur[k]); sh += (double)__fmul_rn(e, e); }
+                        if (j + 1 < W) { const float e = __fsub_rn(right, cur[k]); sw += (double)__fmul_rn(e, e); }
+                    }
+                    if (dp) {
+                        const float wp = j > 0 ? tv_term(gw, cur[k], left) : 0.0f;
+                        const float wm = j + 1 < W ? -tv_term(gw, right, cur[k]) : 0.0f;
+                        const float hm = i + 1 < H ? -tv_term(gh, dn[k], cur[k]) : 0.0f;
+                        const float hp = i > 0 ? tv_term(gh, cur[k], up[k]) : 0.0f;
+                        d[k] = __fadd_rn(__fadd_rn(__fadd_rn(wp, wm), hm), hp);
+                    }
+                }
+                if (dp) {
+                    float* o = dp + (long long)i * W + j0;
+                    if constexpr (V == 4) {
+                        float4 q = make_float4(d[0], d[1], d[2], d[3]);
+                        if (a.accumulate) {
+                            const float4 p = *reinterpret_cast<const float4*>(o);
+                            q = make_float4(__fadd_rn(p.x, q.x), __fadd_rn(p.y, q.y), __fadd_rn(p.z, q.z),
+                                            __fadd_rn(p.w, q.w));
+                        }
+                        *reinterpret_cast<float4*>(o) = q;
+                    } else {
+                        o[0] = a.accumulate ? __fadd_rn(o[0], d[0]) : d[0];
+                    }
+                }
+            }
+        }
+    }
+    if (a.loss_out) {
+        block_sum2(sh, sw);
+        if (threadIdx.x == 0) { a.partials[2 * blockIdx.x] = sh; a.partials[2 * blockIdx.x + 1] = sw; }
+    }
+}
+
+// one CTA: the (h, w) partials summed in a fixed order, then the value in double, rounded once
+__global__ void __launch_bounds__(GSR_L2_THREADS) tv_finish_kernel(const GsrTvArgs a, int nblk) {
+    double h = 0.0, w = 0.0;
+    for (int i = threadIdx.x; i < nblk; i += GSR_L2_THREADS) { h += a.partials[2 * i]; w += a.partials[2 * i + 1]; }
+    block_sum2(h, w);
+    if (threadIdx.x == 0) *a.loss_out = __double2float_rn(2.0 * (h / a.count_h + w / a.count_w) / (double)a.B);
+}
+
+// grid gsr_l2_blocks(3 rows): CTA b owns elements [b CHUNK, min((b + 1) CHUNK, n)); float4 path when scales and
+// d_scales are 16-byte aligned, the < 4-element tail and unaligned buffers take the scalar loop.  The gradient is one
+// constant and reads nothing but d_scales when accumulating.
+__global__ void __launch_bounds__(GSR_L2_THREADS) scale_loss_kernel(const GsrScaleArgs a) {
+    const long long n = 3LL * a.rows;
+    const long long start = (long long)blockIdx.x * GSR_L2_CHUNK;
+    const long long end = start + GSR_L2_CHUNK < n ? start + GSR_L2_CHUNK : n;
+    float* ds = a.d_scales;
+    const float c = ds ? __fmul_rn(__fmul_rn(__ldg(a.grad_out), a.inv_rows), a.inv_3) : 0.0f;
+    double acc = 0.0;
+    long long i0 = start;
+    if (((reinterpret_cast<uintptr_t>(a.scales) | reinterpret_cast<uintptr_t>(ds)) & 15) == 0) {
+        const long long q0 = start >> 2;
+        const int nv = (int)((end - start) >> 2);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const int j = k * GSR_L2_THREADS + threadIdx.x;
+            if (j < nv) {
+                if (a.loss_out) {
+                    const float4 s = __ldg(reinterpret_cast<const float4*>(a.scales) + q0 + j);
+                    acc += ((double)s.x + (double)s.y) + ((double)s.z + (double)s.w);
+                }
+                if (ds) {
+                    float4* o = reinterpret_cast<float4*>(ds) + q0 + j;
+                    float4 q = make_float4(c, c, c, c);
+                    if (a.accumulate) {
+                        const float4 p = *o;
+                        q = make_float4(__fadd_rn(p.x, c), __fadd_rn(p.y, c), __fadd_rn(p.z, c), __fadd_rn(p.w, c));
+                    }
+                    *o = q;
+                }
+            }
+        }
+        i0 = start + 4LL * nv;
+    }
+    for (long long i = i0 + threadIdx.x; i < end; i += GSR_L2_THREADS) {
+        if (a.loss_out) acc += (double)__ldg(a.scales + i);
+        if (ds) ds[i] = a.accumulate ? __fadd_rn(ds[i], c) : c;
+    }
+    if (a.loss_out) {
+        const double s = block_sum(acc);
+        if (threadIdx.x == 0) a.partials[blockIdx.x] = s;
+    }
+}
+
+__global__ void __launch_bounds__(GSR_L2_THREADS) scale_finish_kernel(const GsrScaleArgs a, int nblk) {
+    double s = 0.0;
+    for (int i = threadIdx.x; i < nblk; i += GSR_L2_THREADS) s += a.partials[i];
+    s = block_sum(s);
+    if (threadIdx.x == 0) *a.loss_out = __double2float_rn(s / (3.0 * (double)a.rows));
+}
+
+}  // namespace
+
+cudaError_t gsr_launch_tv_loss(const GsrTvArgs& a, cudaStream_t s) {
+    const bool vec = a.W % 4 == 0 &&
+                     ((reinterpret_cast<uintptr_t>(a.x) | reinterpret_cast<uintptr_t>(a.d_x)) & 15) == 0;
+    const int nblk = (int)gsr_tv_blocks(a.planes, a.H, a.W, vec ? 4 : 1);
+    if (vec) tv_kernel<4><<<nblk, GSR_L2_THREADS, 0, s>>>(a);
+    else tv_kernel<1><<<nblk, GSR_L2_THREADS, 0, s>>>(a);
+    if (a.loss_out) tv_finish_kernel<<<1, GSR_L2_THREADS, 0, s>>>(a, nblk);
+    return cudaGetLastError();
+}
+
+cudaError_t gsr_launch_scale_loss(const GsrScaleArgs& a, cudaStream_t s) {
+    const int nblk = (int)gsr_l2_blocks(3 * a.rows);
+    scale_loss_kernel<<<nblk, GSR_L2_THREADS, 0, s>>>(a);
+    if (a.loss_out) scale_finish_kernel<<<1, GSR_L2_THREADS, 0, s>>>(a, nblk);
+    return cudaGetLastError();
+}

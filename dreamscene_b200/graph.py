@@ -22,14 +22,23 @@ Target mode (the refine stages' reconstruction step, f9) puts the loss into the 
     sg.render(settings_list, shs_aug=False, scale_aug=False, target_index=[i])   # render + recon_l2 loss + gradient
     sg.step()       # no eager loss, no .grad hand-off; sg.loss [B] holds each view's loss
 
+Regulariser mode (the guidance stages' step, f10) puts the reference's total-variation and scale regularisers into the
+graphs, so that the eager loss is the guidance term alone:
+
+    sg = StepGraph(groups, optimizers, views=B, height=H, width=W, tv_weight=1.0, tv_depth_weight=1.0,
+                   scale_weight=1.0)
+    out = sg.render(settings_list, ...)       # also sg.reg_loss [3] = tv(image), tv(disp), mean(mean(scales, -1))
+    guidance_loss(out.image).backward()       # eager
+    sg.step()       # adds weight * each regulariser's gradient to the outputs' gradients before the render backward
+
 ``step(optimize=False)`` replays the backward only (``grads`` and ``d_means2D``), leaving parameters, moments and
 step counters as they are: the reference's densify step, whose optimizer.step() follows densify_and_prune and so
 updates nothing.
 
 The first ``render()`` of a layout runs one eager forward and backward (which measure the pair capacity and set up
 the library) and then captures.  The layout - P, the group tensors, the optimizer state tensors, the per-view
-scale_modifier, deterministic mode and the target tensor and weight - is compared on the host at every ``render()``;
-a change (densify / prune) re-captures.
+scale_modifier, deterministic mode, the target tensor and weight and the regulariser weights - is compared on the
+host at every ``render()``; a change (densify / prune) re-captures.
 """
 from __future__ import annotations
 
@@ -64,10 +73,18 @@ class StepGraph:
 
     target: a CUDA [G,3,H,W] float16 / float32 contiguous tensor of pseudo ground truths, read in place at every
     replay.  The render graph then also computes view v's loss target_weight * mean((fp16(image_v) - target[i_v])^2)
-    (dreamscene_b200.losses.recon_l2_loss) into `loss` and its image gradient; the step minimises the views' sum."""
+    (dreamscene_b200.losses.recon_l2_loss) into `loss` and its image gradient; the step minimises the views' sum.
+
+    tv_weight / tv_depth_weight / scale_weight: the weights of the reference's regularisers tv_loss(image),
+    tv_loss(disp) and mean(mean(scales, -1)) (dreamscene_b200.losses.tv_loss), computed inside the graphs.  A term
+    whose weight is None or 0 is off.  The render graph writes the unweighted values into `reg_loss`; the backward
+    graph adds weight * each term's gradient to the gradient step() takes from the output's .grad, which is the
+    eager step's gradient bit for bit when the eager loss, written before the regularisers, reaches each output
+    through one edge.  Not with target (the refine stages use no regulariser)."""
 
     def __init__(self, groups: Sequence, optimizers: Sequence, *, views: int, height: int, width: int,
-                 target: torch.Tensor | None = None, target_weight: float = 100.0):
+                 target: torch.Tensor | None = None, target_weight: float = 100.0, tv_weight: float | None = None,
+                 tv_depth_weight: float | None = None, scale_weight: float | None = None):
         self.groups = list(groups)
         self.optimizers = list(optimizers)
         self.B, self.H, self.W = int(views), int(height), int(width)
@@ -78,12 +95,15 @@ class StepGraph:
                 raise TypeError(f"StepGraph: only GaussianAdam optimizers can be replayed, got {type(opt).__name__}")
         self.target, self.target_weight = target, float(target_weight)
         self._target_key()
+        self.tv_weight, self.tv_depth_weight, self.scale_weight = tv_weight, tv_depth_weight, scale_weight
+        self._reg_key()
         self._key = None
         self._report = None         # device [2]: max pair count, overflowed replays; kept across re-captures
         self._scratch_key = None
         self.d_means2D = None       # [B,P,3] per-view screen-space gradients of the last step (densification stats)
         self.grads = None           # per group {leaf name: its gradient of the last step} (the backward graph's buffers)
         self.loss = None            # target mode: [B] each view's loss of the last render(), in the target's dtype
+        self.reg_loss = None        # with a regulariser: [3] float32 tv(image), tv(disp), scale of the last render()
 
     def _target_key(self):
         """Host checks of `target` (its device is checked in render()) -> its part of the layout key, None without."""
@@ -99,6 +119,25 @@ class StepGraph:
         if 3 * self.H * self.W >= 2 ** 31:
             raise ValueError("StepGraph: target mode needs 3 H W < 2^31")
         return t.data_ptr(), t.dtype, tuple(t.shape), self.target_weight
+
+    def _reg_key(self):
+        """Host checks of the regulariser weights -> the weights of the terms that are on (tv(image), tv(disp),
+        scale; None for a term that is off), part of the layout key."""
+        out = []
+        for name in ("tv_weight", "tv_depth_weight", "scale_weight"):
+            w = getattr(self, name)
+            if w is not None:
+                w = float(w)
+                if not (0.0 <= w < float("inf")):
+                    raise ValueError(f"StepGraph: {name} must be finite and >= 0, got {w}")
+            out.append(w if w else None)
+        if any(w is not None for w in out):
+            if self.target is not None:
+                raise ValueError("StepGraph: the regularisers (tv_weight, tv_depth_weight, scale_weight) cannot be "
+                                 "combined with target=")
+            if (out[0] is not None or out[1] is not None) and (self.H < 2 or self.W < 2):
+                raise ValueError("StepGraph: the total-variation regularisers need height and width >= 2")
+        return tuple(out)
 
     def _target_indices(self, target_index):
         """-> the B validated target indices, or None without a target."""
@@ -141,7 +180,8 @@ class StepGraph:
                 for p in group["params"]:
                     st = opt.state.get(p, {})
                     states.append((id(p), st["exp_avg"].data_ptr() if st else 0, st["exp_avg_sq"].data_ptr() if st else 0))
-        return (P, M, ptrs, tuple(states), tuple(float(s.scale_modifier) for s in settings), det, self._target_key())
+        return (P, M, ptrs, tuple(states), tuple(float(s.scale_modifier) for s in settings), det, self._target_key(),
+                self._reg_key())
 
     def _upload(self, settings, rec, seed, focal, tidx):
         """One pinned staging tensor, one non_blocking copy of it (plus one device concatenation when the cameras
@@ -273,6 +313,29 @@ class StepGraph:
             ones = torch.ones(B, dtype=target.dtype, device=dev)
             l2_scratch = torch.empty(lib.b200gsr_recon_l2_scratch_bytes(B, 3 * H * W), dtype=torch.uint8, device=dev)
             keep.append((ones, l2_scratch))
+        reg = self._reg_key()
+        reg_loss = None
+        if any(w is not None for w in reg):
+            # each term's value into reg_loss, and weight * its gradient added to the output's gradient buffer
+            reg_loss = torch.zeros(3, dtype=torch.float32, device=dev)
+            reg_go = torch.tensor([w or 0.0 for w in reg], dtype=torch.float32, device=dev)
+            tv_scratch = [torch.empty(lib.b200gsr_tv_loss_scratch_bytes(B, c, H, W), dtype=torch.uint8, device=dev)
+                          for c in (3, 1)]
+            scale_scratch = torch.empty(lib.b200gsr_scale_loss_scratch_bytes(B * P), dtype=torch.uint8, device=dev)
+            keep.append((reg_go, tv_scratch, scale_scratch))
+
+        def regularisers(forward, scale_acc=1):
+            for k, (x, c, gx) in enumerate(((image, 3, g_image), (disp, 1, g_disp))):
+                if reg[k] is not None:
+                    _lib.check(lib.b200gsr_tv_loss(B, c, H, W, ptr(x), None if forward else ptr(reg_go[k]),
+                                                   ptr(reg_loss[k]) if forward else None, None if forward else ptr(gx),
+                                                   1, ptr(tv_scratch[k]), tv_scratch[k].numel(), _lib.stream(dev)),
+                               "b200gsr_tv_loss")
+            if reg[2] is not None:
+                _lib.check(lib.b200gsr_scale_loss(B * P, ptr(scales), None if forward else ptr(reg_go[2]),
+                                                  ptr(reg_loss[2]) if forward else None,
+                                                  None if forward else ptr(g_scales), scale_acc, ptr(scale_scratch),
+                                                  scale_scratch.numel(), _lib.stream(dev)), "b200gsr_scale_loss")
 
         def launch(cap, flags, scratch, saved, notify_ptr, seq):
             return lib.b200gsr_forward_scene_dyn(B, prm, ng, table, views_p, seed_p, ptr(scales), ptr(color), ptr(da),
@@ -291,8 +354,12 @@ class StepGraph:
                                                 self.target_weight, ptr(ones), ptr(loss), ptr(g_image),
                                                 ptr(l2_scratch), l2_scratch.numel(), _lib.stream(dev)),
                            "b200gsr_recon_l2")
+            if reg_loss is not None:
+                regularisers(True)
 
-        def backward(saved, cap):
+        def backward(saved, cap, scale_acc=1):
+            if reg_loss is not None:
+                regularisers(False, scale_acc)
             g_color.view(3, B, Hp, W)[:, :, :H].copy_(g_image.permute(1, 0, 2, 3))
             stats_bwd.copy_(stats)
             _lib.check(lib.b200gsr_disparity_backward_ex(B, H * W, ptr(da4), ptr(focal), ptr(g_disp), ptr(g_alpha),
@@ -336,6 +403,14 @@ class StepGraph:
                 render(saved)
             with torch.cuda.graph(g_backward, pool=pool):
                 backward(saved, cap)
+            # with the scale regulariser, a second backward graph that writes its constant gradient into g_scales
+            # instead of adding it, for steps whose loss leaves out.scales without a .grad (the guidance stages'
+            # usual case): it saves a fill and a read of the [B,P,3] buffer
+            g_backward_w = None
+            if reg[2] is not None:
+                g_backward_w = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g_backward_w, pool=pool):
+                    backward(saved, cap, scale_acc=0)
             if g_adam is not None:
                 with torch.cuda.graph(g_adam, pool=pool):
                     for i0, arr in tables:
@@ -345,8 +420,10 @@ class StepGraph:
         if target is None:
             for t in (image, disp, alpha, scales):
                 t.requires_grad_(True)
-        self._graphs = (g_render, g_backward, g_adam)
+        self._graphs = (g_render, g_backward, g_adam, g_backward_w)
         self.loss = loss
+        self.reg_loss = reg_loss
+        self._accumulated = [reg[0] is not None, reg[1] is not None, False, reg[2] is not None]
         self._keep = (keep, prm, table, garr, tables, raw, saved, color, da, da4, stats, stats_bwd, g_color, g_da, d_da4)
         self._static_grads = (g_image, g_disp, g_alpha, g_scales)
         self._leaves = list(flat)
@@ -369,6 +446,7 @@ class StepGraph:
         S._check_device(flat)
         rec = self._views(settings_list, shs_aug, scale_aug, M)
         tidx = self._target_indices(target_index)
+        self._reg_key()
         if tidx is not None and (self.target.device.type != "cuda" or self.target.device != flat[0].device):
             raise ValueError("StepGraph: target must be a CUDA tensor on the groups' device")
         if seed is None:
@@ -390,11 +468,11 @@ class StepGraph:
 
     def step(self, optimize: bool = True) -> None:
         """Replay the backward graph: the render backward with the .grad of image / disp / alpha / scales (a missing
-        grad counts as zeros; in target mode the loss's image gradient from the render graph instead), the disparity
-        backward; then, with `optimize`, the Adam graph: every optimizer's step.  The leaf gradients come from out.*
-        only: a leaf that holds a .grad of its own (a loss term that reaches it directly, or a gradient not cleared
-        since an eager step) is refused rather than dropped.  Afterwards `grads` holds the leaf gradients and
-        d_means2D the per-view screen-space gradients.
+        grad counts as zeros; in target mode the loss's image gradient from the render graph instead) plus each
+        regulariser's weighted gradient, the disparity backward; then, with `optimize`, the Adam graph: every
+        optimizer's step.  The leaf gradients come from out.* only: a leaf that holds a .grad of its own (a loss term
+        that reaches it directly, or a gradient not cleared since an eager step) is refused rather than dropped.
+        Afterwards `grads` holds the leaf gradients and d_means2D the per-view screen-space gradients.
 
         optimize=False leaves parameters, moments and step counters untouched, as the reference's optimizer.step()
         after densify_and_prune (whose new leaves have no gradient) does.  A step where only some leaves skip Adam
@@ -408,12 +486,18 @@ class StepGraph:
                                    "the leaf gradients from out.image / disp / alpha / scales only and would discard "
                                    "it. Clear the leaves' gradients (optimizer.zero_grad()) and route every loss term "
                                    "through the outputs")
+        # the backward graph that writes the scale regulariser's gradient into g_scales, when there is no eager
+        # gradient of out.scales to add it to
+        write_scales = self._graphs[3] is not None and self.out.scales.grad is None
         if self.loss is None:
-            for t, g in zip((self.out.image, self.out.disp, self.out.alpha, self.out.scales), self._static_grads):
-                if t.grad is None:
-                    g.zero_()
-                else:
+            for t, g, acc in zip((self.out.image, self.out.disp, self.out.alpha, self.out.scales), self._static_grads,
+                                 self._accumulated):
+                if t.grad is not None:
                     g.copy_(t.grad)
+                elif not acc:
+                    g.zero_()
+                elif not (write_scales and t is self.out.scales):
+                    g.fill_(-0.0)       # -0 + r == r bitwise, the sign of zero included: the regulariser's gradient
                 t.grad = None
         if optimize:
             records = self._adam_records()      # this step's lr / betas / eps; same tensors as at capture (the layout)
@@ -422,7 +506,7 @@ class StepGraph:
                 stage = torch.tensor([O.adam_scalars(lr, b1, b2, eps, st.item())
                                       for _, _, _, _, lr, b1, b2, eps, st in records], dtype=torch.float32).pin_memory()
                 self._scalars[:len(records)].copy_(stage, non_blocking=True)
-        self._graphs[1].replay()
+        self._graphs[3 if write_scales else 1].replay()
         if optimize and self._graphs[2] is not None:
             self._graphs[2].replay()
 

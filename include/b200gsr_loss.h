@@ -1,6 +1,7 @@
 /*
- * b200gsr_loss.h - the reconstruction loss of DreamScene's refine stages and its image gradient (additive to b200gsr.h,
- * same conventions and the same library, libb200gsr.so; ABI version unchanged).
+ * b200gsr_loss.h - the reconstruction loss of DreamScene's refine stages and its image gradient, and the guidance
+ * stages' total-variation and scale regularisers (additive to b200gsr.h, same conventions and the same library,
+ * libb200gsr.so; ABI version unchanged).
  *
  * B independent losses over N elements each; view v is image[v N .. (v + 1) N):
  *
@@ -25,6 +26,24 @@
  *                    bitwise reproducible.
  *
  * At least one of loss_out and d_image.  No memset, no allocation, no host sync.
+ *
+ * The guidance stages' regularisers (DESIGN.md f10), same conventions:
+ *
+ *   b200gsr_tv_loss     loss = 2 * (h_tv / (C (H-1) W) + w_tv / (C H (W-1))) / B over x [B,C,H,W], where h_tv / w_tv
+ *                       are the sums of the squared differences of vertically / horizontally adjacent elements (the
+ *                       reference's tv_loss).  H >= 2, W >= 2, at most 2^31 - 1 elements.
+ *   b200gsr_scale_loss  loss = mean(mean(scales, -1)) over scales [rows, 3], at most 2^31 - 1 elements.
+ *
+ *   x / scales     : DEVICE float, contiguous.  Always required (the scale gradient does not read it).
+ *   grad_out       : DEVICE float [1], the incoming gradient of the loss.  Needed only with d_x / d_scales.
+ *   loss_out       : DEVICE float [1], or NULL for no loss.  A fixed-order double sum, bitwise reproducible.
+ *   d_x / d_scales : DEVICE float of x's / scales' shape, or NULL for no gradient.  Bit for bit torch's CUDA
+ *                    autograd gradient of the expression for grad_out (DESIGN.md f10).  With accumulate = 1 the
+ *                    gradient g is added to what the buffer holds (d = d + g, one fp32 add per element), else it is
+ *                    written.
+ *   scratch        : DEVICE, at least *_scratch_bytes(...) bytes, 8-byte aligned; needed only with loss_out.
+ *
+ * At least one of loss_out and the gradient.  No memset, no allocation, no host sync.
  */
 #ifndef B200GSR_LOSS_H
 #define B200GSR_LOSS_H
@@ -39,6 +58,12 @@ size_t b200gsr_recon_l2_scratch_bytes(int32_t B, int32_t N);
 int b200gsr_recon_l2(int32_t B, int32_t N, const float* image, const void* target, int32_t target_is_half,
                      int32_t n_targets, const int32_t* target_index, float weight, const void* grad_out,
                      void* loss_out, float* d_image, void* scratch, size_t scratch_bytes, void* stream);
+size_t b200gsr_tv_loss_scratch_bytes(int32_t B, int32_t C, int32_t H, int32_t W);
+int b200gsr_tv_loss(int32_t B, int32_t C, int32_t H, int32_t W, const float* x, const float* grad_out, float* loss_out,
+                    float* d_x, int32_t accumulate, void* scratch, size_t scratch_bytes, void* stream);
+size_t b200gsr_scale_loss_scratch_bytes(int32_t rows);
+int b200gsr_scale_loss(int32_t rows, const float* scales, const float* grad_out, float* loss_out, float* d_scales,
+                       int32_t accumulate, void* scratch, size_t scratch_bytes, void* stream);
 
 #ifdef __cplusplus
 }
