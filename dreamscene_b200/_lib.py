@@ -1,5 +1,5 @@
 """ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h,
-include/b200gsr_loss.h).  Fails loudly if the library is missing:
+include/b200gsr_loss.h, include/b200gsr_frozen.h).  Fails loudly if the library is missing:
 there is NO CPU or PyTorch fallback in the product path."""
 from __future__ import annotations
 
@@ -141,6 +141,15 @@ LOSS_SIGNATURES = {
     "b200gsr_scale_loss": (C.c_int, [i32, vp, vp, vp, vp, i32, vp, sz, vp]),
 }
 
+# The frozen-group backwards of include/b200gsr_frozen.h (same library), in that header's order: the arguments of
+# b200gsr_backward_scene / _dyn plus the uint32 frozen_groups mask before the stream.
+FROZEN_SIGNATURES = {
+    "b200gsr_backward_scene_frozen": (C.c_int, [i32, _P(Params), i32, _P(Group), _P(GroupGrad), vp, vp, u64] +
+                                      [vp] * 6 + [sz, u64, vp, u32, u32, vp]),
+    "b200gsr_backward_scene_dyn_frozen": (C.c_int, [i32, _P(Params), i32, _P(Group), _P(GroupGrad), vp, vp] +
+                                          [vp] * 6 + [sz, u64, vp, u32, u32, vp]),
+}
+
 _lib = None
 ABI_VERSION = 3
 ERR_BAD_ARG = -1
@@ -169,7 +178,8 @@ def load():
                 f"{LIB_PATH} is missing and could not be built ({err}). Build it with "
                 "`python -m dreamscene_b200._build` (needs nvcc; sm_90a only). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES, **STEP_SIGNATURES, **LOSS_SIGNATURES}.items():
+    for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES, **STEP_SIGNATURES, **LOSS_SIGNATURES,
+                                      **FROZEN_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:

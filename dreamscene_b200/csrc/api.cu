@@ -3,6 +3,7 @@
 #include "common.cuh"
 #include "../../include/b200gsr_step.h"
 #include "../../include/b200gsr_loss.h"
+#include "../../include/b200gsr_frozen.h"
 
 #include <cstdarg>
 #include <cstdio>
@@ -936,18 +937,20 @@ int b200gsr_forward_scene_dyn(int32_t B, const b200gsr_params* prm, int32_t num_
                          scratch_bytes, saved, saved_bytes, max_pairs, flags, host_notify, notify_seq, stream);
 }
 
-// b200gsr_backward_scene and b200gsr_backward_scene_dyn
+// b200gsr_backward_scene, b200gsr_backward_scene_dyn (frozen = 0) and their _frozen variants (include/b200gsr_frozen.h)
 static int backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
                           const b200gsr_group_grad* grads, GsrScene sc, bool dyn, const float* d_scales,
                           const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
                           const float* dL_ddepth_alpha, void* saved, size_t saved_bytes, uint64_t max_pairs,
-                          float* d_means2D, uint32_t flags, void* stream) {
+                          float* d_means2D, uint32_t flags, uint32_t frozen, void* stream) {
     int rc = check_scene(B, prm, num_groups, groups, sc, dyn);
     if (rc) return rc;
     if (flags & ~B200GSR_BWD_DETERMINISTIC) return fail(B200GSR_ERR_BAD_ARG, "unknown flags 0x%x", flags);
+    if (frozen >> num_groups)      // num_groups <= B200GSR_MAX_GROUPS < 32 (check_scene)
+        return fail(B200GSR_ERR_BAD_ARG, "frozen mask 0x%x has bits at or above num_groups %d", frozen, num_groups);
     if (num_groups > 0 && !grads) return fail(B200GSR_ERR_BAD_ARG, "grads is null");
     for (int g = 0; g < num_groups; ++g)
-        if (groups[g].n > 0 && (!grads[g].xyz || !grads[g].opacity || !grads[g].scaling || !grads[g].rotation ||
+        if (groups[g].n > 0 && !((frozen >> g) & 1u) && (!grads[g].xyz || !grads[g].opacity || !grads[g].scaling || !grads[g].rotation ||
                                 !grads[g].f_dc || (prm[0].M > 1 && !grads[g].f_rest)))
             return fail(B200GSR_ERR_BAD_ARG, "group %d: null gradient pointer", g);
     const int P = prm[0].P;
@@ -958,7 +961,7 @@ static int backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_grou
     if ((rc = setup_backward(true, B, prm, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes,
                              max_pairs, (flags & B200GSR_BWD_DETERMINISTIC) != 0, stream, a)))
         return rc;
-    sc.num_groups = num_groups; sc.groups = groups; sc.grads = grads; sc.d_scales = d_scales;
+    sc.num_groups = num_groups; sc.groups = groups; sc.grads = grads; sc.d_scales = d_scales; sc.frozen = frozen;
     a.scene = &sc;
     a.g_begin = 0; a.g_end = P;
     prof_mark_bwd(0, a.stream);
@@ -988,7 +991,7 @@ int b200gsr_backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_gro
     GsrScene sc{};
     sc.shs_noise = shs_noise; sc.scale_noise = scale_noise; sc.seed = seed;
     return backward_scene(B, prm, num_groups, groups, grads, sc, false, d_scales, radii, out_depth_alpha, dL_dcolor,
-                          dL_ddepth_alpha, saved, saved_bytes, max_pairs, d_means2D, flags, stream);
+                          dL_ddepth_alpha, saved, saved_bytes, max_pairs, d_means2D, flags, 0u, stream);
 }
 
 int b200gsr_backward_scene_dyn(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
@@ -999,7 +1002,32 @@ int b200gsr_backward_scene_dyn(int32_t B, const b200gsr_params* prm, int32_t num
     GsrScene sc{};
     sc.dyn_views = views; sc.dyn_seed = reinterpret_cast<const unsigned long long*>(seed);
     return backward_scene(B, prm, num_groups, groups, grads, sc, true, d_scales, radii, out_depth_alpha, dL_dcolor,
-                          dL_ddepth_alpha, saved, saved_bytes, max_pairs, d_means2D, flags, stream);
+                          dL_ddepth_alpha, saved, saved_bytes, max_pairs, d_means2D, flags, 0u, stream);
+}
+
+int b200gsr_backward_scene_frozen(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
+                                  const b200gsr_group_grad* grads, const float* shs_noise, const float* scale_noise,
+                                  uint64_t seed, const float* d_scales, const int32_t* radii,
+                                  const float* out_depth_alpha, const float* dL_dcolor, const float* dL_ddepth_alpha,
+                                  void* saved, size_t saved_bytes, uint64_t max_pairs, float* d_means2D,
+                                  uint32_t flags, uint32_t frozen_groups, void* stream) {
+    GsrScene sc{};
+    sc.shs_noise = shs_noise; sc.scale_noise = scale_noise; sc.seed = seed;
+    return backward_scene(B, prm, num_groups, groups, grads, sc, false, d_scales, radii, out_depth_alpha, dL_dcolor,
+                          dL_ddepth_alpha, saved, saved_bytes, max_pairs, d_means2D, flags, frozen_groups, stream);
+}
+
+int b200gsr_backward_scene_dyn_frozen(int32_t B, const b200gsr_params* prm, int32_t num_groups,
+                                      const b200gsr_group* groups, const b200gsr_group_grad* grads,
+                                      const b200gsr_step_view* views, const uint64_t* seed, const float* d_scales,
+                                      const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
+                                      const float* dL_ddepth_alpha, void* saved, size_t saved_bytes,
+                                      uint64_t max_pairs, float* d_means2D, uint32_t flags, uint32_t frozen_groups,
+                                      void* stream) {
+    GsrScene sc{};
+    sc.dyn_views = views; sc.dyn_seed = reinterpret_cast<const unsigned long long*>(seed);
+    return backward_scene(B, prm, num_groups, groups, grads, sc, true, d_scales, radii, out_depth_alpha, dL_dcolor,
+                          dL_ddepth_alpha, saved, saved_bytes, max_pairs, d_means2D, flags, frozen_groups, stream);
 }
 
 int b200gsr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix,

@@ -218,6 +218,9 @@ struct GsrScene {
     // shs_noise / scale_noise / seed and the views' tanfovx / tanfovy / sh_degree (both null otherwise)
     const b200gsr_step_view* dyn_views;
     const unsigned long long* dyn_seed;
+    // backward (b200gsr_backward_scene[_dyn]_frozen): bit g = group g is frozen; its leaves get no gradient and
+    // composite_bwd / project_bwd run their FROZEN instantiations.  0 = the default kernels.
+    uint32_t frozen;
 };
 
 struct GsrFwdArgs {

@@ -20,6 +20,7 @@
 //     butterfly (12 SHFL for 10 values) and committed with ONE coalesced RED instruction.
 #include "common.cuh"
 #include <cuda_fp16.h>
+#include <type_traits>
 
 namespace {
 
@@ -423,9 +424,34 @@ __device__ __forceinline__ void halve2(float (&v)[10], bool hi) {
     if (Hh & 1) v[Hh - 1] = keep[Hh - 1] + recv[Hh - 1];
 }
 
+// Frozen groups (b200gsr_backward_scene_frozen): the packed rows of the frozen groups as merged half-open intervals
+// [lo, lo + len).  Adjacent frozen groups merge, so 24 groups give at most 12 intervals.
+constexpr int kMaxFrozenIntervals = (B200GSR_MAX_GROUPS + 1) / 2;
+struct NoFrozen {};
+struct FrozenRows {
+    uint32_t n;                              // intervals in use
+    uint32_t P_view;                         // record index q2.w of view v's row r is v * P_view + r
+    uint32_t lo[kMaxFrozenIntervals], len[kMaxFrozenIntervals];
+};
+template <bool FROZEN>
+using FrozenArg = std::conditional_t<FROZEN, FrozenRows, NoFrozen>;
+// A loop over the intervals in use, reading them from the constant bank (fz is a __grid_constant__ parameter, so the
+// dynamic index needs no local copy).  Unrolled over all twelve slots, the test cost every entry about as much as
+// the gradient body it saves on a frozen one (composite_bwd 0.77 -> 1.00 ms with one interval, H100).
+__device__ __forceinline__ bool row_frozen(const FrozenRows& f, uint32_t row) {
+#pragma unroll 1
+    for (uint32_t k = 0; k < f.n; ++k)
+        if (row - f.lo[k] < f.len[k]) return true;
+    return false;
+}
+
 // ACC: how the butterfly's per-(warp item, Gaussian) totals are committed (GSR_ACC_*).  Every commit is a
 // butterfly total, a function of its work item alone, which the deterministic passes rely on.
-template <bool STATS, int ACC = GSR_ACC_FLOAT>
+// FROZEN (STATS false): an entry whose row lies in one of fz's intervals only advances the transmittance and colour
+// recurrences, which the entries behind it need; its gradient body, butterfly, commit and (pass B) dmax load are
+// skipped, so its dgeom / dmax / dfx rows are never written.  The test is warp-uniform (every lane reads the same
+// record) and needs no load beyond the record part 2 that the recurrence reads anyway.
+template <bool STATS, int ACC = GSR_ACC_FLOAT, bool FROZEN = false>
 __global__ void __launch_bounds__(kWarps * 32, kMinCtas)
 composite_bwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, const uint32_t* __restrict__ header,
                      const uint32_t* __restrict__ work_order,
@@ -436,7 +462,8 @@ composite_bwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, cons
                      const uint32_t* __restrict__ n_contrib, const float* __restrict__ dL_dcolor,
                      const float* __restrict__ dL_ddepth_alpha, float* __restrict__ dgeom,
                      unsigned long long* __restrict__ stats, const uint32_t* __restrict__ bwd_items,
-                     uint32_t* __restrict__ dmax, unsigned long long* __restrict__ dfx) {
+                     uint32_t* __restrict__ dmax, unsigned long long* __restrict__ dfx,
+                     const __grid_constant__ FrozenArg<FROZEN> fz) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     SmemRing& sm = *reinterpret_cast<SmemRing*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -581,6 +608,21 @@ composite_bwd_kernel(int H, int W, int gx, int gy_view, int Hs, int ntiles, cons
                 if (STATS) ++st_eval;
                 if (cm == 0u) continue;
                 const float4 q2 = rp[2];
+                if constexpr (FROZEN) {
+                    if (row_frozen(fz, __float_as_uint(q2.w) - (uint32_t)view * fz.P_view)) {
+                        // the recurrence statements of the body below, in its order
+                        const float am = contrib ? alpha : 0.0f;
+                        const float rom = rcp_approx(1.0f - am);
+                        T = contrib ? T * rom : T;
+                        const float2 c01 = make_float2(q2.x, q2.y), c2D = make_float2(q2.z, q1.w);
+                        const float2 nacc01 = make_float2(-acc01.x, -acc01.y), nacc2D = make_float2(-acc2D.x, -acc2D.y);
+                        const float2 d01 = fadd2_rn(c01, nacc01), d2D = fadd2_rn(c2D, nacc2D);
+                        const float2 am2 = make_float2(am, am);
+                        acc01 = ffma2_rn(am2, d01, acc01);
+                        acc2D = ffma2_rn(am2, d2D, acc2D);
+                        continue;
+                    }
+                }
                 uint32_t det_mb = 0u;   // pass B: issued here so that its latency hides behind the body and butterfly
                 if (ACC == GSR_ACC_DET_SUM && commit_lane)
                     det_mb = __ldg(dmax + GSR_DET_COMPONENTS * (size_t)__float_as_uint(q2.w) + vidx);
@@ -762,19 +804,40 @@ cudaError_t gsr_launch_score_finish(int n, const unsigned long long* score_fx, f
     return cudaGetLastError();
 }
 
-template <bool STATS, int ACC = GSR_ACC_FLOAT>
+template <bool STATS, int ACC = GSR_ACC_FLOAT, bool FROZEN = false>
 static cudaError_t launch_bwd(const GsrBwdArgs& a, const CompPtrs& c, uint32_t* queue, float* dgeom,
-                              uint32_t* dmax = nullptr, unsigned long long* dfx = nullptr) {
+                              uint32_t* dmax = nullptr, unsigned long long* dfx = nullptr,
+                              const FrozenArg<FROZEN>& fz = {}) {
     const int smem = (int)sizeof(SmemRing);
     const int nblocks = min(c.grid.ntiles, a.num_sms * kMinCtas);
     static std::atomic<unsigned long long> attr_done{0};
-    cudaError_t e = gsr_smem_once(composite_bwd_kernel<STATS, ACC>, smem, attr_done);
+    cudaError_t e = gsr_smem_once(composite_bwd_kernel<STATS, ACC, FROZEN>, smem, attr_done);
     if (e != cudaSuccess) return e;
-    composite_bwd_kernel<STATS, ACC><<<nblocks, kWarps * 32, smem, a.stream>>>(
+    composite_bwd_kernel<STATS, ACC, FROZEN><<<nblocks, kWarps * 32, smem, a.stream>>>(
         a.prm.image_height, a.prm.image_width, c.grid.gx, a.gy_view, c.H, c.grid.ntiles, c.header, c.work_order, c.tile_start,
         c.keys, c.geom, a.prm.bg, queue, a.out_depth_alpha, c.n_contrib, a.dL_dcolor, a.dL_ddepth_alpha, dgeom,
-        a.stats, c.bwd_items, dmax, dfx);
+        a.stats, c.bwd_items, dmax, dfx, fz);
     return cudaGetLastError();
+}
+
+// The frozen groups' packed rows (bit g of sc.frozen: group g) as merged intervals; empty groups merge away.
+static FrozenRows frozen_rows(const GsrScene& sc, int P_view) {
+    FrozenRows f{};
+    f.P_view = (uint32_t)P_view;
+    uint32_t row = 0;
+    for (int g = 0; g < sc.num_groups; ++g) {
+        const uint32_t n = (uint32_t)sc.groups[g].n;
+        if (n > 0 && ((sc.frozen >> g) & 1u)) {
+            if (f.n > 0 && f.lo[f.n - 1] + f.len[f.n - 1] == row) {
+                f.len[f.n - 1] += n;
+            } else {
+                f.lo[f.n] = row; f.len[f.n] = n;
+                ++f.n;
+            }
+        }
+        row += n;
+    }
+    return f;
 }
 
 cudaError_t gsr_launch_composite_bwd(const GsrBwdArgs& a) {
@@ -782,18 +845,30 @@ cudaError_t gsr_launch_composite_bwd(const GsrBwdArgs& a) {
     if (c.grid.ntiles == 0) return cudaSuccess;
     uint32_t* queue = reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE;
     float* dgeom = reinterpret_cast<float*>(a.saved + a.vl.dgeom);
+    // Frozen groups: the FROZEN instantiations; the instrumented kernel has no such mode and the counters are left
+    // untouched, as in deterministic mode.
+    const bool frozen = a.scene != nullptr && a.scene->frozen != 0u;
+    const FrozenRows fz = frozen ? frozen_rows(*a.scene, a.P_view) : FrozenRows{};
     if (a.det) {
         // Deterministic mode: the default kernel with integer commits, run twice (instrumentation does not apply).
         // Pass B pops its own work queue (header words, zero between calls like the first one): no memset.
         uint32_t* dmax = reinterpret_cast<uint32_t*>(a.saved + a.dl.dmax);
         unsigned long long* dfx = reinterpret_cast<unsigned long long*>(a.saved + a.dl.dfx);
         uint32_t* queue_b = reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE_DET;
-        cudaError_t e = launch_bwd<false, GSR_ACC_DET_MAX>(a, c, queue, dgeom, dmax, dfx);
-        if (e == cudaSuccess) e = launch_bwd<false, GSR_ACC_DET_SUM>(a, c, queue_b, dgeom, dmax, dfx);
+        cudaError_t e;
+        if (frozen) {
+            e = launch_bwd<false, GSR_ACC_DET_MAX, true>(a, c, queue, dgeom, dmax, dfx, fz);
+            if (e == cudaSuccess) e = launch_bwd<false, GSR_ACC_DET_SUM, true>(a, c, queue_b, dgeom, dmax, dfx, fz);
+        } else {
+            e = launch_bwd<false, GSR_ACC_DET_MAX>(a, c, queue, dgeom, dmax, dfx);
+            if (e == cudaSuccess) e = launch_bwd<false, GSR_ACC_DET_SUM>(a, c, queue_b, dgeom, dmax, dfx);
+        }
         if (e != cudaSuccess) return e;
         const int n = a.num_views * a.P_view;
+        // frozen rows: their dmax / dfx rows are zero, so they resolve to dgeom rows of zeros
         det_resolve_kernel<<<(n + 255) / 256, 256, 0, a.stream>>>(n, a.radii, dmax, dfx, dgeom, queue_b);
         return cudaGetLastError();
     }
+    if (frozen) return launch_bwd<false, GSR_ACC_FLOAT, true>(a, c, queue, dgeom, nullptr, nullptr, fz);
     return a.stats != nullptr ? launch_bwd<true>(a, c, queue, dgeom) : launch_bwd<false>(a, c, queue, dgeom);
 }

@@ -268,8 +268,15 @@ struct SceneFwdDyn : SceneFwd { SceneDyn dyn; };
 struct SceneBwdDyn : SceneBwd { SceneDyn dyn; };
 template <bool RAW, bool DYN>
 using FwdScene = std::conditional_t<RAW, std::conditional_t<DYN, SceneFwdDyn, SceneFwd>, NoScene>;
-template <bool RAW, bool DYN>
-using BwdScene = std::conditional_t<RAW, std::conditional_t<DYN, SceneBwdDyn, SceneBwd>, NoScene>;
+// FROZEN (with RAW): bit g of `frozen` = group g is frozen (b200gsr_backward_scene_frozen).  A derived type, so that
+// the other instantiations' kernel argument keeps its layout.
+template <typename S>
+struct SceneFrozen : S { uint32_t frozen; };
+template <bool RAW, bool DYN, bool FROZEN = false>
+using BwdScene = std::conditional_t<
+    RAW, std::conditional_t<FROZEN, SceneFrozen<std::conditional_t<DYN, SceneBwdDyn, SceneBwd>>,
+                            std::conditional_t<DYN, SceneBwdDyn, SceneBwd>>,
+    NoScene>;
 
 struct ViewNoise {
     unsigned long long seed;
@@ -296,6 +303,13 @@ __device__ __forceinline__ ViewNoise view_noise(const S& sc, b200gsr_params& p) 
 #define GSR_SEED (DYN ? nz.seed : sc.seed)
 #define GSR_C_SHS (DYN ? nz.c_shs : sc.c_shs)
 #define GSR_C_SCALE (DYN ? nz.c_scale : sc.c_scale)
+
+// FROZEN: whether active row i belongs to a frozen group.  A constant false otherwise.
+template <bool FROZEN, typename S>
+__device__ __forceinline__ bool frozen_row(const S& sc, bool active, int i) {
+    if constexpr (FROZEN) return active && ((sc.frozen >> find_group(sc.tab, i)) & 1u);
+    else return false;
+}
 
 // A row's shape leaves and what the chain rule needs of them.
 struct RawLeaf {
@@ -612,8 +626,11 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
 // the raw leaves of `sc.tab` and the view's parameter gradients are chained straight to the leaf gradients of
 // `sc.gtab`; view 0 writes every row (zeros on culled rows), later views add into the rows they touched only.  It
 // carries more live state (the leaf values and noise of the row), hence 5 CTAs/SM.  DYN (with RAW): the view's
-// per-step values come from device memory (view_noise).
-template <int MT, bool RAW = false, bool DYN = false>
+// per-step values come from device memory (view_noise).  FROZEN (with RAW): rows of the groups set in sc.frozen are
+// treated as culled - no SH staging, geometry, dgeom access, leaf load or store, or noise draw - except that their
+// d_means2D rows are written (zeros); composite_bwd's FROZEN mode left their dgeom rows at zero.  Every other row runs
+// the default statements.
+template <int MT, bool RAW = false, bool DYN = false, bool FROZEN = false>
 __global__ void __launch_bounds__(kBlock, RAW ? 5 : 6)
 project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
                    const float* __restrict__ shs, const float* __restrict__ colors,
@@ -625,7 +642,7 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
                    float* __restrict__ d_shs, float* __restrict__ d_colors,
                    float* __restrict__ d_opac, float* __restrict__ d_scales,
                    float* __restrict__ d_rots, float* __restrict__ d_cov3d,
-                   const BwdScene<RAW, DYN> sc) {
+                   const BwdScene<RAW, DYN, FROZEN> sc) {
     extern __shared__ __align__(16) float sh_buf[];
     __shared__ uint8_t vis_s[kBlock];
     const ViewNoise nz = view_noise<DYN>(sc, p);
@@ -634,7 +651,8 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
     const int g0 = g_base + blockIdx.x * kBlock;
     const int i = g0 + threadIdx.x;
     const bool active = i < g_end;
-    const bool vis = active && (__ldg(radii + rec_base + i) > 0);
+    const bool fz = frozen_row<FROZEN>(sc, active, i);
+    const bool vis = active && !fz && (__ldg(radii + rec_base + i) > 0);
     const int nsh = 3 * dsh_coefs;          // floats per row of d_shs: 3*M (reference layout) or compact
     const int stride = sh_row_stride(p.M);
     const int deg = p.sh_degree;
@@ -657,7 +675,7 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
         if (active) {
             grp = find_group(sc.tab, i);
             loc = (size_t)(i - sc.tab.start[grp]);
-            if (vis || sc.d_scales != nullptr) raw_shape(sc.tab, grp, loc, i, GSR_SEED, GSR_C_SCALE, sc.view, lf, raw);
+            if (!fz && (vis || sc.d_scales != nullptr)) raw_shape(sc.tab, grp, loc, i, GSR_SEED, GSR_C_SCALE, sc.view, lf, raw);
         }
     }
     if (vis) {
@@ -884,7 +902,7 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
                 go = dop * sig * (1.0f - sig);
                 gq = quat_normalize_grad(lf.q, lf.nrm, make_float4(drot[0], drot[1], drot[2], drot[3]));
             }
-            if (vis || has_ds) {
+            if (!fz && (vis || has_ds)) {
 #pragma unroll
                 for (int k = 0; k < 3; ++k) {
                     float d = dsc[k] + (has_ds ? __ldg(sc.d_scales + 3 * (size_t)i + k) : 0.0f);
@@ -896,7 +914,7 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
             float* po = sc.gtab.opacity[grp] + loc;
             float* ps = sc.gtab.scaling[grp] + 3 * loc;
             float4* pq = reinterpret_cast<float4*>(sc.gtab.rotation[grp]) + loc;
-            const bool rows_touched = first || vis, scale_touched = first || vis || has_ds;
+            const bool rows_touched = !fz && (first || vis), scale_touched = !fz && (first || vis || has_ds);
             if (!first) {
                 if (rows_touched) {
                     const float4 oq = *pq;
@@ -935,9 +953,10 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
                 const int row = (it0 + u) * 8 + w * 2 + hsel;
                 const int gi = g0 + row;
                 const bool v = gi < g_end && vis_s[row];
-                const bool on = gi < g_end && (first || v);
+                bool on = gi < g_end && (first || v);
                 int gg = 0;
                 if (on) gg = find_group(sc.tab, gi);
+                if constexpr (FROZEN) on = on && !((sc.frozen >> gg) & 1u);
                 const size_t ll = on ? (size_t)(gi - sc.tab.start[gg]) : 0;
 #pragma unroll
                 for (int j = 0; j < 3; ++j) {
@@ -1148,12 +1167,13 @@ static SceneBwd scene_bwd(const GsrBwdArgs& a) {
     return sc;
 }
 
-template <int MT, bool RAW = false, bool DYN = false>
+template <int MT, bool RAW = false, bool DYN = false, bool FROZEN = false>
 static void launch_project_bwd(const GsrBwdArgs& a, int g_begin, int g_end, size_t smem) {
-    BwdScene<RAW, DYN> sc{};
+    BwdScene<RAW, DYN, FROZEN> sc{};
     if constexpr (RAW) static_cast<SceneBwd&>(sc) = scene_bwd(a);
     if constexpr (DYN) sc.dyn = SceneDyn{a.scene->dyn_views, a.scene->dyn_seed};
-    project_bwd_kernel<MT, RAW, DYN><<<(g_end - g_begin + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
+    if constexpr (FROZEN) sc.frozen = a.scene->frozen;
+    project_bwd_kernel<MT, RAW, DYN, FROZEN><<<(g_end - g_begin + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
         a.prm, a.means3D, a.shs, a.colors, a.scales, a.rots, a.cov3d, a.radii,
         reinterpret_cast<float*>(a.saved + a.vl.dgeom),
         reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE, g_begin, g_end,
@@ -1166,7 +1186,10 @@ cudaError_t gsr_launch_project_bwd(const GsrBwdArgs& a) {
     const int g_begin = a.g_begin, g_end = a.g_end;
     if (g_end <= g_begin) return cudaSuccess;
     const size_t smem = (a.shs || a.scene) ? (size_t)kBlock * sh_row_stride(a.prm.M) * sizeof(float) : 0;
-    if (a.scene && a.scene->dyn_views) launch_project_bwd<0, true, true>(a, g_begin, g_end, smem);
+    const bool frozen = a.scene && a.scene->frozen;
+    if (a.scene && a.scene->dyn_views && frozen) launch_project_bwd<0, true, true, true>(a, g_begin, g_end, smem);
+    else if (a.scene && frozen) launch_project_bwd<0, true, false, true>(a, g_begin, g_end, smem);
+    else if (a.scene && a.scene->dyn_views) launch_project_bwd<0, true, true>(a, g_begin, g_end, smem);
     else if (a.scene) launch_project_bwd<0, true>(a, g_begin, g_end, smem);
     else if (a.shs && a.prm.M == 16) launch_project_bwd<16>(a, g_begin, g_end, smem);
     else if (a.shs && a.prm.M == 4) launch_project_bwd<4>(a, g_begin, g_end, smem);

@@ -31,14 +31,21 @@ graphs, so that the eager loss is the guidance term alone:
     guidance_loss(out.image).backward()       # eager
     sg.step()       # adds weight * each regulariser's gradient to the outputs' gradients before the render backward
 
+Frozen groups (the scene stages that train one group, f11) are rendered but get no gradient:
+
+    sg = StepGraph(groups, [env_optimizer], views=B, height=H, width=W, frozen=[k != "env" for k in names])
+
+the backward graph computes and stores gradients for the trainable groups only (``grads[k]`` is None for a frozen
+group, whose optimizer must not be passed).
+
 ``step(optimize=False)`` replays the backward only (``grads`` and ``d_means2D``), leaving parameters, moments and
 step counters as they are: the reference's densify step, whose optimizer.step() follows densify_and_prune and so
 updates nothing.
 
 The first ``render()`` of a layout runs one eager forward and backward (which measure the pair capacity and set up
 the library) and then captures.  The layout - P, the group tensors, the optimizer state tensors, the per-view
-scale_modifier, deterministic mode, the target tensor and weight and the regulariser weights - is compared on the
-host at every ``render()``; a change (densify / prune) re-captures.
+scale_modifier, deterministic mode, the target tensor and weight, the regulariser weights and the frozen groups - is
+compared on the host at every ``render()``; a change (densify / prune, or assigning ``frozen``) re-captures.
 """
 from __future__ import annotations
 
@@ -80,11 +87,17 @@ class StepGraph:
     whose weight is None or 0 is off.  The render graph writes the unweighted values into `reg_loss`; the backward
     graph adds weight * each term's gradient to the gradient step() takes from the output's .grad, which is the
     eager step's gradient bit for bit when the eager loss, written before the regularisers, reaches each output
-    through one edge.  Not with target (the refine stages use no regulariser)."""
+    through one edge.  Not with target (the refine stages use no regulariser).
+
+    frozen: None, or one bool per group (render_scene's `frozen`).  A frozen group is rendered but its leaves get no
+    gradient buffer (grads[k] is None) and the backward does no work for it; an optimizer over one of its leaves is
+    refused.  The regularisers are unchanged: the scale term still covers every group's rows.  Assigning
+    `sg.frozen` re-captures at the next render()."""
 
     def __init__(self, groups: Sequence, optimizers: Sequence, *, views: int, height: int, width: int,
                  target: torch.Tensor | None = None, target_weight: float = 100.0, tv_weight: float | None = None,
-                 tv_depth_weight: float | None = None, scale_weight: float | None = None):
+                 tv_depth_weight: float | None = None, scale_weight: float | None = None,
+                 frozen: Sequence[bool] | None = None):
         self.groups = list(groups)
         self.optimizers = list(optimizers)
         self.B, self.H, self.W = int(views), int(height), int(width)
@@ -97,11 +110,14 @@ class StepGraph:
         self._target_key()
         self.tv_weight, self.tv_depth_weight, self.scale_weight = tv_weight, tv_depth_weight, scale_weight
         self._reg_key()
+        self.frozen = frozen
+        self._frozen_key()
         self._key = None
         self._report = None         # device [2]: max pair count, overflowed replays; kept across re-captures
         self._scratch_key = None
         self.d_means2D = None       # [B,P,3] per-view screen-space gradients of the last step (densification stats)
-        self.grads = None           # per group {leaf name: its gradient of the last step} (the backward graph's buffers)
+        self.grads = None           # per group {leaf name: its gradient of the last step} (the backward graph's buffers),
+                                    # None for a frozen group
         self.loss = None            # target mode: [B] each view's loss of the last render(), in the target's dtype
         self.reg_loss = None        # with a regulariser: [3] float32 tv(image), tv(disp), scale of the last render()
 
@@ -138,6 +154,21 @@ class StepGraph:
             if (out[0] is not None or out[1] is not None) and (self.H < 2 or self.W < 2):
                 raise ValueError("StepGraph: the total-variation regularisers need height and width >= 2")
         return tuple(out)
+
+    def _frozen_key(self) -> int:
+        """The frozen groups' bit mask (bit g = group g), part of the layout key."""
+        return S._frozen_mask(self.frozen, len(self.groups), "StepGraph")
+
+    def _check_frozen_leaves(self, flat, mask):
+        """Refuse an optimizer parameter that is a leaf of a frozen group: it would never get a gradient."""
+        frozen = {id(t): i // 6 for i, t in enumerate(flat) if (mask >> (i // 6)) & 1}
+        for opt in self.optimizers:
+            for group in opt.param_groups:
+                for p in group["params"]:
+                    if id(p) in frozen:
+                        raise ValueError(f"StepGraph: an optimizer parameter is a leaf of frozen group {frozen[id(p)]}; "
+                                         "it would never get a gradient. Leave that group's optimizer out or unfreeze "
+                                         "the group")
 
     def _target_indices(self, target_index):
         """-> the B validated target indices, or None without a target."""
@@ -181,7 +212,7 @@ class StepGraph:
                     st = opt.state.get(p, {})
                     states.append((id(p), st["exp_avg"].data_ptr() if st else 0, st["exp_avg_sq"].data_ptr() if st else 0))
         return (P, M, ptrs, tuple(states), tuple(float(s.scale_modifier) for s in settings), det, self._target_key(),
-                self._reg_key())
+                self._reg_key(), self._frozen_key())
 
     def _upload(self, settings, rec, seed, focal, tidx):
         """One pinned staging tensor, one non_blocking copy of it (plus one device concatenation when the cameras
@@ -265,12 +296,13 @@ class StepGraph:
         prm = (_lib.Params * B)(*[R._make_params(s._replace(viewmatrix=vm[v], projmatrix=pm[v], campos=cp[v]), P, M,
                                                  keep, dev, bg, v) for v, s in enumerate(settings)])
         table = S._group_table(raw)
-        grads = [[torch.zeros_like(t) for t in ts] for ts in raw]
+        fmask = self._frozen_key()
+        grads = [[None] * 6 if (fmask >> k) & 1 else [torch.zeros_like(t) for t in ts] for k, ts in enumerate(raw)]
         garr = (_lib.GroupGrad * ng)()
         for k, ts in enumerate(grads):
             for name, t in zip(("xyz", "opacity", "scaling", "rotation", "f_dc", "f_rest"), ts):
-                setattr(garr[k], name, t.data_ptr() if t.numel() else None)
-        self._grad_of = {id(t): g for t, g in zip(flat, [g for gs in grads for g in gs])}
+                setattr(garr[k], name, t.data_ptr() if t is not None and t.numel() else None)
+        self._grad_of = {id(t): g for t, g in zip(flat, [g for gs in grads for g in gs]) if g is not None}
         records = self._adam_records()
         self._scalars = torch.zeros(max(len(records), 1), 6, dtype=torch.float32, device=dev)
         tables = []
@@ -366,10 +398,11 @@ class StepGraph:
                                                          ptr(stats_bwd), ptr(d_da4), bwd_flags, _lib.stream(dev)),
                        "b200gsr_disparity_backward")
             g_da.view(2, B, Hp, W)[:, :, :H].copy_(d_da4.permute(1, 0, 2, 3))
-            _lib.check(lib.b200gsr_backward_scene_dyn(B, prm, ng, table, garr, views_p, seed_p, ptr(g_scales),
-                                                      ptr(radii), ptr(da), ptr(g_color), ptr(g_da), ptr(saved),
-                                                      saved.numel(), cap, ptr(d_means2D), bwd_flags, _lib.stream(dev)),
-                       "b200gsr_backward_scene_dyn")
+            _lib.check(lib.b200gsr_backward_scene_dyn_frozen(B, prm, ng, table, garr, views_p, seed_p, ptr(g_scales),
+                                                             ptr(radii), ptr(da), ptr(g_color), ptr(g_da), ptr(saved),
+                                                             saved.numel(), cap, ptr(d_means2D), bwd_flags, fmask,
+                                                             _lib.stream(dev)),
+                       "b200gsr_backward_scene_dyn_frozen")
 
         layout = (B * P, Hs, W, True, det)
         with torch.no_grad(), torch.cuda.device(dev):
@@ -427,7 +460,7 @@ class StepGraph:
         self._keep = (keep, prm, table, garr, tables, raw, saved, color, da, da4, stats, stats_bwd, g_color, g_da, d_da4)
         self._static_grads = (g_image, g_disp, g_alpha, g_scales)
         self._leaves = list(flat)
-        self.grads = [dict(zip(S._FIELDS, gs)) for gs in grads]
+        self.grads = [None if gs[0] is None else dict(zip(S._FIELDS, gs)) for gs in grads]
         self.out = StepOutputs(image, disp, alpha, radii, scales)
         self.d_means2D = d_means2D
         self._cap = cap
@@ -447,6 +480,7 @@ class StepGraph:
         rec = self._views(settings_list, shs_aug, scale_aug, M)
         tidx = self._target_indices(target_index)
         self._reg_key()
+        self._check_frozen_leaves(flat, self._frozen_key())
         if tidx is not None and (self.target.device.type != "cuda" or self.target.device != flat[0].device):
             raise ValueError("StepGraph: target must be a CUDA tensor on the groups' device")
         if seed is None:

@@ -201,9 +201,19 @@ def _check_settings(settings):
     return B, H, W
 
 
+def _frozen_mask(frozen, num_groups: int, who: str) -> int:
+    """None (nothing frozen) or one bool per group -> the bit mask of the frozen groups (bit g = group g)."""
+    if frozen is None:
+        return 0
+    flags = [bool(f) for f in frozen]
+    if len(flags) != num_groups:
+        raise ValueError(f"{who}: frozen must hold one bool per group ({num_groups}), got {len(flags)}")
+    return sum(1 << g for g, f in enumerate(flags) if f)
+
+
 class _RenderScene(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, settings, num_groups, M, c_shs, c_scale, seed, return_scales, *flat):
+    def forward(ctx, settings, num_groups, M, c_shs, c_scale, seed, return_scales, frozen, *flat):
         # flat = 6 raw leaves per group, then the B means2D ports
         from . import rasterizer as R
         B = len(settings)
@@ -238,7 +248,7 @@ class _RenderScene(torch.autograd.Function):
 
             saved, cap = R._issue_with_capacity(d, (B, P, H, W), B * P, Hs, W, with_backward, det, None, launch,
                                                 capturing, stream.value)
-        ctx.meta = (B, P, M, W, Hs, cap, with_backward, num_groups, seed, det)
+        ctx.meta = (B, P, M, W, Hs, cap, with_backward, num_groups, seed, det, frozen)
         ctx.views = (prm, table, noise)   # reused by the backward; `keep` holds the device constants of `prm`
         ctx.keep = keep
         ctx.saved_buf = saved
@@ -251,7 +261,7 @@ class _RenderScene(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_color, _g_radii, g_da, g_scales=None):
-        B, P, M, W, Hs, cap, with_backward, num_groups, seed, det = ctx.meta
+        B, P, M, W, Hs, cap, with_backward, num_groups, seed, det, frozen = ctx.meta
         prm, table, noise = ctx.views
         radii, depth_alpha = ctx.saved_tensors[:2]
         leaves = ctx.saved_tensors[2:]
@@ -259,7 +269,8 @@ class _RenderScene(torch.autograd.Function):
         dev = radii.device
         if not with_backward:
             raise RuntimeError("b200gsr: backward through a forward that ran without gradient accumulators")
-        grads = [[torch.empty_like(t) for t in ts] for ts in raw]       # every row is written by view 0
+        # every row of a trainable group is written by view 0; a frozen group gets no gradient
+        grads = [[None] * 6 if (frozen >> k) & 1 else [torch.empty_like(t) for t in ts] for k, ts in enumerate(raw)]
         d_means2D = torch.zeros(B, P, 3, dtype=torch.float32, device=dev)
         if P > 0:
             g_color = torch.zeros(3, Hs, W, device=dev) if g_color is None else _lib.prepare(g_color)
@@ -268,20 +279,23 @@ class _RenderScene(torch.autograd.Function):
             garr = (_lib.GroupGrad * num_groups)()
             for k, ts in enumerate(grads):
                 for name, t in zip(("xyz", "opacity", "scaling", "rotation", "f_dc", "f_rest"), ts):
-                    setattr(garr[k], name, t.data_ptr() if t.numel() else None)
+                    setattr(garr[k], name, t.data_ptr() if t is not None and t.numel() else None)
             lib, ptr = _lib.load(), _lib.ptr
+            args = (B, prm, num_groups, table, garr, noise[0], noise[1], seed, ptr(g_scales), ptr(radii),
+                    ptr(depth_alpha), ptr(g_color), ptr(g_da), ptr(ctx.saved_buf), ctx.saved_buf.numel(), cap,
+                    ptr(d_means2D), _lib.BWD_DETERMINISTIC if det else 0)
             with torch.cuda.device(dev):
-                rc = lib.b200gsr_backward_scene(B, prm, num_groups, table, garr, noise[0], noise[1], seed, ptr(g_scales),
-                                                ptr(radii), ptr(depth_alpha), ptr(g_color), ptr(g_da),
-                                                ptr(ctx.saved_buf), ctx.saved_buf.numel(), cap, ptr(d_means2D),
-                                                _lib.BWD_DETERMINISTIC if det else 0, _lib.stream(dev))
-            _lib.check(rc, "b200gsr_backward_scene")
-        return (None,) * 7 + tuple(t for ts in grads for t in ts) + tuple(d_means2D.unbind(0))
+                if frozen:
+                    rc = lib.b200gsr_backward_scene_frozen(*args, frozen, _lib.stream(dev))
+                else:
+                    rc = lib.b200gsr_backward_scene(*args, _lib.stream(dev))
+            _lib.check(rc, "b200gsr_backward_scene_frozen" if frozen else "b200gsr_backward_scene")
+        return (None,) * 8 + tuple(t for ts in grads for t in ts) + tuple(d_means2D.unbind(0))
 
 
 def render_scene(groups: Sequence, settings_list: Sequence, *, shs_aug=True, scale_aug=True, seed: int | None = None,
                  generator: torch.Generator | None = None, means2D: Sequence[torch.Tensor] | None = None,
-                 return_scales: bool = False):
+                 return_scales: bool = False, frozen: Sequence[bool] | None = None):
     """The B views of one training step rendered straight from the raw parameter groups: activations, augmentation
     and rasterization in one op (the reference's scene_render / object_render, scene_gaussian.py:673-893).
 
@@ -292,13 +306,21 @@ def render_scene(groups: Sequence, settings_list: Sequence, *, shs_aug=True, sca
     seed / generator : the in-kernel Philox noise of assemble_scene(noise="fused"): for equal seeds the rasterizer
                     sees bit for bit the inputs of assemble_scene(groups, noise="fused", seed=seed, views=B).
     means2D       : optional B [P,3] tensors whose .grad receives the per-view screen-space gradient.
+    frozen        : None, or one bool per group.  A frozen group is rendered as any other but trained by none of
+                    the step's optimizers (the reference's stages that train one group): its leaves get None as their
+                    gradient, its means2D rows get zeros, and the backward computes nothing for it.  The trainable
+                    groups' gradients are those of the call without `frozen` (bit for bit in deterministic mode).
+                    Explicit, not inferred from requires_grad: a group whose leaves need no gradient still feeds the
+                    means2D gradients unless it is frozen.
     -> list of B (color[3,H,W], radii[P], depth_alpha[2,H,W]); with return_scales also the augmented scales
-       [B,P,3] (differentiable, for the reference's scale loss).  Every group's raw leaves get their gradients."""
+       [B,P,3] (differentiable, for the reference's scale loss).  Every trainable group's raw leaves get their
+       gradients."""
     from . import parallel
     B, H, W = _check_settings(settings_list)
     shs_flags = _view_flags(shs_aug, B, "shs_aug")
     scale_flags = _view_flags(scale_aug, B, "scale_aug")
     flat, M, P = _scene_groups(groups)
+    frozen_mask = _frozen_mask(frozen, len(groups), "render_scene")
     if parallel.reduction_active():
         raise RuntimeError("render_scene does not reduce gradients over ranks inside its backward; call "
                            "dreamscene_b200.parallel.all_reduce_gradients on the leaves after backward instead")
@@ -314,7 +336,7 @@ def render_scene(groups: Sequence, settings_list: Sequence, *, shs_aug=True, sca
     res = _RenderScene.apply(tuple(settings_list), len(groups), M,
                              tuple(NOISE_COEF if f else 0.0 for f in shs_flags),
                              tuple(NOISE_COEF if f else 0.0 for f in scale_flags), int(seed), bool(return_scales),
-                             *flat, *means2D)
+                             frozen_mask, *flat, *means2D)
     color, radii, da = res[0], res[1], res[2]
     Hp = color.shape[1] // B
     outs = [(color[:, v * Hp:v * Hp + H, :], radii[v], da[:, v * Hp:v * Hp + H, :]) for v in range(B)]
