@@ -1,5 +1,5 @@
 """ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h,
-include/b200gsr_loss.h, include/b200gsr_frozen.h).  Fails loudly if the library is missing:
+include/b200gsr_loss.h, include/b200gsr_frozen.h, include/b200gsr_stats.h).  Fails loudly if the library is missing:
 there is NO CPU or PyTorch fallback in the product path."""
 from __future__ import annotations
 
@@ -150,6 +150,21 @@ FROZEN_SIGNATURES = {
                                           [vp] * 6 + [sz, u64, vp, u32, u32, vp]),
 }
 
+
+class GroupStats(C.Structure):      # == b200gsr_group_stats (include/b200gsr_stats.h)
+    _fields_ = [(n, C.c_void_p) for n in ("xyz_gradient_accum", "denom", "max_radii2D")]
+
+
+# The backwards with the densification statistics of include/b200gsr_stats.h (same library), in that header's order:
+# the arguments of b200gsr_backward_scene[_dyn]_frozen up to frozen_groups, then the per-group statistics and the view
+# (an int32 by value, a device pointer under _dyn) before the stream.
+STATS_SIGNATURES = {
+    "b200gsr_backward_scene_stats": (C.c_int, [i32, _P(Params), i32, _P(Group), _P(GroupGrad), vp, vp, u64] +
+                                     [vp] * 6 + [sz, u64, vp, u32, u32, _P(GroupStats), i32, vp]),
+    "b200gsr_backward_scene_dyn_stats": (C.c_int, [i32, _P(Params), i32, _P(Group), _P(GroupGrad), vp, vp] +
+                                         [vp] * 6 + [sz, u64, vp, u32, u32, _P(GroupStats), vp, vp]),
+}
+
 _lib = None
 ABI_VERSION = 3
 ERR_BAD_ARG = -1
@@ -179,7 +194,7 @@ def load():
                 "`python -m dreamscene_b200._build` (needs nvcc; sm_90a only). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES, **STEP_SIGNATURES, **LOSS_SIGNATURES,
-                                      **FROZEN_SIGNATURES}.items():
+                                      **FROZEN_SIGNATURES, **STATS_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:

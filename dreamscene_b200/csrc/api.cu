@@ -4,6 +4,7 @@
 #include "../../include/b200gsr_step.h"
 #include "../../include/b200gsr_loss.h"
 #include "../../include/b200gsr_frozen.h"
+#include "../../include/b200gsr_stats.h"
 
 #include <cstdarg>
 #include <cstdio>
@@ -937,17 +938,47 @@ int b200gsr_forward_scene_dyn(int32_t B, const b200gsr_params* prm, int32_t num_
                          scratch_bytes, saved, saved_bytes, max_pairs, flags, host_notify, notify_seq, stream);
 }
 
-// b200gsr_backward_scene, b200gsr_backward_scene_dyn (frozen = 0) and their _frozen variants (include/b200gsr_frozen.h)
+// The statistics arguments of b200gsr_backward_scene[_dyn]_stats (include/b200gsr_stats.h), after check_scene and the
+// frozen mask's check.  -> whether any group gathers.
+static int check_stats(int32_t B, int32_t num_groups, uint32_t frozen, const b200gsr_group_stats* stats, bool dyn,
+                       int32_t stats_view, const int32_t* dyn_stats_view, bool& any) {
+    any = false;
+    if (!dyn && (stats_view < -1 || stats_view >= B))
+        return fail(B200GSR_ERR_BAD_ARG, "stats_view %d not in -1..%d", stats_view, B - 1);
+    for (int g = 0; g < num_groups && stats; ++g) {
+        const b200gsr_group_stats& st = stats[g];
+        if ((st.xyz_gradient_accum == nullptr) != (st.denom == nullptr))
+            return fail(B200GSR_ERR_BAD_ARG, "group %d: xyz_gradient_accum and denom must both be set or both be null", g);
+        if (st.xyz_gradient_accum == nullptr && st.max_radii2D != nullptr)
+            return fail(B200GSR_ERR_BAD_ARG, "group %d: max_radii2D without xyz_gradient_accum and denom", g);
+        if (st.xyz_gradient_accum == nullptr) continue;
+        if ((frozen >> g) & 1u)
+            return fail(B200GSR_ERR_BAD_ARG, "group %d: statistics on a frozen group (its rows would count in denom with "
+                        "a zero gradient)", g);
+        any = true;
+    }
+    if (any && dyn && !dyn_stats_view)
+        return fail(B200GSR_ERR_BAD_ARG, "stats_view must be a device pointer to an int32 when a group gathers statistics");
+    return B200GSR_OK;
+}
+
+// b200gsr_backward_scene, b200gsr_backward_scene_dyn (frozen = 0), their _frozen variants (include/b200gsr_frozen.h)
+// and their _stats variants (include/b200gsr_stats.h, `with_stats`: d_means2D may be null)
 static int backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
                           const b200gsr_group_grad* grads, GsrScene sc, bool dyn, const float* d_scales,
                           const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
                           const float* dL_ddepth_alpha, void* saved, size_t saved_bytes, uint64_t max_pairs,
-                          float* d_means2D, uint32_t flags, uint32_t frozen, void* stream) {
+                          float* d_means2D, uint32_t flags, uint32_t frozen, void* stream, bool with_stats = false,
+                          const b200gsr_group_stats* stats = nullptr, int32_t stats_view = -1,
+                          const int32_t* dyn_stats_view = nullptr) {
     int rc = check_scene(B, prm, num_groups, groups, sc, dyn);
     if (rc) return rc;
     if (flags & ~B200GSR_BWD_DETERMINISTIC) return fail(B200GSR_ERR_BAD_ARG, "unknown flags 0x%x", flags);
     if (frozen >> num_groups)      // num_groups <= B200GSR_MAX_GROUPS < 32 (check_scene)
         return fail(B200GSR_ERR_BAD_ARG, "frozen mask 0x%x has bits at or above num_groups %d", frozen, num_groups);
+    bool gathers = false;
+    if (with_stats && (rc = check_stats(B, num_groups, frozen, stats, dyn, stats_view, dyn_stats_view, gathers)))
+        return rc;
     if (num_groups > 0 && !grads) return fail(B200GSR_ERR_BAD_ARG, "grads is null");
     for (int g = 0; g < num_groups; ++g)
         if (groups[g].n > 0 && !((frozen >> g) & 1u) && (!grads[g].xyz || !grads[g].opacity || !grads[g].scaling || !grads[g].rotation ||
@@ -955,13 +986,20 @@ static int backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_grou
             return fail(B200GSR_ERR_BAD_ARG, "group %d: null gradient pointer", g);
     const int P = prm[0].P;
     if (P == 0) return B200GSR_OK;
-    if (!radii || !out_depth_alpha || !dL_dcolor || !dL_ddepth_alpha || !saved || !d_means2D)
+    if (!radii || !out_depth_alpha || !dL_dcolor || !dL_ddepth_alpha || !saved || (!d_means2D && !with_stats))
         return fail(B200GSR_ERR_BAD_ARG, "null saved-state/gradient pointer");
     GsrBwdArgs a;
     if ((rc = setup_backward(true, B, prm, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes,
                              max_pairs, (flags & B200GSR_BWD_DETERMINISTIC) != 0, stream, a)))
         return rc;
     sc.num_groups = num_groups; sc.groups = groups; sc.grads = grads; sc.d_scales = d_scales; sc.frozen = frozen;
+    if (gathers) {
+        sc.stats = stats;
+        sc.stats_view = stats_view;
+        sc.dyn_stats_view = dyn_stats_view;
+    } else {
+        sc.stats_view = -1;
+    }
     a.scene = &sc;
     a.g_begin = 0; a.g_end = P;
     prof_mark_bwd(0, a.stream);
@@ -973,7 +1011,10 @@ static int backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_grou
     GSR_RANGE_PUSH("b200gsr.scene.project_bwd");
     for (int v = 0; v < B && !rc; ++v) {      // in view order: view 0 writes the leaf gradients, later views add
         a.prm = prm[v]; a.view = v;
-        a.d_means2D = d_means2D + 3 * (size_t)P * v;
+        a.d_means2D = d_means2D ? d_means2D + 3 * (size_t)P * v : nullptr;
+        // the STATS kernel where it has work: every view under _dyn (the view to gather is read on the device) or
+        // without d_means2D; by value, only the launch of the view that gathers.  The other launches are _frozen's.
+        sc.stats_mode = with_stats && (dyn || !d_means2D || (gathers && v == stats_view));
         rc = check_cuda(gsr_launch_project_bwd(a), "project_bwd");
     }
     GSR_RANGE_POP();
@@ -1028,6 +1069,34 @@ int b200gsr_backward_scene_dyn_frozen(int32_t B, const b200gsr_params* prm, int3
     sc.dyn_views = views; sc.dyn_seed = reinterpret_cast<const unsigned long long*>(seed);
     return backward_scene(B, prm, num_groups, groups, grads, sc, true, d_scales, radii, out_depth_alpha, dL_dcolor,
                           dL_ddepth_alpha, saved, saved_bytes, max_pairs, d_means2D, flags, frozen_groups, stream);
+}
+
+int b200gsr_backward_scene_stats(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
+                                 const b200gsr_group_grad* grads, const float* shs_noise, const float* scale_noise,
+                                 uint64_t seed, const float* d_scales, const int32_t* radii,
+                                 const float* out_depth_alpha, const float* dL_dcolor, const float* dL_ddepth_alpha,
+                                 void* saved, size_t saved_bytes, uint64_t max_pairs, float* d_means2D,
+                                 uint32_t flags, uint32_t frozen_groups, const b200gsr_group_stats* stats,
+                                 int32_t stats_view, void* stream) {
+    GsrScene sc{};
+    sc.shs_noise = shs_noise; sc.scale_noise = scale_noise; sc.seed = seed;
+    return backward_scene(B, prm, num_groups, groups, grads, sc, false, d_scales, radii, out_depth_alpha, dL_dcolor,
+                          dL_ddepth_alpha, saved, saved_bytes, max_pairs, d_means2D, flags, frozen_groups, stream,
+                          true, stats, stats_view, nullptr);
+}
+
+int b200gsr_backward_scene_dyn_stats(int32_t B, const b200gsr_params* prm, int32_t num_groups,
+                                     const b200gsr_group* groups, const b200gsr_group_grad* grads,
+                                     const b200gsr_step_view* views, const uint64_t* seed, const float* d_scales,
+                                     const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
+                                     const float* dL_ddepth_alpha, void* saved, size_t saved_bytes,
+                                     uint64_t max_pairs, float* d_means2D, uint32_t flags, uint32_t frozen_groups,
+                                     const b200gsr_group_stats* stats, const int32_t* stats_view, void* stream) {
+    GsrScene sc{};
+    sc.dyn_views = views; sc.dyn_seed = reinterpret_cast<const unsigned long long*>(seed);
+    return backward_scene(B, prm, num_groups, groups, grads, sc, true, d_scales, radii, out_depth_alpha, dL_dcolor,
+                          dL_ddepth_alpha, saved, saved_bytes, max_pairs, d_means2D, flags, frozen_groups, stream,
+                          true, stats, -1, stats_view);
 }
 
 int b200gsr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix,

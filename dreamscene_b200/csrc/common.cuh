@@ -4,7 +4,7 @@
 #include <stdint.h>
 #include <atomic>
 
-#include "../../include/b200gsr_step.h"
+#include "../../include/b200gsr_stats.h"
 
 #define GSR_TILE 16
 #define GSR_NEAR_Z 0.2f
@@ -196,6 +196,18 @@ __device__ __forceinline__ float rcp_approx(float x) {
 }
 #endif
 
+// ---- densification statistics ------------------------------------------------------------
+// |(gx, gy)|, the reference's torch.norm(grad[:, :2], dim=-1), as sqrt(fma(gx, gx, gy * gy)) with every step rounded
+// to nearest: the contraction nvcc chose for sqrtf(gx * gx + gy * gy), now fixed.  densify_stats_kernel and
+// project_bwd's STATS mode both call it, so the statistics gathered inside the backward equal those of
+// b200gsr_densify_stats over the stored d_means2D rows bit for bit.  The product and the FMA are written in PTX
+// because __fmul_rn / __fmaf_rn reorder densify_stats_kernel's two loads (same arithmetic, different SASS).
+__device__ __forceinline__ float gsr_screen_grad_norm(float gx, float gy) {
+    float s;
+    asm("{\n\t.reg .f32 yy;\n\tmul.rn.f32 yy, %2, %2;\n\tfma.rn.f32 %0, %1, %1, yy;\n\t}" : "=f"(s) : "f"(gx), "f"(gy));
+    return __fsqrt_rn(s);
+}
+
 // ---- shared-memory address helper (cp.async destinations) ----------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return (uint32_t)__cvta_generic_to_shared(p);
@@ -220,7 +232,13 @@ struct GsrScene {
     const unsigned long long* dyn_seed;
     // backward (b200gsr_backward_scene[_dyn]_frozen): bit g = group g is frozen; its leaves get no gradient and
     // composite_bwd / project_bwd run their FROZEN instantiations.  0 = the default kernels.
-    uint32_t frozen;
+    uint32_t frozen;    // backward (b200gsr_backward_scene[_dyn]_stats): project_bwd runs its STATS instantiation, which takes a null
+    // d_means2D and gathers the densification statistics of `stats` (host array [num_groups], or null) in the launch
+    // of the view stats_view (by value) or *dyn_stats_view (the _dyn entry point).  false = the other kernels.
+    bool stats_mode;
+    const b200gsr_group_stats* stats;
+    int32_t stats_view;
+    const int32_t* dyn_stats_view;
 };
 
 struct GsrFwdArgs {

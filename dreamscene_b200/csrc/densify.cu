@@ -27,7 +27,7 @@ __global__ void densify_stats_kernel(int P, const float* __restrict__ vs_grad, c
     const int r = radii[i];
     if (r <= 0) return;                                   // visibility_filter = radii > 0
     const float gx = vs_grad[3 * (size_t)i], gy = vs_grad[3 * (size_t)i + 1];
-    accum[i] += sqrtf(gx * gx + gy * gy);                 // torch.norm(grad[:, :2], dim=-1)
+    accum[i] += gsr_screen_grad_norm(gx, gy);             // torch.norm(grad[:, :2], dim=-1)
     denom[i] += 1.0f;
     if (max_radii != nullptr) max_radii[i] = fmaxf(max_radii[i], (float)r);
 }

@@ -38,14 +38,22 @@ Frozen groups (the scene stages that train one group, f11) are rendered but get 
 the backward graph computes and stores gradients for the trainable groups only (``grads[k]`` is None for a frozen
 group, whose optimizer must not be passed).
 
+Densification statistics (f12): the reference's add_densification_stats of the step's last view, gathered inside the
+backward graph instead of by an eager kernel over ``d_means2D`` afterwards:
+
+    sg = StepGraph(groups, optimizers, views=B, height=H, width=W,
+                   densify_stats=[(g.xyz_gradient_accum, g.denom, g.max_radii2D) for g in models], keep_means2D=False)
+    sg.step(stats_view=-1 if step < densify_until_iter else None)     # -1 = view B-1, None = off; no re-capture
+
 ``step(optimize=False)`` replays the backward only (``grads`` and ``d_means2D``), leaving parameters, moments and
 step counters as they are: the reference's densify step, whose optimizer.step() follows densify_and_prune and so
 updates nothing.
 
 The first ``render()`` of a layout runs one eager forward and backward (which measure the pair capacity and set up
 the library) and then captures.  The layout - P, the group tensors, the optimizer state tensors, the per-view
-scale_modifier, deterministic mode, the target tensor and weight, the regulariser weights and the frozen groups - is
-compared on the host at every ``render()``; a change (densify / prune, or assigning ``frozen``) re-captures.
+scale_modifier, deterministic mode, the target tensor and weight, the regulariser weights, the frozen groups and the
+densification statistics tensors - is compared on the host at every ``render()``; a change (densify / prune, or
+assigning ``frozen`` / ``densify_stats``) re-captures.
 """
 from __future__ import annotations
 
@@ -92,12 +100,21 @@ class StepGraph:
     frozen: None, or one bool per group (render_scene's `frozen`).  A frozen group is rendered but its leaves get no
     gradient buffer (grads[k] is None) and the backward does no work for it; an optimizer over one of its leaves is
     refused.  The regularisers are unchanged: the scale term still covers every group's rows.  Assigning
-    `sg.frozen` re-captures at the next render()."""
+    `sg.frozen` re-captures at the next render().
+
+    densify_stats: None, or one entry per group (render_scene's `densify_stats`): None, or the group's
+    (xyz_gradient_accum, denom, max_radii2D or None), updated in place by the backward graph for the view that step()
+    selects.  Their pointers are part of the layout: densify / prune replaces them together with the leaves, and
+    assigning the new ones to `sg.densify_stats` re-captures at the next render().  A frozen group's entry is refused.
+
+    keep_means2D: False leaves `d_means2D` None: the backward stores no [B,P,3] screen-space gradient (the statistics
+    need none).  True (default) keeps it."""
 
     def __init__(self, groups: Sequence, optimizers: Sequence, *, views: int, height: int, width: int,
                  target: torch.Tensor | None = None, target_weight: float = 100.0, tv_weight: float | None = None,
                  tv_depth_weight: float | None = None, scale_weight: float | None = None,
-                 frozen: Sequence[bool] | None = None):
+                 frozen: Sequence[bool] | None = None, densify_stats: Sequence | None = None,
+                 keep_means2D: bool = True):
         self.groups = list(groups)
         self.optimizers = list(optimizers)
         self.B, self.H, self.W = int(views), int(height), int(width)
@@ -112,10 +129,14 @@ class StepGraph:
         self._reg_key()
         self.frozen = frozen
         self._frozen_key()
+        self.densify_stats = densify_stats
+        self.keep_means2D = bool(keep_means2D)
+        self._stats_key()
         self._key = None
         self._report = None         # device [2]: max pair count, overflowed replays; kept across re-captures
         self._scratch_key = None
-        self.d_means2D = None       # [B,P,3] per-view screen-space gradients of the last step (densification stats)
+        self._stats_view = None     # with densify_stats: (device int32 [1] read by the backward graph, its value)
+        self.d_means2D = None       # [B,P,3] per-view screen-space gradients of the last step (None: keep_means2D=False)
         self.grads = None           # per group {leaf name: its gradient of the last step} (the backward graph's buffers),
                                     # None for a frozen group
         self.loss = None            # target mode: [B] each view's loss of the last render(), in the target's dtype
@@ -158,6 +179,17 @@ class StepGraph:
     def _frozen_key(self) -> int:
         """The frozen groups' bit mask (bit g = group g), part of the layout key."""
         return S._frozen_mask(self.frozen, len(self.groups), "StepGraph")
+
+    def _stats(self):
+        """The validated densify_stats entries (scene._densify_stats), None when no group gathers."""
+        return S._densify_stats(self.densify_stats, self.groups, self._frozen_key(), "StepGraph")
+
+    def _stats_key(self):
+        """The statistics tensors' pointers and keep_means2D, part of the layout key."""
+        st = self._stats()
+        ptrs = None if st is None else tuple(None if e is None else tuple(0 if t is None else t.data_ptr() for t in e)
+                                             for e in st)
+        return ptrs, bool(self.keep_means2D)
 
     def _check_frozen_leaves(self, flat, mask):
         """Refuse an optimizer parameter that is a leaf of a frozen group: it would never get a gradient."""
@@ -212,7 +244,7 @@ class StepGraph:
                     st = opt.state.get(p, {})
                     states.append((id(p), st["exp_avg"].data_ptr() if st else 0, st["exp_avg_sq"].data_ptr() if st else 0))
         return (P, M, ptrs, tuple(states), tuple(float(s.scale_modifier) for s in settings), det, self._target_key(),
-                self._reg_key(), self._frozen_key())
+                self._reg_key(), self._frozen_key(), self._stats_key())
 
     def _upload(self, settings, rec, seed, focal, tidx):
         """One pinned staging tensor, one non_blocking copy of it (plus one device concatenation when the cameras
@@ -325,7 +357,13 @@ class StepGraph:
         g_scales = torch.zeros_like(scales)
         g_color, g_da = torch.zeros(3, Hs, W, device=dev), torch.zeros(2, Hs, W, device=dev)
         d_da4 = torch.zeros_like(da4)
-        d_means2D = torch.zeros(B, P, 3, device=dev)
+        d_means2D = torch.zeros(B, P, 3, device=dev) if self.keep_means2D else None
+        dstats = self._stats()
+        # the backward with the statistics entry point when it gathers or stores no d_means2D; its view is read from
+        # stats_view_t at every replay (step() writes it; -1 = off, as for the eager run below)
+        with_stats = dstats is not None or d_means2D is None
+        stats_view_t = torch.full((1,), -1, dtype=torch.int32, device=dev)
+        stats_arr = S._stats_table(dstats)
         if self._report is None or self._report.device != dev:
             self._report = torch.zeros(2, dtype=torch.int32, device=dev)
         report = self._report           # one per StepGraph: a re-capture keeps the counts check() has not read yet
@@ -398,6 +436,13 @@ class StepGraph:
                                                          ptr(stats_bwd), ptr(d_da4), bwd_flags, _lib.stream(dev)),
                        "b200gsr_disparity_backward")
             g_da.view(2, B, Hp, W)[:, :, :H].copy_(d_da4.permute(1, 0, 2, 3))
+            if with_stats:
+                _lib.check(lib.b200gsr_backward_scene_dyn_stats(B, prm, ng, table, garr, views_p, seed_p, ptr(g_scales),
+                                                                ptr(radii), ptr(da), ptr(g_color), ptr(g_da), ptr(saved),
+                                                                saved.numel(), cap, ptr(d_means2D), bwd_flags, fmask,
+                                                                stats_arr, ptr(stats_view_t), _lib.stream(dev)),
+                           "b200gsr_backward_scene_dyn_stats")
+                return
             _lib.check(lib.b200gsr_backward_scene_dyn_frozen(B, prm, ng, table, garr, views_p, seed_p, ptr(g_scales),
                                                              ptr(radii), ptr(da), ptr(g_color), ptr(g_da), ptr(saved),
                                                              saved.numel(), cap, ptr(d_means2D), bwd_flags, fmask,
@@ -457,7 +502,9 @@ class StepGraph:
         self.loss = loss
         self.reg_loss = reg_loss
         self._accumulated = [reg[0] is not None, reg[1] is not None, False, reg[2] is not None]
-        self._keep = (keep, prm, table, garr, tables, raw, saved, color, da, da4, stats, stats_bwd, g_color, g_da, d_da4)
+        self._keep = (keep, prm, table, garr, tables, raw, saved, color, da, da4, stats, stats_bwd, g_color, g_da, d_da4,
+                      stats_arr, stats_view_t)
+        self._stats_view = (stats_view_t, -1) if dstats is not None else None    # device slot, value last written
         self._static_grads = (g_image, g_disp, g_alpha, g_scales)
         self._leaves = list(flat)
         self.grads = [None if gs[0] is None else dict(zip(S._FIELDS, gs)) for gs in grads]
@@ -481,6 +528,7 @@ class StepGraph:
         tidx = self._target_indices(target_index)
         self._reg_key()
         self._check_frozen_leaves(flat, self._frozen_key())
+        self._stats_key()
         if tidx is not None and (self.target.device.type != "cuda" or self.target.device != flat[0].device):
             raise ValueError("StepGraph: target must be a CUDA tensor on the groups' device")
         if seed is None:
@@ -500,13 +548,18 @@ class StepGraph:
             t.grad = None
         return self.out
 
-    def step(self, optimize: bool = True) -> None:
+    def step(self, optimize: bool = True, stats_view: int | None = -1) -> None:
         """Replay the backward graph: the render backward with the .grad of image / disp / alpha / scales (a missing
         grad counts as zeros; in target mode the loss's image gradient from the render graph instead) plus each
         regulariser's weighted gradient, the disparity backward; then, with `optimize`, the Adam graph: every
         optimizer's step.  The leaf gradients come from out.* only: a leaf that holds a .grad of its own (a loss term
         that reaches it directly, or a gradient not cleared since an eager step) is refused rather than dropped.
         Afterwards `grads` holds the leaf gradients and d_means2D the per-view screen-space gradients.
+
+        stats_view (with densify_stats): the view whose densification statistics this backward adds, -1 = the last
+        view (B - 1), or None = none (past the reference's densify_until_iter).  Written to device memory with the
+        step's other values: no re-capture.  The statistics are gathered by the backward graph, so optimize=False steps
+        gather them too, as the reference's add_densification_stats precedes its densify and optimizer.step().
 
         optimize=False leaves parameters, moments and step counters untouched, as the reference's optimizer.step()
         after densify_and_prune (whose new leaves have no gradient) does.  A step where only some leaves skip Adam
@@ -533,6 +586,15 @@ class StepGraph:
                 elif not (write_scales and t is self.out.scales):
                     g.fill_(-0.0)       # -0 + r == r bitwise, the sign of zero included: the regulariser's gradient
                 t.grad = None
+        if stats_view is not None and not -1 <= int(stats_view) < self.B:
+            raise ValueError(f"StepGraph.step(): stats_view must be -1 (the last view), None or in 0..{self.B - 1}, "
+                             f"got {stats_view}")
+        if self._stats_view is not None:
+            sv = -1 if stats_view is None else (self.B - 1 if int(stats_view) == -1 else int(stats_view))
+            slot, last = self._stats_view
+            if sv != last:
+                slot.copy_(torch.tensor([sv], dtype=torch.int32).pin_memory(), non_blocking=True)
+                self._stats_view = (slot, sv)
         if optimize:
             records = self._adam_records()      # this step's lr / betas / eps; same tensors as at capture (the layout)
             if records:

@@ -211,10 +211,55 @@ def _frozen_mask(frozen, num_groups: int, who: str) -> int:
     return sum(1 << g for g, f in enumerate(flags) if f)
 
 
+def _densify_stats(densify_stats, groups: Sequence, frozen_mask: int, who: str):
+    """None, or one entry per group - None or (xyz_gradient_accum, denom, max_radii2D or None) - -> a tuple of the
+    validated entries (the tensors themselves: they are updated in place), or None when no group gathers."""
+    if densify_stats is None:
+        return None
+    entries = list(densify_stats)
+    if len(entries) != len(groups):
+        raise ValueError(f"{who}: densify_stats must hold one entry per group ({len(groups)}), got {len(entries)}")
+    out = []
+    for g, (grp, e) in enumerate(zip(groups, entries)):
+        if e is None:
+            out.append(None)
+            continue
+        if len(e) != 3 or e[0] is None or e[1] is None:
+            raise ValueError(f"{who}: densify_stats[{g}] must be (xyz_gradient_accum, denom, max_radii2D or None)")
+        if (frozen_mask >> g) & 1:
+            raise ValueError(f"{who}: densify_stats[{g}] gathers statistics for frozen group {g}; the reference gathers "
+                             "them for the trained groups only")
+        xyz = _get(grp, "_xyz")
+        n = int(xyz.shape[0])
+        for name, t in zip(("xyz_gradient_accum", "denom", "max_radii2D"), e):
+            if t is None:
+                continue
+            if not torch.is_tensor(t) or t.dtype != torch.float32 or not t.is_contiguous():
+                raise ValueError(f"{who}: densify_stats[{g}] {name} must be a contiguous float32 tensor")
+            if t.numel() != n:
+                raise ValueError(f"{who}: densify_stats[{g}] {name} has {t.numel()} elements, group {g} has {n} rows")
+            if t.device != xyz.device:
+                raise ValueError(f"{who}: densify_stats[{g}] {name} must be on the groups' device ({xyz.device})")
+        out.append((e[0], e[1], e[2]))
+    return tuple(out) if any(e is not None for e in out) else None
+
+
+def _stats_table(stats):
+    """The b200gsr_group_stats records of _densify_stats' entries (NULL for None: no group gathers)."""
+    if stats is None:
+        return None
+    arr = (_lib.GroupStats * len(stats))()
+    for g, e in enumerate(stats):
+        if e is not None:
+            arr[g] = _lib.GroupStats(*[None if t is None else t.data_ptr() for t in e])
+    return arr
+
+
 class _RenderScene(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, settings, num_groups, M, c_shs, c_scale, seed, return_scales, frozen, *flat):
-        # flat = 6 raw leaves per group, then the B means2D ports
+    def forward(ctx, settings, num_groups, M, c_shs, c_scale, seed, return_scales, frozen, stats, *flat):
+        # flat = 6 raw leaves per group, then the B means2D ports (none when `stats` = (entries, view) is given
+        # without them: then no screen-space gradient is stored at all)
         from . import rasterizer as R
         B = len(settings)
         raw = [[_lib.prepare(t.detach()) for t in flat[6 * k:6 * k + 6]] for k in range(num_groups)]
@@ -249,6 +294,8 @@ class _RenderScene(torch.autograd.Function):
             saved, cap = R._issue_with_capacity(d, (B, P, H, W), B * P, Hs, W, with_backward, det, None, launch,
                                                 capturing, stream.value)
         ctx.meta = (B, P, M, W, Hs, cap, with_backward, num_groups, seed, det, frozen)
+        ctx.stats = stats
+        ctx.ports = len(flat) - 6 * num_groups
         ctx.views = (prm, table, noise)   # reused by the backward; `keep` holds the device constants of `prm`
         ctx.keep = keep
         ctx.saved_buf = saved
@@ -262,6 +309,7 @@ class _RenderScene(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_color, _g_radii, g_da, g_scales=None):
         B, P, M, W, Hs, cap, with_backward, num_groups, seed, det, frozen = ctx.meta
+        stats = ctx.stats
         prm, table, noise = ctx.views
         radii, depth_alpha = ctx.saved_tensors[:2]
         leaves = ctx.saved_tensors[2:]
@@ -271,7 +319,7 @@ class _RenderScene(torch.autograd.Function):
             raise RuntimeError("b200gsr: backward through a forward that ran without gradient accumulators")
         # every row of a trainable group is written by view 0; a frozen group gets no gradient
         grads = [[None] * 6 if (frozen >> k) & 1 else [torch.empty_like(t) for t in ts] for k, ts in enumerate(raw)]
-        d_means2D = torch.zeros(B, P, 3, dtype=torch.float32, device=dev)
+        d_means2D = torch.zeros(B, P, 3, dtype=torch.float32, device=dev) if ctx.ports else None
         if P > 0:
             g_color = torch.zeros(3, Hs, W, device=dev) if g_color is None else _lib.prepare(g_color)
             g_da = torch.zeros(2, Hs, W, device=dev) if g_da is None else _lib.prepare(g_da)
@@ -285,17 +333,24 @@ class _RenderScene(torch.autograd.Function):
                     ptr(depth_alpha), ptr(g_color), ptr(g_da), ptr(ctx.saved_buf), ctx.saved_buf.numel(), cap,
                     ptr(d_means2D), _lib.BWD_DETERMINISTIC if det else 0)
             with torch.cuda.device(dev):
-                if frozen:
+                if stats is not None:
+                    name = "b200gsr_backward_scene_stats"
+                    rc = lib.b200gsr_backward_scene_stats(*args, frozen, _stats_table(stats[0]), stats[1], _lib.stream(dev))
+                elif frozen:
+                    name = "b200gsr_backward_scene_frozen"
                     rc = lib.b200gsr_backward_scene_frozen(*args, frozen, _lib.stream(dev))
                 else:
+                    name = "b200gsr_backward_scene"
                     rc = lib.b200gsr_backward_scene(*args, _lib.stream(dev))
-            _lib.check(rc, "b200gsr_backward_scene_frozen" if frozen else "b200gsr_backward_scene")
-        return (None,) * 8 + tuple(t for ts in grads for t in ts) + tuple(d_means2D.unbind(0))
+            _lib.check(rc, name)
+        ports = tuple(d_means2D.unbind(0)) if ctx.ports else ()
+        return (None,) * 9 + tuple(t for ts in grads for t in ts) + ports
 
 
 def render_scene(groups: Sequence, settings_list: Sequence, *, shs_aug=True, scale_aug=True, seed: int | None = None,
                  generator: torch.Generator | None = None, means2D: Sequence[torch.Tensor] | None = None,
-                 return_scales: bool = False, frozen: Sequence[bool] | None = None):
+                 return_scales: bool = False, frozen: Sequence[bool] | None = None, densify_stats: Sequence | None = None,
+                 stats_view: int = -1):
     """The B views of one training step rendered straight from the raw parameter groups: activations, augmentation
     and rasterization in one op (the reference's scene_render / object_render, scene_gaussian.py:673-893).
 
@@ -312,6 +367,17 @@ def render_scene(groups: Sequence, settings_list: Sequence, *, shs_aug=True, sca
                     groups' gradients are those of the call without `frozen` (bit for bit in deterministic mode).
                     Explicit, not inferred from requires_grad: a group whose leaves need no gradient still feeds the
                     means2D gradients unless it is frozen.
+    densify_stats : None, or one entry per group: None, or the reference's (xyz_gradient_accum, denom, max_radii2D or
+                    None) of that group (float32, contiguous, one element per row).  The backward then also does the
+                    reference's add_densification_stats for view `stats_view`, in place and inside the render
+                    backward: for each row whose radius in that view is positive, accum += |screen-space gradient
+                    [:2]|, denom += 1, max_radii2D = max(max_radii2D, radius) - bit for bit what
+                    densify.add_densification_stats does with that view's means2D gradient and radii.  A frozen group
+                    gathers nothing (refused).  Each backward adds once: a second backward through the same forward
+                    (retain_graph) adds a second time, as calling the reference twice would.  Without `means2D` the
+                    backward then stores no screen-space gradient at all (no [B,P,3] buffer).
+    stats_view    : the view whose statistics are gathered: -1 (default) is the last view, B - 1 - the view whose
+                    gradient the reference's `out` holds after its view loop.
     -> list of B (color[3,H,W], radii[P], depth_alpha[2,H,W]); with return_scales also the augmented scales
        [B,P,3] (differentiable, for the reference's scale loss).  Every trainable group's raw leaves get their
        gradients."""
@@ -321,14 +387,21 @@ def render_scene(groups: Sequence, settings_list: Sequence, *, shs_aug=True, sca
     scale_flags = _view_flags(scale_aug, B, "scale_aug")
     flat, M, P = _scene_groups(groups)
     frozen_mask = _frozen_mask(frozen, len(groups), "render_scene")
+    stats = _densify_stats(densify_stats, groups, frozen_mask, "render_scene")
+    if densify_stats is not None:
+        sv = int(stats_view)
+        if not -1 <= sv < B:
+            raise ValueError(f"render_scene: stats_view must be -1 (the last view) or in 0..{B - 1}, got {stats_view}")
+        sv = B - 1 if sv == -1 else sv
     if parallel.reduction_active():
         raise RuntimeError("render_scene does not reduce gradients over ranks inside its backward; call "
                            "dreamscene_b200.parallel.all_reduce_gradients on the leaves after backward instead")
     _check_device(flat)
     dev = flat[0].device
     if means2D is None:
-        means2D = [torch.zeros(P, 3, device=dev) for _ in range(B)]
-    if len(means2D) != B:
+        # with densify_stats no port is needed: the backward then writes no screen-space gradient
+        means2D = [] if densify_stats is not None else [torch.zeros(P, 3, device=dev) for _ in range(B)]
+    if len(means2D) != B and not (densify_stats is not None and len(means2D) == 0):
         raise ValueError(f"means2D: expected {B} per-view tensors")
     if seed is None:
         cpu_gen = generator if generator is not None and generator.device.type == "cpu" else None
@@ -336,7 +409,7 @@ def render_scene(groups: Sequence, settings_list: Sequence, *, shs_aug=True, sca
     res = _RenderScene.apply(tuple(settings_list), len(groups), M,
                              tuple(NOISE_COEF if f else 0.0 for f in shs_flags),
                              tuple(NOISE_COEF if f else 0.0 for f in scale_flags), int(seed), bool(return_scales),
-                             frozen_mask, *flat, *means2D)
+                             frozen_mask, None if densify_stats is None else (stats, sv), *flat, *means2D)
     color, radii, da = res[0], res[1], res[2]
     Hp = color.shape[1] // B
     outs = [(color[:, v * Hp:v * Hp + H, :], radii[v], da[:, v * Hp:v * Hp + H, :]) for v in range(B)]
