@@ -14,7 +14,8 @@ SOURCES = ["api.cu", "project.cu", "binning.cu", "composite.cu", "knn.cu", "asse
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "scene_math.cuh"), os.path.join(CSRC, "project_bwd_body.cuh"),
            os.path.join(HERE, "..", "include", "b200gsr.h"), os.path.join(HERE, "..", "include", "b200gsr_scene.h"),
            os.path.join(HERE, "..", "include", "b200gsr_step.h"), os.path.join(HERE, "..", "include", "b200gsr_loss.h"),
-           os.path.join(HERE, "..", "include", "b200gsr_frozen.h"), os.path.join(HERE, "..", "include", "b200gsr_stats.h")]
+           os.path.join(HERE, "..", "include", "b200gsr_frozen.h"), os.path.join(HERE, "..", "include", "b200gsr_stats.h"),
+           os.path.join(HERE, "..", "include", "b200gsr_reserve.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

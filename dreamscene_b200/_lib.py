@@ -1,5 +1,6 @@
 """ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h,
-include/b200gsr_loss.h, include/b200gsr_frozen.h, include/b200gsr_stats.h).  Fails loudly if the library is missing:
+include/b200gsr_loss.h, include/b200gsr_frozen.h, include/b200gsr_stats.h,
+include/b200gsr_reserve.h).  Fails loudly if the library is missing:
 there is NO CPU or PyTorch fallback in the product path."""
 from __future__ import annotations
 
@@ -165,6 +166,23 @@ STATS_SIGNATURES = {
                                          [vp] * 6 + [sz, u64, vp, u32, u32, _P(GroupStats), vp, vp]),
 }
 
+
+class AdamLive(C.Structure):        # == b200gsr_adam_live (include/b200gsr_reserve.h)
+    _fields_ = [("rows", C.c_void_p), ("row_floats", C.c_int32), ("reserved", C.c_int32)]
+
+
+# The entry points over groups with reserved rows of include/b200gsr_reserve.h (same library), in that header's order:
+# the arguments of b200gsr_forward_scene_dyn / b200gsr_backward_scene_dyn_stats plus the device live counts before the
+# stream; the scale loss over the groups' table; the _dyn Adam step plus one live record per tensor.
+RESERVE_SIGNATURES = {
+    "b200gsr_forward_scene_dyn_live": (C.c_int, [i32, _P(Params), i32, _P(Group), vp, vp] + [vp] * 5 +
+                                       [sz, vp, sz, u64, u32, vp, u32, vp, vp]),
+    "b200gsr_backward_scene_dyn_live": (C.c_int, [i32, _P(Params), i32, _P(Group), _P(GroupGrad), vp, vp] +
+                                        [vp] * 6 + [sz, u64, vp, u32, u32, _P(GroupStats), vp, vp, vp]),
+    "b200gsr_scale_loss_live": (C.c_int, [i32, i32, _P(Group), vp, vp, vp, vp, vp, i32, vp, sz, vp]),
+    "b200gsr_adam_step_dyn_live": (C.c_int, [i32, _P(AdamTensor), vp, _P(AdamLive), vp]),
+}
+
 _lib = None
 ABI_VERSION = 3
 ERR_BAD_ARG = -1
@@ -194,7 +212,7 @@ def load():
                 "`python -m dreamscene_b200._build` (needs nvcc; sm_90a only). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES, **STEP_SIGNATURES, **LOSS_SIGNATURES,
-                                      **FROZEN_SIGNATURES, **STATS_SIGNATURES}.items():
+                                      **FROZEN_SIGNATURES, **STATS_SIGNATURES, **RESERVE_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:

@@ -5,6 +5,7 @@
 #include "../../include/b200gsr_loss.h"
 #include "../../include/b200gsr_frozen.h"
 #include "../../include/b200gsr_stats.h"
+#include "../../include/b200gsr_reserve.h"
 
 #include <cstdarg>
 #include <cstdio>
@@ -749,6 +750,19 @@ int b200gsr_adam_step_dyn(int32_t n_tensors, const b200gsr_adam_tensor* tensors,
     return check_cuda(gsr_launch_adam_dyn(n_tensors, tensors, scalars, GSR_ST(stream)), "adam_step_dyn");
 }
 
+int b200gsr_adam_step_dyn_live(int32_t n_tensors, const b200gsr_adam_tensor* tensors, const float* scalars,
+                               const b200gsr_adam_live* live, void* stream) {
+    int rc = check_adam(n_tensors, tensors);
+    if (rc) return rc;
+    if (n_tensors > 0 && !scalars) return fail(B200GSR_ERR_BAD_ARG, "adam_step_dyn_live: scalars must be a device array [n, 6]");
+    if (n_tensors > 0 && !live) return fail(B200GSR_ERR_BAD_ARG, "adam_step_dyn_live: live must be a host array of n records");
+    for (int i = 0; i < n_tensors; ++i)
+        if (live[i].rows && (live[i].row_floats < 1 || tensors[i].n % live[i].row_floats))
+            return fail(B200GSR_ERR_BAD_ARG, "adam_step_dyn_live: tensor %d: row_floats %d must be >= 1 and divide its "
+                        "length %lld", i, live[i].row_floats, (long long)tensors[i].n);
+    return check_cuda(gsr_launch_adam_dyn_live(n_tensors, tensors, scalars, live, GSR_ST(stream)), "adam_step_dyn_live");
+}
+
 int b200gsr_pair_report(const void* saved, uint32_t* report, void* stream) {
     if (!saved || !report) return fail(B200GSR_ERR_BAD_ARG, "pair_report: saved and report must be device pointers");
     return check_cuda(gsr_launch_pair_report(static_cast<const uint32_t*>(saved), report, GSR_ST(stream)), "pair_report");
@@ -835,6 +849,42 @@ int b200gsr_scale_loss(int32_t rows, const float* scales, const float* grad_out,
     return check_cuda(gsr_launch_scale_loss(a, GSR_ST(stream)), "scale_loss");
 }
 
+int b200gsr_scale_loss_live(int32_t B, int32_t num_groups, const b200gsr_group* groups, const int32_t* live,
+                            const float* scales, const float* grad_out, float* loss_out, float* d_scales,
+                            int32_t accumulate, void* scratch, size_t scratch_bytes, void* stream) {
+    if (B < 1 || B > B200GSR_MAX_VIEWS) return fail(B200GSR_ERR_BAD_ARG, "scale_loss_live: B %d not in 1..%d", B, B200GSR_MAX_VIEWS);
+    if (num_groups < 1 || num_groups > B200GSR_MAX_GROUPS || !groups)
+        return fail(B200GSR_ERR_BAD_ARG, "scale_loss_live: need a host array of 1..%d groups", B200GSR_MAX_GROUPS);
+    if (!live) return fail(B200GSR_ERR_BAD_ARG, "scale_loss_live: live must be a device array [num_groups]");
+    GsrScaleLiveArgs a;
+    long long P = 0;
+    for (int g = 0; g < num_groups; ++g) {
+        if (groups[g].n < 0) return fail(B200GSR_ERR_BAD_ARG, "scale_loss_live: group %d has a negative n", g);
+        a.start[g] = (int32_t)P;
+        P += groups[g].n;
+        if (P > INT32_MAX) return fail(B200GSR_ERR_UNSUPPORTED, "scale_loss_live: more than 2^31 - 1 rows");
+    }
+    if ((long long)B * P > INT32_MAX) return fail(B200GSR_ERR_UNSUPPORTED, "scale_loss_live: B * P too large");
+    const int32_t rows = (int32_t)(B * P);
+    if (rows < 1) return fail(B200GSR_ERR_BAD_ARG, "scale_loss_live: the groups hold no row");
+    if (3LL * rows > INT32_MAX) return fail(B200GSR_ERR_UNSUPPORTED, "scale_loss_live: at most 2^31 - 1 elements, got %lld", 3LL * rows);
+    if (accumulate != 0 && accumulate != 1) return fail(B200GSR_ERR_BAD_ARG, "scale_loss_live: accumulate must be 0 or 1");
+    if (!scales) return fail(B200GSR_ERR_BAD_ARG, "scale_loss_live: scales must be a device pointer");
+    if (!loss_out && !d_scales) return fail(B200GSR_ERR_BAD_ARG, "scale_loss_live: nothing to compute (loss_out and d_scales are null)");
+    if (d_scales && !grad_out) return fail(B200GSR_ERR_BAD_ARG, "scale_loss_live: d_scales needs grad_out");
+    if (loss_out && (!scratch || scratch_bytes < b200gsr_scale_loss_scratch_bytes(rows) || (uintptr_t)scratch % 8))
+        return fail(B200GSR_ERR_WORKSPACE, "scale_loss_live: scratch must be 8-byte aligned and hold %zu bytes (got %zu)",
+                    b200gsr_scale_loss_scratch_bytes(rows), scratch ? scratch_bytes : (size_t)0);
+    a.start[num_groups] = (int32_t)P;
+    a.rows = rows;
+    a.inv_rows = 0.0f;                      // formed on the device from the live counts
+    a.inv_3 = 1.0f / 3.0f;
+    a.scales = scales; a.grad_out = grad_out; a.loss_out = loss_out; a.d_scales = d_scales; a.accumulate = accumulate;
+    a.partials = static_cast<double*>(scratch);
+    a.B = B; a.P = (int32_t)P; a.num_groups = num_groups; a.live = live;
+    return check_cuda(gsr_launch_scale_loss_live(a, GSR_ST(stream)), "scale_loss_live");
+}
+
 int b200gsr_debug_counters(unsigned long long* device_counters) {
     g_stats = device_counters;
     return B200GSR_OK;
@@ -875,6 +925,7 @@ static int check_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups,
     if (!prm) return fail(B200GSR_ERR_BAD_ARG, "null view array");
     if (dyn && (!sc.dyn_views || !sc.dyn_seed))
         return fail(B200GSR_ERR_BAD_ARG, "views / seed must be device pointers to B step records and the seed");
+    if (sc.live_call && !sc.live) return fail(B200GSR_ERR_BAD_ARG, "live must be a device array [num_groups]");
     if (!dyn && (!sc.shs_noise || !sc.scale_noise))
         return fail(B200GSR_ERR_BAD_ARG, "shs_noise / scale_noise must be host arrays of B coefficients");
     int rc = check_groups(num_groups, groups, prm[0].M);
@@ -1094,6 +1145,35 @@ int b200gsr_backward_scene_dyn_stats(int32_t B, const b200gsr_params* prm, int32
                                      const b200gsr_group_stats* stats, const int32_t* stats_view, void* stream) {
     GsrScene sc{};
     sc.dyn_views = views; sc.dyn_seed = reinterpret_cast<const unsigned long long*>(seed);
+    return backward_scene(B, prm, num_groups, groups, grads, sc, true, d_scales, radii, out_depth_alpha, dL_dcolor,
+                          dL_ddepth_alpha, saved, saved_bytes, max_pairs, d_means2D, flags, frozen_groups, stream,
+                          true, stats, -1, stats_view);
+}
+
+int b200gsr_forward_scene_dyn_live(int32_t B, const b200gsr_params* prm, int32_t num_groups,
+                                   const b200gsr_group* groups, const b200gsr_step_view* views, const uint64_t* seed,
+                                   float* out_scales, float* out_color, float* out_depth_alpha, int32_t* radii,
+                                   void* scratch, size_t scratch_bytes, void* saved, size_t saved_bytes,
+                                   uint64_t max_pairs, uint32_t flags, uint32_t* host_notify, uint32_t notify_seq,
+                                   const int32_t* live, void* stream) {
+    GsrScene sc{};
+    sc.dyn_views = views; sc.dyn_seed = reinterpret_cast<const unsigned long long*>(seed);
+    sc.live = live; sc.live_call = true;
+    return forward_scene(B, prm, num_groups, groups, sc, true, out_scales, out_color, out_depth_alpha, radii, scratch,
+                         scratch_bytes, saved, saved_bytes, max_pairs, flags, host_notify, notify_seq, stream);
+}
+
+int b200gsr_backward_scene_dyn_live(int32_t B, const b200gsr_params* prm, int32_t num_groups,
+                                    const b200gsr_group* groups, const b200gsr_group_grad* grads,
+                                    const b200gsr_step_view* views, const uint64_t* seed, const float* d_scales,
+                                    const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
+                                    const float* dL_ddepth_alpha, void* saved, size_t saved_bytes,
+                                    uint64_t max_pairs, float* d_means2D, uint32_t flags, uint32_t frozen_groups,
+                                    const b200gsr_group_stats* stats, const int32_t* stats_view,
+                                    const int32_t* live, void* stream) {
+    GsrScene sc{};
+    sc.dyn_views = views; sc.dyn_seed = reinterpret_cast<const unsigned long long*>(seed);
+    sc.live = live; sc.live_call = true;
     return backward_scene(B, prm, num_groups, groups, grads, sc, true, d_scales, radii, out_depth_alpha, dL_dcolor,
                           dL_ddepth_alpha, saved, saved_bytes, max_pairs, d_means2D, flags, frozen_groups, stream,
                           true, stats, -1, stats_view);

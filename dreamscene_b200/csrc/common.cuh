@@ -4,7 +4,7 @@
 #include <stdint.h>
 #include <atomic>
 
-#include "../../include/b200gsr_stats.h"
+#include "../../include/b200gsr_reserve.h"
 
 #define GSR_TILE 16
 #define GSR_NEAR_Z 0.2f
@@ -239,6 +239,10 @@ struct GsrScene {
     const b200gsr_group_stats* stats;
     int32_t stats_view;
     const int32_t* dyn_stats_view;
+    // b200gsr_*_scene_dyn_live: device [num_groups] live row counts (include/b200gsr_reserve.h); project_sh /
+    // project_bwd run their LIVE instantiations.  Null otherwise.
+    const int32_t* live;
+    bool live_call;                      // a _live entry point: `live` must be set
 };
 
 struct GsrFwdArgs {
@@ -416,6 +420,9 @@ __host__ __device__ inline GsrAdamChunk gsr_adam_chunk(const GsrAdamEntry& e, lo
 cudaError_t gsr_launch_adam(int n, const b200gsr_adam_tensor* t, cudaStream_t s);
 // b200gsr_adam_step_dyn: the scalars of record i are read from scalars[6 i ..] in device memory
 cudaError_t gsr_launch_adam_dyn(int n, const b200gsr_adam_tensor* t, const float* scalars, cudaStream_t s);
+// b200gsr_adam_step_dyn_live: as _dyn, each tensor cut to its live elements (*live[i].rows * live[i].row_floats)
+cudaError_t gsr_launch_adam_dyn_live(int n, const b200gsr_adam_tensor* t, const float* scalars,
+                                     const b200gsr_adam_live* live, cudaStream_t s);
 // b200gsr_pair_report: fold a forward's pair count and overflow flag (its saved header) into report[2]
 cudaError_t gsr_launch_pair_report(const uint32_t* header, uint32_t* report, cudaStream_t s);
 
@@ -470,3 +477,11 @@ struct GsrScaleArgs {
     double* partials;               // with loss_out: gsr_l2_blocks(3 rows)
 };
 cudaError_t gsr_launch_scale_loss(const GsrScaleArgs& a, cudaStream_t s);
+// b200gsr_scale_loss_live: rows = B P over the groups' capacities; element e of view row r is live iff r's row in its
+// group is below live[group].  inv_rows is formed on the device from B sum(live).
+struct GsrScaleLiveArgs : GsrScaleArgs {
+    int32_t B, P, num_groups;
+    int32_t start[B200GSR_MAX_GROUPS + 1];   // first row of group g in a view; start[num_groups] = P
+    const int32_t* live;
+};
+cudaError_t gsr_launch_scale_loss_live(const GsrScaleLiveArgs& a, cudaStream_t s);

@@ -348,7 +348,61 @@ __global__ void __launch_bounds__(GSR_L2_THREADS) scale_finish_kernel(const GsrS
     if (threadIdx.x == 0) *a.loss_out = __double2float_rn(s / (3.0 * (double)a.rows));
 }
 
+// b200gsr_scale_loss_live: the live rows' count of group g, clamped to its capacity
+__device__ __forceinline__ int scale_live_rows(const GsrScaleLiveArgs& a, int g) {
+    return min(max(__ldg(a.live + g), 0), a.start[g + 1] - a.start[g]);
+}
+// fp32(1 / (B sum(live))) as the host forms fp32(1 / rows) for the compact layout
+__device__ __forceinline__ float scale_live_inv_rows(const GsrScaleLiveArgs& a, long long& rows) {
+    long long n = 0;
+    for (int g = 0; g < a.num_groups; ++g) n += scale_live_rows(a, g);
+    rows = (long long)a.B * n;
+    return __fdiv_rn(1.0f, (float)rows);
+}
+
+// The scalar path of scale_loss_kernel over the live elements only (rows over the groups' capacities); a dead
+// element adds nothing to the sum and gets a zero gradient (left as it is when accumulating).
+__global__ void __launch_bounds__(GSR_L2_THREADS) scale_loss_live_kernel(const GsrScaleLiveArgs a) {
+    const long long n = 3LL * a.rows;
+    const long long start = (long long)blockIdx.x * GSR_L2_CHUNK;
+    const long long end = start + GSR_L2_CHUNK < n ? start + GSR_L2_CHUNK : n;
+    float* ds = a.d_scales;
+    long long rows;
+    const float inv_rows = scale_live_inv_rows(a, rows);
+    const float c = ds ? __fmul_rn(__fmul_rn(__ldg(a.grad_out), inv_rows), a.inv_3) : 0.0f;
+    double acc = 0.0;
+    for (long long i = start + threadIdx.x; i < end; i += GSR_L2_THREADS) {
+        const int r = (int)((i / 3) % a.P);
+        int g = 0;
+        while (g + 1 < a.num_groups && r >= a.start[g + 1]) ++g;
+        const bool alive = r - a.start[g] < scale_live_rows(a, g);
+        if (a.loss_out && alive) acc += (double)__ldg(a.scales + i);
+        if (ds && alive) ds[i] = a.accumulate ? __fadd_rn(ds[i], c) : c;
+        else if (ds && !a.accumulate) ds[i] = 0.0f;
+    }
+    if (a.loss_out) {
+        const double s = block_sum(acc);
+        if (threadIdx.x == 0) a.partials[blockIdx.x] = s;
+    }
+}
+
+__global__ void __launch_bounds__(GSR_L2_THREADS) scale_finish_live_kernel(const GsrScaleLiveArgs a, int nblk) {
+    double s = 0.0;
+    for (int i = threadIdx.x; i < nblk; i += GSR_L2_THREADS) s += a.partials[i];
+    s = block_sum(s);
+    long long rows;
+    scale_live_inv_rows(a, rows);
+    if (threadIdx.x == 0) *a.loss_out = __double2float_rn(s / (3.0 * (double)rows));
+}
+
 }  // namespace
+
+cudaError_t gsr_launch_scale_loss_live(const GsrScaleLiveArgs& a, cudaStream_t s) {
+    const int nblk = (int)gsr_l2_blocks(3 * a.rows);
+    scale_loss_live_kernel<<<nblk, GSR_L2_THREADS, 0, s>>>(a);
+    if (a.loss_out) scale_finish_live_kernel<<<1, GSR_L2_THREADS, 0, s>>>(a, nblk);
+    return cudaGetLastError();
+}
 
 cudaError_t gsr_launch_tv_loss(const GsrTvArgs& a, cudaStream_t s) {
     const bool vec = a.W % 4 == 0 &&

@@ -40,6 +40,12 @@ struct GsrAdamDynTable {
     int row[B200GSR_ADAM_MAX_TENSORS];   // entries skip empty tensors, rows do not
 };
 
+// LIVE (b200gsr_adam_step_dyn_live): the DYN table plus, per entry, the device live row count and the row's floats.
+struct GsrAdamLiveTable : GsrAdamDynTable {
+    const int32_t* rows[B200GSR_ADAM_MAX_TENSORS];     // null: the whole tensor
+    int row_floats[B200GSR_ADAM_MAX_TENSORS];
+};
+
 // One CTA = one GSR_ADAM_CHUNK-element chunk of one tensor.  The vector path issues all of a thread's loads
 // (4 x 4 float4) before the first use, so each thread keeps 256 bytes in flight.
 __device__ __forceinline__ void adam_chunk(const GsrAdamEntry& e) {
@@ -72,13 +78,22 @@ __device__ __forceinline__ void adam_chunk(const GsrAdamEntry& e) {
     }
 }
 
-// DYN: each CTA loads its entry's six scalars from device memory once, in place of the table's.
-template <bool DYN = false>
+// DYN: each CTA loads its entry's six scalars from device memory once, in place of the table's.  LIVE (with DYN): the
+// entry ends at its live element count; a CTA whose chunk starts at or past it returns at once.
+template <bool DYN = false, bool LIVE = false>
 __global__ void __launch_bounds__(GSR_ADAM_THREADS)
-adam_step_kernel(const __grid_constant__ std::conditional_t<DYN, GsrAdamDynTable, GsrAdamTable> tab) {
+adam_step_kernel(const __grid_constant__ std::conditional_t<
+                 LIVE, GsrAdamLiveTable, std::conditional_t<DYN, GsrAdamDynTable, GsrAdamTable>> tab) {
     if constexpr (DYN) {
         const int k = gsr_adam_find(tab.t, blockIdx.x);
         GsrAdamEntry e = tab.t.e[k];
+        if constexpr (LIVE) {
+            if (tab.rows[k] != nullptr) {
+                const long long n = (long long)max(__ldg(tab.rows[k]), 0) * tab.row_floats[k];
+                if (n < e.n) e.n = n;
+            }
+            if ((blockIdx.x - e.block0) * (long long)GSR_ADAM_CHUNK >= e.n) return;
+        }
         const float* s = tab.scalars + 6 * (size_t)tab.row[k];
         e.w = __ldg(s); e.beta2 = __ldg(s + 1); e.omb2 = __ldg(s + 2); e.eps = __ldg(s + 3);
         e.step_size = __ldg(s + 4); e.bc2_sqrt = __ldg(s + 5);
@@ -108,5 +123,22 @@ cudaError_t gsr_launch_adam_dyn(int n, const b200gsr_adam_tensor* t, const float
     for (int i = 0, k = 0; i < n; ++i)
         if (t[i].n > 0) tab.row[k++] = i;
     adam_step_kernel<true><<<(unsigned)blocks, GSR_ADAM_THREADS, 0, s>>>(tab);
+    return cudaGetLastError();
+}
+
+cudaError_t gsr_launch_adam_dyn_live(int n, const b200gsr_adam_tensor* t, const float* scalars,
+                                     const b200gsr_adam_live* live, cudaStream_t s) {
+    GsrAdamLiveTable tab;
+    const long long blocks = gsr_adam_plan(n, t, &tab.t);
+    if (blocks == 0) return cudaSuccess;
+    if (blocks > 0x7fffffffLL) return cudaErrorInvalidConfiguration;
+    tab.scalars = scalars;
+    for (int i = 0, k = 0; i < n; ++i)
+        if (t[i].n > 0) {
+            tab.row[k] = i;
+            tab.rows[k] = live[i].rows;
+            tab.row_floats[k++] = live[i].row_floats;
+        }
+    adam_step_kernel<true, true><<<(unsigned)blocks, GSR_ADAM_THREADS, 0, s>>>(tab);
     return cudaGetLastError();
 }

@@ -289,6 +289,25 @@ struct StatsTable {
 };
 template <bool DYN>
 struct SceneStats : SceneFrozen<std::conditional_t<DYN, SceneBwdDyn, SceneBwd>> { StatsTable st; };
+// LIVE (b200gsr_*_scene_dyn_live): the device live row count of each group (include/b200gsr_reserve.h).  A derived
+// type, so that the other instantiations' kernel argument keeps its layout.
+template <typename S>
+struct SceneLive : S { const int32_t* live; };
+template <bool RAW, bool DYN, bool LIVE>
+using FwdSceneLive = std::conditional_t<LIVE, SceneLive<SceneFwdDyn>, FwdScene<RAW, DYN>>;
+template <bool DYN, bool LIVE>
+using StatsScene = std::conditional_t<LIVE, SceneLive<SceneStats<DYN>>, SceneStats<DYN>>;
+
+// LIVE: row `loc` of group `grp` -> its row in the compact layout (sum_{h<grp} live[h] + loc), the counter of its
+// augmentation noise, or -1 when it is dead (loc >= live[grp]).  Live counts are clamped to the group's capacity.
+template <typename S>
+__device__ __forceinline__ int live_row(const S& sc, int grp, size_t loc) {
+    int base = 0;
+#pragma unroll 1
+    for (int h = 0; h < grp; ++h) base += min(max(__ldg(sc.live + h), 0), sc.tab.start[h + 1] - sc.tab.start[h]);
+    const int lv = min(max(__ldg(sc.live + grp), 0), sc.tab.start[grp + 1] - sc.tab.start[grp]);
+    return (int)loc < lv ? base + (int)loc : -1;
+}
 
 struct ViewNoise {
     unsigned long long seed;
@@ -445,8 +464,10 @@ __device__ __forceinline__ void sh_color(const float (&B)[16], const float* row,
 // augmented exp scale and normalized rotation are formed per row, the visible rows' SH coefficients are staged from
 // f_dc / f_rest and augmented in shared memory before the colour is evaluated, and with sc.out_scales every row's
 // augmented scales are written out.  The packed input pointers are null.  Compile-time guards only, as for GEO.
-// DYN (with RAW): the view's per-step values come from device memory (view_noise).
-template <int MT, bool DET = false, bool GEO = false, bool RAW = false, bool DYN = false>
+// DYN (with RAW): the view's per-step values come from device memory (view_noise).  LIVE (with DYN): a row at or past
+// its group's live count (sc.live) is culled before any of its leaves is read (radius 0, no pairs, a zero out_scales
+// row), and a live row's noise is keyed by its compact row (live_row).
+template <int MT, bool DET = false, bool GEO = false, bool RAW = false, bool DYN = false, bool LIVE = false>
 __global__ void __launch_bounds__(kBlock)
 project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
                   const float* __restrict__ shs, const float* __restrict__ colors,
@@ -458,7 +479,7 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
                   int rec_base, int tile_row_off, int ntiles_total,
                   uint32_t* __restrict__ det_max, unsigned long long* __restrict__ det_fx,
                   unsigned long long* __restrict__ score_fx, uint32_t* __restrict__ det_queue,
-                  const FwdScene<RAW, DYN> sc) {
+                  const FwdSceneLive<RAW, DYN, LIVE> sc) {
     extern __shared__ __align__(16) float sh_buf[];
     __shared__ uint8_t vis_s[kBlock];
     const ViewNoise nz = view_noise<DYN>(sc, p);
@@ -481,26 +502,37 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
     int grp = 0;                 // RAW: the row's group and its row inside the group
     size_t loc = 0;
     RawShape rs;                 // RAW: the row's rasterizer shape inputs
+    int ci = i;                  // the row's noise counter (LIVE: its compact row)
+    bool dead = false;           // LIVE: the row is past its group's live count
     if (active) {
         if constexpr (RAW) {
             grp = find_group(sc.tab, i);
             loc = (size_t)(i - sc.tab.start[grp]);
-            const float* xp = sc.tab.xyz[grp] + 3 * loc;
-            x = __ldg(xp); y = __ldg(xp + 1); z = __ldg(xp + 2);
+            if constexpr (LIVE) { ci = live_row(sc, grp, loc); dead = ci < 0; }
+            if (!dead) {
+                const float* xp = sc.tab.xyz[grp] + 3 * loc;
+                x = __ldg(xp); y = __ldg(xp + 1); z = __ldg(xp + 2);
+            }
         } else {
             x = __ldg(means3D + 3 * (size_t)i); y = __ldg(means3D + 3 * (size_t)i + 1);
             z = __ldg(means3D + 3 * (size_t)i + 2);
         }
         geo_view(C, x, y, z, g);
+        if constexpr (LIVE) {
+            if (dead) g.tz = 0.0f;                   // culled by the depth test below
+        }
         rd.z = __float_as_uint(g.tz);
         if constexpr (RAW) {
-            if (g.tz > GSR_NEAR_Z || sc.out_scales != nullptr) {
+            if (!dead && (g.tz > GSR_NEAR_Z || sc.out_scales != nullptr)) {
                 RawLeaf lf;
-                raw_shape(sc.tab, grp, loc, i, GSR_SEED, GSR_C_SCALE, sc.view, lf, rs);
+                raw_shape(sc.tab, grp, loc, ci, GSR_SEED, GSR_C_SCALE, sc.view, lf, rs);
                 if (sc.out_scales != nullptr) {      // every row, culled ones included (the scale loss reads them all)
                     float* so = sc.out_scales + 3 * (size_t)i;
                     so[0] = rs.s[0]; so[1] = rs.s[1]; so[2] = rs.s[2];
                 }
+            } else if (dead && sc.out_scales != nullptr) {
+                float* so = sc.out_scales + 3 * (size_t)i;
+                so[0] = 0.0f; so[1] = 0.0f; so[2] = 0.0f;
             }
         }
         if (g.tz > GSR_NEAR_Z) {
@@ -575,7 +607,7 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
     } else if (RAW || shs != nullptr) {
         if constexpr (RAW) {     // this thread's own row: no barrier needed
             if (GSR_C_SHS != 0.0f)
-                raw_sh_noise<false>(sh_buf + threadIdx.x * stride, 3 * ncoef, (size_t)i * 3 * p.M, GSR_SEED,
+                raw_sh_noise<false>(sh_buf + threadIdx.x * stride, 3 * ncoef, (size_t)ci * 3 * p.M, GSR_SEED,
                                     kStreamShs + 2u * sc.view, GSR_C_SHS);
         }
         float dx = x - C.cam[0], dy = y - C.cam[1], dz = z - C.cam[2];
@@ -660,12 +692,13 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
                    float* __restrict__ d_opac, float* __restrict__ d_scales,
                    float* __restrict__ d_rots, float* __restrict__ d_cov3d,
                    const BwdScene<RAW, DYN, FROZEN> sc) {
-    constexpr bool STATS = false;
+    constexpr bool STATS = false, LIVE = false;
 #include "project_bwd_body.cuh"
 }
 
-// The raw-parameter backward with the densification statistics (b200gsr_backward_scene[_dyn]_stats).
-template <bool DYN, bool FROZEN>
+// The raw-parameter backward with the densification statistics (b200gsr_backward_scene[_dyn]_stats).  LIVE (with
+// DYN, b200gsr_backward_scene_dyn_live): dead rows get zero gradients and no statistics, and read no leaf.
+template <bool DYN, bool FROZEN, bool LIVE = false>
 __global__ void __launch_bounds__(kBlock, 5)
 project_bwd_stats_kernel(b200gsr_params p, const float* __restrict__ means3D,
                          const float* __restrict__ shs, const float* __restrict__ colors,
@@ -677,7 +710,7 @@ project_bwd_stats_kernel(b200gsr_params p, const float* __restrict__ means3D,
                          float* __restrict__ d_shs, float* __restrict__ d_colors,
                          float* __restrict__ d_opac, float* __restrict__ d_scales,
                          float* __restrict__ d_rots, float* __restrict__ d_cov3d,
-                         const SceneStats<DYN> sc) {
+                         const StatsScene<DYN, LIVE> sc) {
     constexpr int MT = 0;
     constexpr bool RAW = true, STATS = true;
 #include "project_bwd_body.cuh"
@@ -708,7 +741,7 @@ static SceneFwd scene_fwd(const GsrFwdArgs& a) {
     return sc;
 }
 
-template <int MT, bool DET, bool GEO = false, bool RAW = false, bool DYN = false>
+template <int MT, bool DET, bool GEO = false, bool RAW = false, bool DYN = false, bool LIVE = false>
 static void launch_project_sh(const GsrFwdArgs& a, int P, size_t smem) {
     // multisplit path: counters + the single per-tile counter array are zeroed in the prologue
     // (api.cu issues a memset instead on the large-grid fallback, where this kernel counts itself)
@@ -716,10 +749,11 @@ static void launch_project_sh(const GsrFwdArgs& a, int P, size_t smem) {
     tg.gy = a.num_views * a.gy_view; tg.ntiles = tg.gx * tg.gy;      // the stacked image
     const int nzero = gsr_use_multisplit(tg.ntiles) ? (int)gsr_counter_words(a.sl, tg.ntiles) : 0;
     const bool bwd = !(a.flags & B200GSR_FWD_NO_BACKWARD);
-    FwdScene<RAW, DYN> sc{};
+    FwdSceneLive<RAW, DYN, LIVE> sc{};
     if constexpr (RAW) static_cast<SceneFwd&>(sc) = scene_fwd(a);
     if constexpr (DYN) sc.dyn = SceneDyn{a.scene->dyn_views, a.scene->dyn_seed};
-    project_sh_kernel<MT, DET, GEO, RAW, DYN><<<(P + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
+    if constexpr (LIVE) sc.live = a.scene->live;
+    project_sh_kernel<MT, DET, GEO, RAW, DYN, LIVE><<<(P + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
         a.prm, a.means3D, a.shs, a.colors, a.opac, a.scales, a.rots, a.cov3d, a.radii,
         reinterpret_cast<uint4*>(a.scratch + a.sl.rectdepth),
         reinterpret_cast<GsrRec*>(a.saved + a.vl.geom),
@@ -743,7 +777,9 @@ cudaError_t gsr_launch_project(const GsrFwdArgs& a, bool geo) {
     } else if (a.scene) {
         // the raw rows are staged with 4-byte copies whatever M is: no per-M instantiation
         const bool dyn = a.scene->dyn_views != nullptr;
-        if (dyn && a.det) launch_project_sh<0, true, false, true, true>(a, P, smem);
+        if (a.scene->live && a.det) launch_project_sh<0, true, false, true, true, true>(a, P, smem);
+        else if (a.scene->live) launch_project_sh<0, false, false, true, true, true>(a, P, smem);
+        else if (dyn && a.det) launch_project_sh<0, true, false, true, true>(a, P, smem);
         else if (dyn) launch_project_sh<0, false, false, true, true>(a, P, smem);
         else if (a.det) launch_project_sh<0, true, false, true>(a, P, smem);
         else launch_project_sh<0, false, false, true>(a, P, smem);
@@ -785,9 +821,9 @@ static void launch_project_bwd(const GsrBwdArgs& a, int g_begin, int g_end, size
         a.d_colors, a.d_opac, a.d_scales, a.d_rots, a.d_cov3d, sc);
 }
 
-template <bool DYN, bool FROZEN>
+template <bool DYN, bool FROZEN, bool LIVE = false>
 static void launch_project_bwd_stats(const GsrBwdArgs& a, int g_begin, int g_end, size_t smem) {
-    SceneStats<DYN> sc{};
+    StatsScene<DYN, LIVE> sc{};
     static_cast<SceneBwd&>(sc) = scene_bwd(a);
     if constexpr (DYN) sc.dyn = SceneDyn{a.scene->dyn_views, a.scene->dyn_seed};
     sc.frozen = a.scene->frozen;
@@ -799,7 +835,8 @@ static void launch_project_bwd_stats(const GsrBwdArgs& a, int g_begin, int g_end
     }
     sc.st.view = s.stats_view;
     sc.st.view_dev = s.dyn_stats_view;
-    project_bwd_stats_kernel<DYN, FROZEN><<<(g_end - g_begin + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
+    if constexpr (LIVE) sc.live = s.live;
+    project_bwd_stats_kernel<DYN, FROZEN, LIVE><<<(g_end - g_begin + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
         a.prm, a.means3D, a.shs, a.colors, a.scales, a.rots, a.cov3d, a.radii,
         reinterpret_cast<float*>(a.saved + a.vl.dgeom),
         reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE, g_begin, g_end,
@@ -813,7 +850,10 @@ cudaError_t gsr_launch_project_bwd(const GsrBwdArgs& a) {
     if (g_end <= g_begin) return cudaSuccess;
     const size_t smem = (a.shs || a.scene) ? (size_t)kBlock * sh_row_stride(a.prm.M) * sizeof(float) : 0;
     const bool frozen = a.scene && a.scene->frozen;
-    if (a.scene && a.scene->stats_mode) {
+    if (a.scene && a.scene->live) {     // b200gsr_backward_scene_dyn_live: every launch is the STATS kernel's
+        if (frozen) launch_project_bwd_stats<true, true, true>(a, g_begin, g_end, smem);
+        else launch_project_bwd_stats<true, false, true>(a, g_begin, g_end, smem);
+    } else if (a.scene && a.scene->stats_mode) {
         const bool dyn = a.scene->dyn_views != nullptr;
         if (dyn && frozen) launch_project_bwd_stats<true, true>(a, g_begin, g_end, smem);
         else if (dyn) launch_project_bwd_stats<true, false>(a, g_begin, g_end, smem);

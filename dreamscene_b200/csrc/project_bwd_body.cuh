@@ -1,5 +1,6 @@
 // The statements of project_bwd_kernel and project_bwd_stats_kernel (project.cu), included into the body of each.
-// In scope: the kernel's parameters and the compile-time MT, RAW, DYN, FROZEN and STATS (see project_bwd_kernel).
+// In scope: the kernel's parameters and the compile-time MT, RAW, DYN, FROZEN, STATS and LIVE (see project_bwd_kernel
+// and project_bwd_stats_kernel).
 extern __shared__ __align__(16) float sh_buf[];
 __shared__ uint8_t vis_s[kBlock];
 const ViewNoise nz = view_noise<DYN>(sc, p);
@@ -28,11 +29,15 @@ float4* dg = nullptr;
 int grp = 0;                 // RAW: the row's group, its row inside the group and its shape leaves
 size_t loc = 0;
 RawLeaf lf;
+int ci = i;                  // the row's noise counter (LIVE: its compact row)
+bool dead = false;           // LIVE: the row is past its group's live count (its radius is 0: not visible)
 if constexpr (RAW) {
     if (active) {
         grp = find_group(sc.tab, i);
         loc = (size_t)(i - sc.tab.start[grp]);
-        if (!fz && (vis || sc.d_scales != nullptr)) raw_shape(sc.tab, grp, loc, i, GSR_SEED, GSR_C_SCALE, sc.view, lf, raw);
+        if constexpr (LIVE) { ci = live_row(sc, grp, loc); dead = ci < 0; }
+        if (!fz && !dead && (vis || sc.d_scales != nullptr))
+            raw_shape(sc.tab, grp, loc, ci, GSR_SEED, GSR_C_SCALE, sc.view, lf, raw);
     }
 }
 if (vis) {
@@ -52,7 +57,7 @@ if (RAW || shs != nullptr) {
 }
 if constexpr (RAW) {         // the visible rows' SH coefficients as the forward augmented them (own row)
     if (vis && GSR_C_SHS != 0.0f)
-        raw_sh_noise<false>(sh_buf + threadIdx.x * stride, 3 * ncoef, (size_t)i * 3 * p.M, GSR_SEED,
+        raw_sh_noise<false>(sh_buf + threadIdx.x * stride, 3 * ncoef, (size_t)ci * 3 * p.M, GSR_SEED,
                             kStreamShs + 2u * sc.view, GSR_C_SHS);
 }
 float dmean[3] = {0.f, 0.f, 0.f};
@@ -246,7 +251,7 @@ if constexpr (RAW) {
     // ---- leaf gradients.  View 0 writes every row (zeros on culled rows); a later view adds into the rows it
     // touched: its visible rows, and every row's _scaling when the augmented scales have an incoming gradient.
     const bool first = sc.view == 0;
-    const bool has_ds = sc.d_scales != nullptr;
+    const bool has_ds = sc.d_scales != nullptr && !dead;      // a dead row's scales gradient is zero
     if (active) {
         if (!STATS || d_means2D != nullptr) {
             d_means2D[3 * (size_t)i] = dm2[0]; d_means2D[3 * (size_t)i + 1] = dm2[1]; d_means2D[3 * (size_t)i + 2] = 0.f;
@@ -307,7 +312,7 @@ if constexpr (RAW) {
     // to f_dc / f_rest, half a warp per row (the leaves' rows are not 16-byte aligned).
     const int nf = 3 * ncoef, nrow = 3 * p.M;
     if (vis && GSR_C_SHS != 0.0f)
-        raw_sh_noise<true>(sh_buf + threadIdx.x * stride, nf, (size_t)i * nrow, GSR_SEED, kStreamShs + 2u * sc.view,
+        raw_sh_noise<true>(sh_buf + threadIdx.x * stride, nf, (size_t)ci * nrow, GSR_SEED, kStreamShs + 2u * sc.view,
                            GSR_C_SHS);
     __syncthreads();
     // Half a warp per row, four rows per thread at a time: a later view loads the old values of all of them

@@ -45,6 +45,19 @@ backward graph instead of by an eager kernel over ``d_means2D`` afterwards:
                    densify_stats=[(g.xyz_gradient_accum, g.denom, g.max_radii2D) for g in models], keep_means2D=False)
     sg.step(stats_view=-1 if step < densify_until_iter else None)     # -1 = view B-1, None = off; no re-capture
 
+Reserved groups (f13, dreamscene_b200.reserve.ReservedGroup) hold their rows at a fixed capacity with the live count
+in device memory, so densify, prune, filter and opacity reset rewrite a prefix of the same tensors and the next
+render() replays instead of capturing again:
+
+    g = ReservedGroup.from_group(model)
+    sg = StepGraph([g], [opt], views=B, height=H, width=W, densify_stats=[g], keep_means2D=False)
+    out = sg.render(...); loss.backward(); sg.step(optimize=False, stats_view=-1)
+    g.densify_and_prune(opt, max_grad, min_opacity, extent, max_screen_size)     # the next render() replays
+
+Reserved and plain groups mix (a plain group's live count is its row count).  The layout holds the capacities;
+out.radii, out.scales, d_means2D and grads keep the capacity layout with zeros in the dead rows.  A densify_stats
+entry may be the reserved group itself (its statistics, followed through a growth).
+
 ``step(optimize=False)`` replays the backward only (``grads`` and ``d_means2D``), leaving parameters, moments and
 step counters as they are: the reference's densify step, whose optimizer.step() follows densify_and_prune and so
 updates nothing.
@@ -66,6 +79,7 @@ import torch
 from . import _lib
 from . import optim as O
 from . import rasterizer as R
+from . import reserve as RS
 from . import scene as S
 
 _SEED_WORDS = 8             # the uint64 seed, padded so the view records start 32-byte aligned
@@ -181,8 +195,16 @@ class StepGraph:
         return S._frozen_mask(self.frozen, len(self.groups), "StepGraph")
 
     def _stats(self):
-        """The validated densify_stats entries (scene._densify_stats), None when no group gathers."""
-        return S._densify_stats(self.densify_stats, self.groups, self._frozen_key(), "StepGraph")
+        """The validated densify_stats entries (scene._densify_stats), None when no group gathers.  An entry that is a
+        ReservedGroup stands for its current statistics tensors."""
+        entries = self.densify_stats
+        if entries is not None:
+            entries = [e.stats if isinstance(e, RS.ReservedGroup) else e for e in entries]
+        return S._densify_stats(entries, self.groups, self._frozen_key(), "StepGraph")
+
+    def _reserved(self):
+        """One bool per group: a ReservedGroup (part of the layout key: it selects the _live entry points)."""
+        return tuple(isinstance(g, RS.ReservedGroup) for g in self.groups)
 
     def _stats_key(self):
         """The statistics tensors' pointers and keep_means2D, part of the layout key."""
@@ -244,7 +266,7 @@ class StepGraph:
                     st = opt.state.get(p, {})
                     states.append((id(p), st["exp_avg"].data_ptr() if st else 0, st["exp_avg_sq"].data_ptr() if st else 0))
         return (P, M, ptrs, tuple(states), tuple(float(s.scale_modifier) for s in settings), det, self._target_key(),
-                self._reg_key(), self._frozen_key(), self._stats_key())
+                self._reg_key(), self._frozen_key(), self._stats_key(), self._reserved())
 
     def _upload(self, settings, rec, seed, focal, tidx):
         """One pinned staging tensor, one non_blocking copy of it (plus one device concatenation when the cameras
@@ -330,6 +352,17 @@ class StepGraph:
         table = S._group_table(raw)
         fmask = self._frozen_key()
         grads = [[None] * 6 if (fmask >> k) & 1 else [torch.zeros_like(t) for t in ts] for k, ts in enumerate(raw)]
+        # reserved groups: the live row counts the kernels read, copied from each group's `live` at the start of
+        # every render (a plain group's entry is its row count)
+        reserved = self._reserved()
+        live_mode = any(reserved)
+        live_t = torch.tensor([int(ts[0].shape[0]) for ts in raw], dtype=torch.int32, device=dev)
+        group_of = {id(t): i // 6 for i, t in enumerate(flat)}
+
+        def copy_live():
+            for k, g in enumerate(self.groups):
+                if reserved[k]:
+                    live_t[k:k + 1].copy_(g.live)
         garr = (_lib.GroupGrad * ng)()
         for k, ts in enumerate(grads):
             for name, t in zip(("xyz", "opacity", "scaling", "rotation", "f_dc", "f_rest"), ts):
@@ -340,9 +373,14 @@ class StepGraph:
         tables = []
         for i0 in range(0, len(records), _lib.ADAM_MAX_TENSORS):
             part = records[i0:i0 + _lib.ADAM_MAX_TENSORS]
+            live_arr = None
+            if live_mode:       # each reserved leaf stops at its group's live rows
+                live_arr = (_lib.AdamLive * len(part))(*[
+                    _lib.AdamLive(live_t.data_ptr() + 4 * group_of[id(p)], p[0].numel() if p.shape[0] else 1, 0)
+                    if reserved[group_of[id(p)]] else _lib.AdamLive(None, 0, 0) for p, *_ in part])
             tables.append((i0, (_lib.AdamTensor * len(part))(*[_lib.AdamTensor(p.data_ptr(), g.data_ptr(), m.data_ptr(),
                                                                                v.data_ptr(), p.numel())
-                                                                for p, g, m, v, *_ in part])))
+                                                                for p, g, m, v, *_ in part]), live_arr))
         # static outputs and gradient inputs
         color = torch.empty(3, Hs, W, device=dev)
         da = torch.empty(2, Hs, W, device=dev)
@@ -401,13 +439,25 @@ class StepGraph:
                                                    ptr(reg_loss[k]) if forward else None, None if forward else ptr(gx),
                                                    1, ptr(tv_scratch[k]), tv_scratch[k].numel(), _lib.stream(dev)),
                                "b200gsr_tv_loss")
-            if reg[2] is not None:
+            if reg[2] is not None and live_mode:        # the mean over the live rows
+                _lib.check(lib.b200gsr_scale_loss_live(B, ng, table, ptr(live_t), ptr(scales),
+                                                       None if forward else ptr(reg_go[2]),
+                                                       ptr(reg_loss[2]) if forward else None,
+                                                       None if forward else ptr(g_scales), scale_acc, ptr(scale_scratch),
+                                                       scale_scratch.numel(), _lib.stream(dev)),
+                           "b200gsr_scale_loss_live")
+            elif reg[2] is not None:
                 _lib.check(lib.b200gsr_scale_loss(B * P, ptr(scales), None if forward else ptr(reg_go[2]),
                                                   ptr(reg_loss[2]) if forward else None,
                                                   None if forward else ptr(g_scales), scale_acc, ptr(scale_scratch),
                                                   scale_scratch.numel(), _lib.stream(dev)), "b200gsr_scale_loss")
 
         def launch(cap, flags, scratch, saved, notify_ptr, seq):
+            if live_mode:
+                return lib.b200gsr_forward_scene_dyn_live(B, prm, ng, table, views_p, seed_p, ptr(scales), ptr(color),
+                                                          ptr(da), ptr(radii), ptr(scratch), scratch.numel(), ptr(saved),
+                                                          saved.numel(), cap, flags, notify_ptr, seq, ptr(live_t),
+                                                          _lib.stream(dev))
             return lib.b200gsr_forward_scene_dyn(B, prm, ng, table, views_p, seed_p, ptr(scales), ptr(color), ptr(da),
                                                  ptr(radii), ptr(scratch), scratch.numel(), ptr(saved), saved.numel(),
                                                  cap, flags, notify_ptr, seq, _lib.stream(dev))
@@ -436,6 +486,14 @@ class StepGraph:
                                                          ptr(stats_bwd), ptr(d_da4), bwd_flags, _lib.stream(dev)),
                        "b200gsr_disparity_backward")
             g_da.view(2, B, Hp, W)[:, :, :H].copy_(d_da4.permute(1, 0, 2, 3))
+            if live_mode:
+                _lib.check(lib.b200gsr_backward_scene_dyn_live(B, prm, ng, table, garr, views_p, seed_p, ptr(g_scales),
+                                                               ptr(radii), ptr(da), ptr(g_color), ptr(g_da), ptr(saved),
+                                                               saved.numel(), cap, ptr(d_means2D), bwd_flags, fmask,
+                                                               stats_arr, ptr(stats_view_t), ptr(live_t),
+                                                               _lib.stream(dev)),
+                           "b200gsr_backward_scene_dyn_live")
+                return
             if with_stats:
                 _lib.check(lib.b200gsr_backward_scene_dyn_stats(B, prm, ng, table, garr, views_p, seed_p, ptr(g_scales),
                                                                 ptr(radii), ptr(da), ptr(g_color), ptr(g_da), ptr(saved),
@@ -456,6 +514,7 @@ class StepGraph:
             key = (B, P, H, W)
             run_cap, _ = d.capacity_for(key, B * P, False)
             issued = {}
+            copy_live()
 
             def issue(c):
                 issued["saved"], slot, seq = R._issue_once(d, layout, fwd_flags, c, launch, skey, False,
@@ -468,6 +527,12 @@ class StepGraph:
             # the graphs run at the capacity a later eager forward of this shape would use: the user's, or twice the
             # measured count
             cap = max(run_cap, d.capacity_for(key, B * P, True)[0])
+            if live_mode:
+                # reserved rows: the measured pairs per live row (with the 2x head-room of d.note) for every row of the
+                # capacity, so that an event that fills the reserve replays without overflowing (DESIGN.md f13)
+                p_live = sum(g.live_count if reserved[k] else int(raw[k][0].shape[0]) for k, g in enumerate(self.groups))
+                if p_live > 0:
+                    cap = max(cap, R._round_cap(-(-d.caps.get(key, cap) * P // p_live)))
             scratch_bytes, _ = R._layouts(B * P, Hs, W, cap, True, det)
             d.ensure_scratch(skey, scratch_bytes)
             torch.cuda.current_stream(dev).synchronize()
@@ -475,6 +540,7 @@ class StepGraph:
             g_render, g_backward = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
             g_adam = torch.cuda.CUDAGraph() if tables else None     # an empty graph cannot be replayed
             with torch.cuda.graph(g_render, pool=pool):
+                copy_live()
                 saved, _, _ = R._issue_once(d, layout, fwd_flags, cap, launch, skey, True,
                                             "b200gsr_forward_scene_dyn", Exception)
                 _lib.check(lib.b200gsr_pair_report(ptr(saved), ptr(report), _lib.stream(dev)), "b200gsr_pair_report")
@@ -491,10 +557,14 @@ class StepGraph:
                     backward(saved, cap, scale_acc=0)
             if g_adam is not None:
                 with torch.cuda.graph(g_adam, pool=pool):
-                    for i0, arr in tables:
-                        _lib.check(lib.b200gsr_adam_step_dyn(len(arr), arr,
-                                                             C.c_void_p(self._scalars.data_ptr() + 24 * i0),
-                                                             _lib.stream(dev)), "b200gsr_adam_step_dyn")
+                    for i0, arr, live_arr in tables:
+                        scal = C.c_void_p(self._scalars.data_ptr() + 24 * i0)
+                        if live_arr is not None:
+                            _lib.check(lib.b200gsr_adam_step_dyn_live(len(arr), arr, scal, live_arr, _lib.stream(dev)),
+                                       "b200gsr_adam_step_dyn_live")
+                        else:
+                            _lib.check(lib.b200gsr_adam_step_dyn(len(arr), arr, scal, _lib.stream(dev)),
+                                       "b200gsr_adam_step_dyn")
         if target is None:
             for t in (image, disp, alpha, scales):
                 t.requires_grad_(True)
@@ -503,7 +573,7 @@ class StepGraph:
         self.reg_loss = reg_loss
         self._accumulated = [reg[0] is not None, reg[1] is not None, False, reg[2] is not None]
         self._keep = (keep, prm, table, garr, tables, raw, saved, color, da, da4, stats, stats_bwd, g_color, g_da, d_da4,
-                      stats_arr, stats_view_t)
+                      stats_arr, stats_view_t, live_t)
         self._stats_view = (stats_view_t, -1) if dstats is not None else None    # device slot, value last written
         self._static_grads = (g_image, g_disp, g_alpha, g_scales)
         self._leaves = list(flat)
@@ -524,6 +594,11 @@ class StepGraph:
             raise RuntimeError("StepGraph does not reduce gradients over ranks; view sharding cannot be replayed")
         flat, M, P = S._scene_groups(self.groups)
         S._check_device(flat)
+        for k, g in enumerate(self.groups):
+            if isinstance(g, RS.ReservedGroup) and not (0 <= g.live_count <= g.capacity and g.live.numel() == 1 and
+                                                         g.live.dtype == torch.int32 and g.live.device == flat[0].device):
+                raise ValueError(f"StepGraph: reserved group {k}: live count {g.live_count} not in 0..{g.capacity} or "
+                                 "its `live` is not a device int32 [1] on the groups' device")
         rec = self._views(settings_list, shs_aug, scale_aug, M)
         tidx = self._target_indices(target_index)
         self._reg_key()
