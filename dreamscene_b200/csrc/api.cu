@@ -335,9 +335,10 @@ int b200gsr_scratch_layout_query(int32_t P, int32_t H, int32_t W, uint64_t max_p
     out->tile_count = off;  off = align_up(off + (size_t)GSR_COPIES * g.ntiles * sizeof(uint32_t));
     out->tile_cursor = off; off = align_up(off + (size_t)GSR_COPIES * g.ntiles * sizeof(uint32_t));
     out->rectdepth = off;   off = align_up(off + (size_t)P * sizeof(uint4));
-    {
-        const size_t nblk = (size_t)gsr_ms_blocks(P);
-        out->ms_hist = off; off = align_up(off + (gsr_use_multisplit(g.ntiles) ? nblk * g.ntiles * sizeof(uint32_t) : 0));
+    out->ms_hist = off;
+    if (gsr_use_multisplit(g.ntiles)) {   // per-CTA tile histograms, then the padded key buffer (common.cuh)
+        off = gsr_pad_keys_offset(*out, P, g.ntiles);
+        off = align_up(off + (size_t)gsr_pad_key_capacity(max_pairs, P, g.ntiles) * sizeof(unsigned long long));
     }
     out->total = off;
     return B200GSR_OK;

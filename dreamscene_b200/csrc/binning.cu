@@ -9,10 +9,12 @@
 //   scan_order_kernel : exclusive scan -> tile_start[], cursors, total pair count (also written to a
 //                       mapped host word), and the work order (tiles by list length, longest first)
 //   multisplit<scatter>: every Gaussian appends (depth_bits<<32 | idx) to each tile it touches; a CTA
-//                       reserves one slice per touched tile, ranks inside it come from smem atomics
-//                       [fallback: scatter_kernel with returned global atomics]
+//                       reserves one slice per touched tile, padded to whole 32-byte sectors, in a
+//                       padded key buffer, stages the keys in smem and writes the slices out whole
+//                       [fallback: scatter_kernel with returned global atomics, straight into the lists]
 //                       (arrival order inside a tile is arbitrary ...)
-//   sort kernels      : ... and is then fixed by sorting each tile's keys on (depth bits, idx):
+//   sort kernels      : ... and is then fixed by sorting each tile's keys on (depth bits, idx), after
+//                       the pad slots are dropped:
 //                       identical to a stable sort of (tile<<32 | depth bits) over pairs emitted
 //                       in Gaussian-index order, i.e. bit-exact with the oracle's lists.
 //                       In-smem LSD radix sort (8-bit digits, match.any ranking, constant digit
@@ -125,48 +127,55 @@ scan_order_kernel(int ntiles, int ncopies, uint32_t max_pairs, const uint32_t* _
 
 // Single-pass variant for the multisplit path (one counter copy, ntiles <= 1024*kScanItems): every
 // thread owns kScanItems consecutive tiles in registers, so there are two barriers in total and
-// the counts are never re-read.
+// the counts are never re-read.  It also scans the padded counts into the tiles' segments of the
+// padded key buffer (pad_start[0..ntiles]) and the scatter's cursors into them.
 constexpr int kScanItems = GSR_MS_MAX_TILES / 1024;   // 12
 
 __global__ void __launch_bounds__(1024)
 scan_order_fast_kernel(int ntiles, uint32_t max_pairs, const uint32_t* __restrict__ tile_count,
-                       uint32_t* __restrict__ tile_start, uint32_t* __restrict__ tile_cursor,
+                       const uint32_t* __restrict__ pad_count, uint32_t* __restrict__ tile_start,
+                       uint32_t* __restrict__ pad_start, uint32_t* __restrict__ pad_cursor,
                        uint32_t* __restrict__ work_order, uint32_t* __restrict__ header,
                        volatile uint32_t* host_notify, uint32_t notify_seq) {
     extern __shared__ uint32_t cnt_s[];                  // [ntiles] copy of the counts for the last pass
-    __shared__ uint32_t warp_sums[32];
+    __shared__ uint32_t warp_sums[32], pad_warp_sums[32];
     __shared__ uint32_t bucket_cnt[33];
     __shared__ uint32_t bucket_pos[33];
     __shared__ uint32_t total_s;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const int per = (ntiles + 1023) / 1024;             // tiles per thread (<= kScanItems)
     if (tid < 33) bucket_cnt[tid] = 0;
-    uint32_t v[kScanItems], sum = 0;
+    uint32_t v[kScanItems], sum = 0, pv[kScanItems], pad_sum = 0;   // pair counts, padded counts
 #pragma unroll
     for (int k = 0; k < kScanItems; ++k) {
         const int t = tid * per + k;
         v[k] = (k < per && t < ntiles) ? __ldg(tile_count + t) : 0u;
+        pv[k] = (k < per && t < ntiles) ? __ldg(pad_count + t) : 0u;
         if (k < per && t < ntiles) cnt_s[t] = v[k];
         sum += v[k];
+        pad_sum += pv[k];
     }
-    uint32_t incl = sum;
+    uint32_t incl = sum, pad_incl = pad_sum;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
         const uint32_t n = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += n;
+        const uint32_t pn = __shfl_up_sync(0xffffffffu, pad_incl, o);
+        if (lane >= o) { incl += n; pad_incl += pn; }
     }
-    if (lane == 31) warp_sums[wid] = incl;
+    if (lane == 31) { warp_sums[wid] = incl; pad_warp_sums[wid] = pad_incl; }
     __syncthreads();
     if (wid == 0) {
-        const uint32_t w = warp_sums[lane];
-        uint32_t wi = w;
+        const uint32_t w = warp_sums[lane], pw = pad_warp_sums[lane];
+        uint32_t wi = w, pwi = pw;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
             const uint32_t n = __shfl_up_sync(0xffffffffu, wi, o);
-            if (lane >= o) wi += n;
+            const uint32_t pn = __shfl_up_sync(0xffffffffu, pwi, o);
+            if (lane >= o) { wi += n; pwi += pn; }
         }
         warp_sums[lane] = wi - w;   // exclusive
-        if (lane == 31) total_s = wi;
+        pad_warp_sums[lane] = pwi - pw;
+        if (lane == 31) { total_s = wi; pad_start[ntiles] = pwi; }
     }
 #pragma unroll
     for (int k = 0; k < kScanItems; ++k) {
@@ -174,12 +183,13 @@ scan_order_fast_kernel(int ntiles, uint32_t max_pairs, const uint32_t* __restric
         if (k < per && t < ntiles) atomicAdd(&bucket_cnt[size_bucket(v[k])], 1u);
     }
     __syncthreads();
-    uint32_t run = warp_sums[wid] + incl - sum;
+    uint32_t run = warp_sums[wid] + incl - sum, pad_run = pad_warp_sums[wid] + pad_incl - pad_sum;
 #pragma unroll
     for (int k = 0; k < kScanItems; ++k) {
         const int t = tid * per + k;
-        if (k < per && t < ntiles) { tile_start[t] = run; tile_cursor[t] = run; }
+        if (k < per && t < ntiles) { tile_start[t] = run; pad_start[t] = pad_run; pad_cursor[t] = pad_run; }
         run += v[k];
+        pad_run += pv[k];
     }
     if (wid == 0) {   // exclusive prefix over the 33 length buckets (bucket 32 = empty tiles, handled by lane 0)
         const uint32_t c = bucket_cnt[lane];
@@ -257,27 +267,34 @@ scatter_kernel(int P, int gx, int ntiles, uint32_t max_pairs, const uint4* __res
 
 // ---------------------------------------------------------------------------------------------
 // Block multisplit (default path).  count: smem histogram of the CTA's tile hits, then ONE global
-// RED per touched tile; the histogram is kept in global memory.  scatter: re-reads it, ONE returned
-// global atomic per touched tile reserves the CTA's contiguous slice of that tile's segment, then
-// every pair takes its slot inside the slice from a shared-memory atomic.
+// RED per touched tile into the pair counts and one into the padded counts (rounded up to 4 keys);
+// the histogram is kept in global memory.  scatter: re-reads it, ONE returned global atomic per
+// touched tile reserves the CTA's slice of that tile's segment in the padded key buffer, rounded up
+// to whole 32-byte sectors.  The keys are staged in shared memory at the slices' local offsets (pad
+// slots prefilled with ~0ull) and copied out as 16-byte stores by consecutive threads, so every
+// sector of the output is written whole by one warp instruction: scattered 8-byte stores would
+// leave partly written sectors that L2 has to read back from HBM when it evicts them.  The staging
+// buffer holds a band of consecutive tiles at a time; the CTA cuts the bands from its own histogram
+// and clips every rectangle to the band, so all pairs are walked once.
 // ---------------------------------------------------------------------------------------------
 template <bool SCATTER>
-__global__ void __launch_bounds__(1024)
-multisplit_kernel(int P, int per, int gx, int ntiles, uint32_t max_pairs, const uint4* __restrict__ rectdepth,
-                  uint32_t* __restrict__ tile_count, uint32_t* __restrict__ tile_cursor,
-                  uint32_t* __restrict__ block_hist, unsigned long long* __restrict__ keys) {
-    extern __shared__ uint32_t ms_smem[];
-    uint32_t* hist = ms_smem;            // [ntiles] counts (count) / global write cursors of this CTA's slices (scatter)
+__global__ void __launch_bounds__(1024, 2)      // two CTAs per SM: at most 32 registers
+multisplit_kernel(int P, int per, int gx, int ntiles, const uint4* __restrict__ rectdepth,
+                  uint32_t* __restrict__ tile_count, uint32_t* __restrict__ pad_count,
+                  uint32_t* __restrict__ pad_cursor, uint32_t* __restrict__ block_hist,
+                  unsigned long long* __restrict__ pad_keys, uint32_t pad_cap, int stage_keys) {
+    extern __shared__ __align__(16) uint32_t ms_smem[];
     const int i0 = blockIdx.x * per;                 // this CTA's Gaussians: [i0, min(P, i0 + per)), per <= 4096
     const int i1 = min(P, i0 + per);
     uint32_t* my_hist = block_hist + (size_t)blockIdx.x * ntiles;   // written by count, re-read by scatter
-    uint4 rd[GSR_MS_ITEMS];
-#pragma unroll
-    for (int u = 0; u < GSR_MS_ITEMS; ++u) {
-        const int i = i0 + u * 1024 + threadIdx.x;
-        rd[u] = (i < i1) ? __ldg(rectdepth + i) : make_uint4(0u, 0u, 0u, 0u);
-    }
     if constexpr (!SCATTER) {
+        uint4 rd[GSR_MS_ITEMS];
+#pragma unroll
+        for (int u = 0; u < GSR_MS_ITEMS; ++u) {
+            const int i = i0 + u * 1024 + threadIdx.x;
+            rd[u] = (i < i1) ? __ldg(rectdepth + i) : make_uint4(0u, 0u, 0u, 0u);
+        }
+        uint32_t* hist = ms_smem;            // [ntiles] counts
         for (int t = threadIdx.x; t < ntiles; t += 1024) hist[t] = 0u;
         __syncthreads();
 #pragma unroll
@@ -292,28 +309,97 @@ multisplit_kernel(int P, int per, int gx, int ntiles, uint32_t max_pairs, const 
         for (int t = threadIdx.x; t < ntiles; t += 1024) {
             const uint32_t c = hist[t];
             my_hist[t] = c;
-            if (c) atomicAdd(tile_count + t, c);
+            if (c) { atomicAdd(tile_count + t, c); atomicAdd(pad_count + t, (c + 3u) & ~3u); }
         }
     } else {
-        // reserve this CTA's slice of every touched tile: the in-slice cursor starts at the slice's
-        // global position, so a pair's slot is ONE shared-memory atomic (no second lookup)
-        for (int t = threadIdx.x; t < ntiles; t += 1024) {
-            const uint32_t c = my_hist[t];
-            if (c) hist[t] = atomicAdd(tile_cursor + t, c);
+        __shared__ uint32_t warp_sums[32];
+        const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+        unsigned long long* stage = reinterpret_cast<unsigned long long*>(ms_smem);   // [stage_keys]
+        uint32_t* base = ms_smem + 2 * stage_keys;   // [ntiles] global start of this CTA's slice of each tile
+        uint32_t* pre = base + ntiles;               // [ntiles + 1] local offsets: exclusive prefix of the padded counts
+        uint32_t* cur = pre + ntiles + 1;            // [ntiles] staging cursors of the current band
+        for (int t = tid; t < ntiles; t += 1024) {
+            const uint32_t c = my_hist[t], pc = (c + 3u) & ~3u;
+            pre[t] = pc;
+            if (c) base[t] = atomicAdd(pad_cursor + t, pc);
         }
         __syncthreads();
+        {   // exclusive scan of pre[0, ntiles) in place: every thread owns `span` consecutive tiles
+            const int span = (ntiles + 1023) / 1024, t0 = min(ntiles, tid * span), t1 = min(ntiles, t0 + span);
+            uint32_t sum = 0;
+            for (int t = t0; t < t1; ++t) sum += pre[t];
+            uint32_t incl = sum;
 #pragma unroll
-        for (int u = 0; u < GSR_MS_ITEMS; ++u) {
-            if (rd[u].w) {
-                const int i = i0 + u * 1024 + threadIdx.x;
-                const int minx = rd[u].x & 0xffff, miny = rd[u].x >> 16, maxx = rd[u].y & 0xffff, maxy = rd[u].y >> 16;
-                const unsigned long long key = ((unsigned long long)rd[u].z << 32) | (uint32_t)i;
-                for (int ty = miny; ty < maxy; ++ty)
-                    for (int tx = minx; tx < maxx; ++tx) {
-                        const uint32_t pos = atomicAdd(&hist[ty * gx + tx], 1u);
-                        if (pos < max_pairs) keys[pos] = key;
-                    }
+            for (int o = 1; o < 32; o <<= 1) {
+                const uint32_t n = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += n;
             }
+            if (lane == 31) warp_sums[wid] = incl;
+            __syncthreads();
+            if (wid == 0) {
+                const uint32_t w = warp_sums[lane];
+                uint32_t wi = w;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const uint32_t n = __shfl_up_sync(0xffffffffu, wi, o);
+                    if (lane >= o) wi += n;
+                }
+                warp_sums[lane] = wi - w;
+                if (lane == 31) pre[ntiles] = wi;
+            }
+            __syncthreads();
+            uint32_t run = warp_sums[wid] + incl - sum;
+            for (int t = t0; t < t1; ++t) { const uint32_t pc = pre[t]; pre[t] = run; run += pc; }
+            __syncthreads();
+        }
+        // bands of tiles [tb, te) whose padded slices fit the staging buffer (a slice holds at most
+        // round_up(per, 4) <= 4096 <= stage_keys keys, so every band holds at least one tile)
+        for (int tb = 0; tb < ntiles;) {
+            const uint32_t b0 = pre[tb];
+            int lo = tb + 1, hi = ntiles;            // te = the largest tile boundary with pre[te] - b0 <= stage_keys
+            while (lo < hi) {
+                const int mid = (lo + hi + 1) >> 1;
+                if (pre[mid] - b0 <= (uint32_t)stage_keys) lo = mid; else hi = mid - 1;
+            }
+            const int te = lo;
+            const int nkeys = (int)(pre[te] - b0);   // a multiple of 4
+            for (int t = tb + tid; t < te; t += 1024) cur[t] = pre[t] - b0;
+            for (int q = tid; q < nkeys / 2; q += 1024)
+                reinterpret_cast<uint4*>(stage)[q] = make_uint4(~0u, ~0u, ~0u, ~0u);
+            __syncthreads();
+            const int rb = tb / gx, re = (te - 1) / gx + 1;   // tile rows the band touches
+            // the rectangles are re-read per band (L2) rather than held in registers across the bands
+            uint4 rd[GSR_MS_ITEMS];
+#pragma unroll
+            for (int u = 0; u < GSR_MS_ITEMS; ++u) {
+                const int i = i0 + u * 1024 + tid;
+                rd[u] = (i < i1) ? __ldg(rectdepth + i) : make_uint4(0u, 0u, 0u, 0u);
+            }
+#pragma unroll
+            for (int u = 0; u < GSR_MS_ITEMS; ++u) {   // an empty rectangle (w == 0) walks no tile
+                const int minx = rd[u].x & 0xffff, miny = rd[u].x >> 16, maxx = rd[u].y & 0xffff, maxy = rd[u].y >> 16;
+                const unsigned long long key = ((unsigned long long)rd[u].z << 32) | (uint32_t)(i0 + u * 1024 + tid);
+                for (int ty = max(miny, rb); ty < min(maxy, re); ++ty) {
+                    const int t1 = min(ty * gx + maxx, te);
+                    for (int t = max(ty * gx + minx, tb); t < t1; ++t) stage[atomicAdd(&cur[t], 1u)] = key;
+                }
+            }
+            __syncthreads();
+            // copy out: 16 B (two keys) per thread; the band position q2 = 2q lies in the slice of the last tile t
+            // of the band with pre[t] - b0 <= q2 (empty tiles before it share its offset)
+            for (int q = tid; q < nkeys / 2; q += 1024) {
+                const uint32_t p = b0 + 2u * (uint32_t)q;
+                int a = tb, z = te - 1;
+                while (a < z) {
+                    const int mid = (a + z + 1) >> 1;
+                    if (pre[mid] <= p) a = mid; else z = mid - 1;
+                }
+                const uint32_t dst = base[a] + (p - pre[a]);
+                if (dst + 2u <= pad_cap)
+                    *reinterpret_cast<uint4*>(pad_keys + dst) = reinterpret_cast<const uint4*>(stage)[q];
+            }
+            __syncthreads();
+            tb = te;
         }
     }
 }
@@ -447,8 +533,8 @@ __device__ __forceinline__ void radix_sort_smem(unsigned long long* s, uint32_t*
 }
 
 // ---------------------------------------------------------------------------------------------
-// Fast path: one-pass interpolation bucket sort.  The keys are read from global memory straight into
-// registers (g[0..n), coalesced); depth bits are mapped monotonically onto NB buckets between the
+// Fast path: one-pass interpolation bucket sort.  The keys are read from s[0..n) (gathered there by
+// gather_keys) into registers; depth bits are mapped monotonically onto NB buckets between the
 // list's min and max; a shared-memory atomic hands every key its arrival slot inside the bucket and
 // the keys are scattered bucket by bucket into s.  Every key then counts the smaller FULL 64-bit
 // keys of its own (tiny) bucket - one thread per key, no dependent read-modify-write chains - which
@@ -459,8 +545,8 @@ __device__ __forceinline__ void radix_sort_smem(unsigned long long* s, uint32_t*
 constexpr int kBucketLimit = 32;
 
 template <int NT, int ITEMS, int NB>
-__device__ __forceinline__ void tile_sort_items(const unsigned long long* g, unsigned long long* s, uint32_t* hist,
-                                               uint32_t* digit_base, uint32_t* red, int n) {
+__device__ __forceinline__ void tile_sort_items(unsigned long long* s, uint32_t* hist, uint32_t* digit_base,
+                                               uint32_t* red, int n) {
     static_assert(NB + 1 <= (NT / 32) * 256 + 32, "bucket counters alias the radix histogram (+32 spare words)");
     static_assert(NB % NT == 0, "whole number of buckets per thread");
     static_assert(NT / 32 <= 32 && ITEMS % 2 == 0, "one lane per warp total; positions are packed in pairs");
@@ -474,7 +560,7 @@ __device__ __forceinline__ void tile_sort_items(const unsigned long long* g, uns
         const int e = j * NT + tid;
         k[j] = ~0ull;
         if (e < n) {
-            k[j] = __ldcg(g + e);                 // L2: the multi-chunk caller rewrites g between calls
+            k[j] = s[e];
             dmin = min(dmin, (uint32_t)(k[j] >> 32)); dmax = max(dmax, (uint32_t)(k[j] >> 32));
         }
     }
@@ -578,12 +664,54 @@ __device__ __forceinline__ void tile_sort_items(const unsigned long long* g, uns
 // n <= NT * 16 keys; the per-thread item count is a compile-time constant of each instantiation, so
 // short lists do not walk (predicated-off) rows they do not have.  The branch is CTA-uniform.
 template <int NT, int NB>
-__device__ __forceinline__ void tile_sort_smem(const unsigned long long* g, unsigned long long* s, uint32_t* hist,
-                                               uint32_t* digit_base, uint32_t* red, int n) {
-    if (n <= NT * 4) tile_sort_items<NT, 4, NB>(g, s, hist, digit_base, red, n);
-    else if (n <= NT * 8) tile_sort_items<NT, 8, NB>(g, s, hist, digit_base, red, n);
-    else if (n <= NT * 12) tile_sort_items<NT, 12, NB>(g, s, hist, digit_base, red, n);
-    else tile_sort_items<NT, 16, NB>(g, s, hist, digit_base, red, n);
+__device__ __forceinline__ void tile_sort_smem(unsigned long long* s, uint32_t* hist, uint32_t* digit_base,
+                                               uint32_t* red, int n) {
+    if (n <= NT * 4) tile_sort_items<NT, 4, NB>(s, hist, digit_base, red, n);
+    else if (n <= NT * 8) tile_sort_items<NT, 8, NB>(s, hist, digit_base, red, n);
+    else if (n <= NT * 12) tile_sort_items<NT, 12, NB>(s, hist, digit_base, red, n);
+    else tile_sort_items<NT, 16, NB>(s, hist, digit_base, red, n);
+}
+
+// Copies the keys of in[0, n_in) that are not pad slots (~0ull: a real key's high word is a finite
+// float's bits) into s[0, n) and returns n, at most n_max.  They arrive in any order: the sort orders
+// them completely on (depth bits, index).  U keys per thread are loaded before any is placed; a warp
+// reserves the room for all of its keys of a round with one shared-memory atomic.
+template <int NT, int U>
+__device__ __forceinline__ int gather_keys(const unsigned long long* in, int n_in, int n_max, unsigned long long* s,
+                                           uint32_t* cnt) {
+    const int lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) *cnt = 0u;
+    __syncthreads();
+    for (int b = 0; b < n_in; b += NT * U) {
+        unsigned long long k[U];
+        uint32_t mine = 0u;
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            const int e = b + u * NT + (int)threadIdx.x;
+            k[u] = e < n_in ? __ldcg(in + e) : ~0ull;
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u) mine += k[u] != ~0ull ? 1u : 0u;
+        uint32_t incl = mine;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += v;
+        }
+        uint32_t pos = 0u;
+        if (lane == 31 && incl) pos = atomicAdd(cnt, incl);
+        pos = __shfl_sync(0xffffffffu, pos, 31) + incl - mine;
+#pragma unroll
+        for (int u = 0; u < U; ++u)
+            if (k[u] != ~0ull) {
+                if (pos < (uint32_t)n_max) s[pos] = k[u];
+                ++pos;
+            }
+    }
+    __syncthreads();
+    const int n = min((int)*cnt, n_max);
+    __syncthreads();
+    return n;
 }
 
 __device__ __forceinline__ int next_pow2(int n) {
@@ -603,10 +731,15 @@ struct SortSmemBig {
     uint32_t red[4];
 };
 
+// Both sort kernels read tile t's keys from in_keys[in_start[t], in_start[t + 1]) (clipped to in_cap):
+// on the multisplit path the tile's padded segment, whose pad slots they drop, and on the large-grid
+// fallback the key list itself (in_keys == keys, in_start == tile_start).  They write the sorted list
+// to keys[tile_start[t], tile_start[t + 1]).
 // small tiles: n <= 4096, 256 threads x 16 items
 __global__ void __launch_bounds__(256, 4)
 sort_small_kernel(const uint32_t* __restrict__ header, const uint32_t* __restrict__ work_order,
-                  const uint32_t* __restrict__ tile_start, unsigned long long* __restrict__ keys) {
+                  const uint32_t* __restrict__ tile_start, const unsigned long long* in_keys,
+                  const uint32_t* __restrict__ in_start, uint32_t in_cap, unsigned long long* keys) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     SortSmemSmall& sm = *reinterpret_cast<SortSmemSmall*>(smem_raw);
     const uint32_t max_pairs = header[GSR_H_MAX_PAIRS];
@@ -617,18 +750,21 @@ sort_small_kernel(const uint32_t* __restrict__ header, const uint32_t* __restric
         if (end - beg > GSR_SORT_SMALL_MAX) continue;          // big kernel's job
         if (end > max_pairs) end = max_pairs;                  // overflow: stay in bounds
         if (beg >= end) continue;
-        const int n = (int)(end - beg);
-        tile_sort_smem<256, 2048>(keys + beg, sm.keys, sm.hist, sm.digit_base, sm.red, n);
+        const uint32_t ib = in_start[tile], ie = min(in_start[tile + 1], in_cap);
+        if (ib >= ie) continue;
+        const int n = gather_keys<256, 16>(in_keys + ib, (int)(ie - ib), (int)(end - beg), sm.keys, &sm.red[3]);
+        tile_sort_smem<256, 2048>(sm.keys, sm.hist, sm.digit_base, sm.red, n);
         for (int i = threadIdx.x; i < n; i += 256) keys[beg + i] = sm.keys[i];
         __syncthreads();
     }
 }
 
-// big tiles: 1024 threads x 8 items per 8192-key chunk; lists longer than one chunk are sorted
-// chunk by chunk (radix) and merged in place in global memory with bitonic merge steps.
+// big tiles: 1024 threads x 8 items per 8192-key chunk; lists longer than one chunk are gathered
+// into the output, sorted there chunk by chunk (radix) and merged in place with bitonic merge steps.
 __global__ void __launch_bounds__(1024)
 sort_big_kernel(const uint32_t* __restrict__ header, const uint32_t* __restrict__ work_order,
-                const uint32_t* __restrict__ tile_start, unsigned long long* __restrict__ keys) {
+                const uint32_t* __restrict__ tile_start, const unsigned long long* in_keys,
+                const uint32_t* __restrict__ in_start, uint32_t in_cap, unsigned long long* keys) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     SortSmemBig& sm = *reinterpret_cast<SortSmemBig*>(smem_raw);
     unsigned long long* sb = sm.keys;
@@ -641,19 +777,36 @@ sort_big_kernel(const uint32_t* __restrict__ header, const uint32_t* __restrict_
         if (end - beg <= GSR_SORT_SMALL_MAX) continue;
         if (end > max_pairs) end = max_pairs;
         if (beg >= end) continue;
-        const int n = (int)(end - beg);
+        const uint32_t ib = in_start[tile], ie = min(in_start[tile + 1], in_cap);
+        if (ib >= ie) continue;
+        const unsigned long long* gin = in_keys + ib;
+        const int n_in = (int)(ie - ib);
+        int n = (int)(end - beg);
         unsigned long long* gk = keys + beg;
         if (n <= CH) {
-            tile_sort_smem<1024, 8192>(gk, sb, sm.hist, sm.digit_base, sm.red, n);
+            n = gather_keys<1024, 8>(gin, n_in, n, sb, &sm.red[3]);
+            tile_sort_smem<1024, 8192>(sb, sm.hist, sm.digit_base, sm.red, n);
             for (int i = threadIdx.x; i < n; i += 1024) gk[i] = sb[i];
             __syncthreads();
             continue;
         }
-        // ---- longer than one chunk: radix-sort CH-sized chunks, then bitonic merges ---------
+        // ---- longer than one chunk: gather into the output chunk by chunk (in place on the fallback path: a
+        // chunk is read whole before its keys are written, never past it) --------------------------------------
+        int m_out = 0;
+        for (int c0 = 0; c0 < n_in; c0 += CH) {
+            const int m = gather_keys<1024, 8>(gin + c0, min(CH, n_in - c0), min(CH, n - m_out), sb, &sm.red[3]);
+            for (int i = threadIdx.x; i < m; i += 1024) __stcg(gk + m_out + i, sb[i]);
+            m_out += m;
+            __syncthreads();
+        }
+        n = m_out;
+        // ---- radix-sort CH-sized chunks, then bitonic merges ------------------------------------
         const int N = next_pow2(n);
         for (int c0 = 0; c0 < n; c0 += CH) {
             const int m = min(CH, n - c0);
-            tile_sort_items<1024, 16, 8192>(gk + c0, sb, sm.hist, sm.digit_base, sm.red, m);
+            for (int i = threadIdx.x; i < m; i += 1024) sb[i] = __ldcg(gk + c0 + i);
+            __syncthreads();
+            tile_sort_items<1024, 16, 8192>(sb, sm.hist, sm.digit_base, sm.red, m);
             for (int i = threadIdx.x; i < m; i += 1024) __stcg(gk + c0 + i, sb[i]);
             __syncthreads();
         }
@@ -704,24 +857,46 @@ sort_big_kernel(const uint32_t* __restrict__ header, const uint32_t* __restrict_
     }
 }
 
+// On the multisplit path only the first of the GSR_COPIES counter and cursor arrays is a pair count /
+// cursor; the second counter array holds the padded counts, and the cursor arrays hold the scatter's
+// padded cursors, then the padded segment starts [ntiles + 1].
 struct BinPtrs {
     GsrTileGrid grid;
     uint32_t *header, *tile_start, *work_order, *tile_count, *tile_cursor;
-    unsigned long long* keys;
+    uint32_t *pad_count, *pad_cursor, *pad_start;
+    unsigned long long *keys, *pad_keys;
+    uint32_t pad_cap;
     const uint4* rectdepth;
 };
 BinPtrs bin_ptrs(const GsrFwdArgs& a) {
     BinPtrs b;
     b.grid = gsr_grid(a.prm.image_height, a.prm.image_width);
     if (a.num_views > 1) { b.grid.gy = a.num_views * a.gy_view; b.grid.ntiles = b.grid.gx * b.grid.gy; }
+    const int P = a.num_views * a.P_view;     // virtual Gaussians (view-major)
     b.header = reinterpret_cast<uint32_t*>(a.saved + a.vl.header);
     b.tile_start = reinterpret_cast<uint32_t*>(a.saved + a.vl.tile_start);
     b.work_order = reinterpret_cast<uint32_t*>(a.saved + a.vl.work_order);
     b.tile_count = reinterpret_cast<uint32_t*>(a.scratch + a.sl.tile_count);
     b.tile_cursor = reinterpret_cast<uint32_t*>(a.scratch + a.sl.tile_cursor);
+    b.pad_count = b.tile_count + b.grid.ntiles;
+    b.pad_cursor = b.tile_cursor;
+    b.pad_start = b.tile_cursor + b.grid.ntiles;
     b.keys = reinterpret_cast<unsigned long long*>(a.saved + a.vl.keys);
+    b.pad_keys = reinterpret_cast<unsigned long long*>(a.scratch + gsr_pad_keys_offset(a.sl, P, b.grid.ntiles));
+    b.pad_cap = gsr_pad_key_capacity(a.max_pairs, P, b.grid.ntiles);
     b.rectdepth = reinterpret_cast<const uint4*>(a.scratch + a.sl.rectdepth);
     return b;
+}
+
+// Keys the scatter stages per band: as many as keep its shared memory within kScatterSmem (two CTAs per SM
+// on H100), and never fewer than one slice can hold (round_up(4096 Gaussians, 4)).
+constexpr int kScatterSmem = 112 * 1024;
+int scatter_stage_keys(int ntiles) {
+    const int fixed = (3 * ntiles + 1) * (int)sizeof(uint32_t);
+    return max(1024 * GSR_MS_ITEMS, ((kScatterSmem - fixed) / (int)sizeof(unsigned long long)) & ~3);
+}
+int scatter_smem(int ntiles) {
+    return scatter_stage_keys(ntiles) * (int)sizeof(unsigned long long) + (3 * ntiles + 1) * (int)sizeof(uint32_t);
 }
 }  // namespace
 
@@ -732,13 +907,12 @@ cudaError_t gsr_launch_scan(const GsrFwdArgs& a) {
         static std::atomic<unsigned long long> attr_done{0};
         cudaError_t e = gsr_smem_once(scan_order_fast_kernel, GSR_MS_MAX_TILES * (int)sizeof(uint32_t), attr_done);
         if (e != cudaSuccess) return e;
-        scan_order_fast_kernel<<<1, 1024, b.grid.ntiles * sizeof(uint32_t), a.stream>>>(b.grid.ntiles, a.max_pairs, b.tile_count, b.tile_start,
-                                                          b.tile_cursor, b.work_order, b.header, a.host_notify,
-                                                          a.notify_seq);
+        scan_order_fast_kernel<<<1, 1024, b.grid.ntiles * sizeof(uint32_t), a.stream>>>(
+            b.grid.ntiles, a.max_pairs, b.tile_count, b.pad_count, b.tile_start, b.pad_start, b.pad_cursor,
+            b.work_order, b.header, a.host_notify, a.notify_seq);
         return cudaGetLastError();
     }
-    scan_order_kernel<<<1, 1024, 0, a.stream>>>(b.grid.ntiles, gsr_use_multisplit(b.grid.ntiles) ? 1 : GSR_COPIES,
-                                                 a.max_pairs, b.tile_count, b.tile_start,
+    scan_order_kernel<<<1, 1024, 0, a.stream>>>(b.grid.ntiles, GSR_COPIES, a.max_pairs, b.tile_count, b.tile_start,
                                                  b.tile_cursor, b.work_order, b.header, a.host_notify,
                                                  a.notify_seq);
     return cudaGetLastError();
@@ -749,20 +923,21 @@ static cudaError_t launch_multisplit(const GsrFwdArgs& a, const BinPtrs& b, bool
     if (P == 0) return cudaSuccess;
     const int nblk = gsr_ms_blocks(P);
     const int per = (P + nblk - 1) / nblk;
-    const int smem = b.grid.ntiles * (int)sizeof(uint32_t);
-    const int smem_max = GSR_MS_MAX_TILES * (int)sizeof(uint32_t);
+    uint32_t* ms_hist = reinterpret_cast<uint32_t*>(a.scratch + a.sl.ms_hist);
     static std::atomic<unsigned long long> done_scatter{0}, done_count{0};
-    cudaError_t e = scatter ? gsr_smem_once(multisplit_kernel<true>, smem_max, done_scatter)
-                            : gsr_smem_once(multisplit_kernel<false>, smem_max, done_count);
-    if (e != cudaSuccess) return e;
-    if (scatter)
-        multisplit_kernel<true><<<nblk, 1024, smem, a.stream>>>(
-            P, per, b.grid.gx, b.grid.ntiles, a.max_pairs, b.rectdepth, b.tile_count, b.tile_cursor,
-            reinterpret_cast<uint32_t*>(a.scratch + a.sl.ms_hist), b.keys);
-    else
-        multisplit_kernel<false><<<nblk, 1024, smem, a.stream>>>(
-            P, per, b.grid.gx, b.grid.ntiles, a.max_pairs, b.rectdepth, b.tile_count, b.tile_cursor,
-            reinterpret_cast<uint32_t*>(a.scratch + a.sl.ms_hist), b.keys);
+    if (scatter) {
+        cudaError_t e = gsr_smem_once(multisplit_kernel<true>, scatter_smem(GSR_MS_MAX_TILES), done_scatter);
+        if (e != cudaSuccess) return e;
+        multisplit_kernel<true><<<nblk, 1024, scatter_smem(b.grid.ntiles), a.stream>>>(
+            P, per, b.grid.gx, b.grid.ntiles, b.rectdepth, b.tile_count, b.pad_count, b.pad_cursor, ms_hist,
+            b.pad_keys, b.pad_cap, scatter_stage_keys(b.grid.ntiles));
+    } else {
+        cudaError_t e = gsr_smem_once(multisplit_kernel<false>, GSR_MS_MAX_TILES * (int)sizeof(uint32_t), done_count);
+        if (e != cudaSuccess) return e;
+        multisplit_kernel<false><<<nblk, 1024, b.grid.ntiles * (int)sizeof(uint32_t), a.stream>>>(
+            P, per, b.grid.gx, b.grid.ntiles, b.rectdepth, b.tile_count, b.pad_count, b.pad_cursor, ms_hist,
+            b.pad_keys, b.pad_cap, 0);
+    }
     return cudaGetLastError();
 }
 
@@ -788,6 +963,10 @@ cudaError_t gsr_launch_scatter(const GsrFwdArgs& a) {
 // small-tile kernel runs there concurrently with the big-tile kernel (joined before returning).
 cudaError_t gsr_launch_sort(const GsrFwdArgs& a, cudaStream_t side, cudaEvent_t fork, cudaEvent_t join) {
     const BinPtrs b = bin_ptrs(a);
+    const bool ms = gsr_use_multisplit(b.grid.ntiles);   // padded segments in scratch; the fallback sorts in place
+    const unsigned long long* in_keys = ms ? b.pad_keys : b.keys;
+    const uint32_t* in_start = ms ? b.pad_start : b.tile_start;
+    const uint32_t in_cap = ms ? b.pad_cap : a.max_pairs;
     const int big_smem = (int)sizeof(SortSmemBig), small_smem = (int)sizeof(SortSmemSmall);
     static std::atomic<unsigned long long> done_big{0}, done_small{0};
     cudaError_t e = gsr_smem_once(sort_big_kernel, big_smem, done_big);
@@ -803,8 +982,10 @@ cudaError_t gsr_launch_sort(const GsrFwdArgs& a, cudaStream_t side, cudaEvent_t 
         if ((e = cudaStreamWaitEvent(side, fork, 0)) != cudaSuccess) return e;
         s_small = side;
     }
-    sort_big_kernel<<<big_grid, 1024, big_smem, a.stream>>>(b.header, b.work_order, b.tile_start, b.keys);
-    sort_small_kernel<<<small_grid, 256, small_smem, s_small>>>(b.header, b.work_order, b.tile_start, b.keys);
+    sort_big_kernel<<<big_grid, 1024, big_smem, a.stream>>>(b.header, b.work_order, b.tile_start, in_keys, in_start,
+                                                            in_cap, b.keys);
+    sort_small_kernel<<<small_grid, 256, small_smem, s_small>>>(b.header, b.work_order, b.tile_start, in_keys, in_start,
+                                                                in_cap, b.keys);
     if (side != nullptr) {
         if ((e = cudaEventRecord(join, side)) != cudaSuccess) return e;
         if ((e = cudaStreamWaitEvent(a.stream, join, 0)) != cudaSuccess) return e;

@@ -99,10 +99,22 @@ __host__ __device__ inline int gsr_ms_blocks(long long P) {
 #define GSR_MS_MAX_TILES 12288   // 4 B x tiles of dynamic smem (48 KB); 12 tiles per thread in the scan kernel
 __host__ __device__ inline bool gsr_use_multisplit(int ntiles) { return ntiles <= GSR_MS_MAX_TILES; }
 // uint32 words at the start of scratch that must be zero before the count kernel runs: the queue counters and the
-// per-tile pair counters (one array on the multisplit path, all GSR_COPIES on the large-grid fallback).  The
-// multisplit projection zeroes them in its prologue; otherwise the forward issues a memset.  Host code only.
+// per-tile pair counters (on the multisplit path two arrays, the pair counts and the padded counts; all GSR_COPIES on
+// the large-grid fallback).  The multisplit projection zeroes them in its prologue; otherwise the forward issues a
+// memset.  Host code only.
 inline size_t gsr_counter_words(const b200gsr_scratch_layout& sl, int ntiles) {
-    return (gsr_use_multisplit(ntiles) ? sl.tile_count + (size_t)ntiles * sizeof(uint32_t) : sl.tile_cursor) / sizeof(uint32_t);
+    return (gsr_use_multisplit(ntiles) ? sl.tile_count + 2 * (size_t)ntiles * sizeof(uint32_t) : sl.tile_cursor) / sizeof(uint32_t);
+}
+// Multisplit path: the key scatter writes every CTA's slice of a tile rounded up to whole 32-byte sectors (4 keys, the
+// pad slots hold ~0ull) into a padded key buffer at the end of scratch, and the tile sort compacts each tile's padded
+// segment into saved.keys.  A slice has at most 3 pad keys, so the buffer holds max_pairs + 3 * CTAs * tiles keys
+// (capped so that a padded position fits in 32 bits).  P = virtual Gaussians.  Host code only.
+inline uint32_t gsr_pad_key_capacity(uint64_t max_pairs, int P, int ntiles) {
+    const uint64_t cap = max_pairs + 3ull * (uint64_t)gsr_ms_blocks(P) * (uint64_t)ntiles;
+    return (uint32_t)(cap < 0xfffffff0ull ? cap : 0xfffffff0ull);
+}
+inline size_t gsr_pad_keys_offset(const b200gsr_scratch_layout& sl, int P, int ntiles) {
+    return (sl.ms_hist + (size_t)gsr_ms_blocks(P) * ntiles * sizeof(uint32_t) + 255) / 256 * 256;
 }
 
 // ---- deterministic mode (B200GSR_FWD_DETERMINISTIC / B200GSR_BWD_DETERMINISTIC) ------------------------

@@ -96,7 +96,8 @@ typedef struct b200gsr_scratch_layout {
     size_t tile_count;    /* uint32[16][num_tiles] privatised per-tile pair counters */
     size_t tile_cursor;   /* uint32[16][num_tiles] write cursors */
     size_t rectdepth;     /* uint4[P]: (minx|miny<<16, maxx|maxy<<16, depth bits, tiles touched) */
-    size_t ms_hist;       /* uint32[num_CTAs(P)][num_tiles] per-CTA tile histograms (multisplit binning) */
+    size_t ms_hist;       /* uint32[num_CTAs(P)][num_tiles] per-CTA tile histograms (multisplit binning), followed
+                             inside `total` by the binning's padded key buffer */
     size_t total;
 } b200gsr_scratch_layout;
 
