@@ -1,6 +1,6 @@
 """ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h,
 include/b200gsr_loss.h, include/b200gsr_frozen.h, include/b200gsr_stats.h,
-include/b200gsr_reserve.h).  Fails loudly if the library is missing:
+include/b200gsr_reserve.h, include/b200gsr_frames.h).  Fails loudly if the library is missing:
 there is NO CPU or PyTorch fallback in the product path."""
 from __future__ import annotations
 
@@ -183,6 +183,12 @@ RESERVE_SIGNATURES = {
     "b200gsr_adam_step_dyn_live": (C.c_int, [i32, _P(AdamTensor), vp, _P(AdamLive), vp]),
 }
 
+# The video-frame entry point of include/b200gsr_frames.h (same library).
+FRAMES_SIGNATURES = {
+    "b200gsr_frames": (C.c_int, [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp]),
+}
+FRAMES_STATS_BYTES = 32             # B200GSR_FRAMES_STATS_BYTES: scratch per view of b200gsr_frames
+
 _lib = None
 ABI_VERSION = 3
 ERR_BAD_ARG = -1
@@ -212,7 +218,8 @@ def load():
                 "`python -m dreamscene_b200._build` (needs nvcc; sm_90a only). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES, **STEP_SIGNATURES, **LOSS_SIGNATURES,
-                                      **FROZEN_SIGNATURES, **STATS_SIGNATURES, **RESERVE_SIGNATURES}.items():
+                                      **FROZEN_SIGNATURES, **STATS_SIGNATURES, **RESERVE_SIGNATURES,
+                                      **FRAMES_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:

@@ -6,6 +6,7 @@
 #include "../../include/b200gsr_frozen.h"
 #include "../../include/b200gsr_stats.h"
 #include "../../include/b200gsr_reserve.h"
+#include "../../include/b200gsr_frames.h"
 
 #include <cstdarg>
 #include <cstdio>
@@ -677,6 +678,24 @@ int b200gsr_disparity_backward_ex(int32_t B, int32_t N, const float* depth_alpha
 int b200gsr_disparity_backward(int32_t B, int32_t N, const float* depth_alpha, const float* focal, const float* g_disp,
                                const float* g_alpha, void* stats, float* d_depth_alpha, void* stream) {
     return b200gsr_disparity_backward_ex(B, N, depth_alpha, focal, g_disp, g_alpha, stats, d_depth_alpha, 0u, stream);
+}
+
+int b200gsr_frames(int32_t B, int32_t H, int32_t W, const float* color, const float* depth_alpha, const float* focal,
+                   uint8_t* rgb8, uint8_t* depth8, void* stats, void* stream) {
+    if (B < 1 || B > B200GSR_MAX_VIEWS) return fail(B200GSR_ERR_BAD_ARG, "frames: B = %d not in 1..%d", B, B200GSR_MAX_VIEWS);
+    if (H < 1 || W < 1) return fail(B200GSR_ERR_BAD_ARG, "frames: image size %d x %d must be positive", W, H);
+    if (!color || !depth_alpha || !focal || !rgb8 || !depth8 || !stats)
+        return fail(B200GSR_ERR_BAD_ARG, "frames: null pointer");
+    if ((reinterpret_cast<uintptr_t>(rgb8) | reinterpret_cast<uintptr_t>(depth8)) & 3u)
+        return fail(B200GSR_ERR_BAD_ARG, "frames: rgb8 and depth8 must be 4-byte aligned");
+    // the forwards' composite addresses a single view with its own height (unpadded), B > 1 views stacked
+    const long long Hs = B == 1 ? H : (long long)B * gsr_grid(H, W).gy * GSR_TILE;
+    if ((long long)B * H * W * 3 >= (1ll << 31) || Hs * W * 3 >= (1ll << 31))
+        return fail(B200GSR_ERR_BAD_ARG, "frames: %d views of %d x %d are too large", B, W, H);
+    DeviceState* ds = device_state();
+    if (!ds) return fail(B200GSR_ERR_CUDA, "cannot query the current CUDA device");
+    return check_cuda(gsr_launch_frames(B, H, W, (int)Hs, color, depth_alpha, focal, rgb8, depth8, stats, ds->num_sms,
+                                        static_cast<cudaStream_t>(stream)), "frames");
 }
 
 #define GSR_ST(x) static_cast<cudaStream_t>(x)

@@ -346,6 +346,9 @@ cudaError_t gsr_launch_disparity_fwd(int B, int N, const float* da, const float*
 cudaError_t gsr_launch_disparity_bwd(int B, int N, const float* da, const float* focal, const float* g_out,
                                      const float* g_alpha, void* stats, float* d_da, bool deterministic, int num_sms,
                                      cudaStream_t s);
+// 8-bit video frames of B stacked views (postprocess.cu; b200gsr_frames)
+cudaError_t gsr_launch_frames(int B, int H, int W, int Hs, const float* color, const float* da, const float* focal,
+                              uint8_t* rgb8, uint8_t* depth8, void* stats, int num_sms, cudaStream_t s);
 
 // densification / pruning (densify.cu)
 cudaError_t gsr_densify_stats(int P, const float* vs_grad, const int32_t* radii, float* accum, float* denom,

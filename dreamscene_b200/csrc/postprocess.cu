@@ -10,6 +10,7 @@
 // (evenly distributed over ties, as torch.min()/max() do) and through the clamp (pass-through on
 // the closed interval).
 #include "common.cuh"
+#include "../../include/b200gsr_frames.h"
 
 namespace {
 
@@ -26,6 +27,7 @@ struct DispStats {
     unsigned int ties_min, ties_max;
 };
 static_assert(sizeof(DispStats) == 32, "stats record is 8 words");
+static_assert(sizeof(DispStats) == B200GSR_FRAMES_STATS_BYTES, "b200gsr_frames' scratch is one record per view");
 
 __global__ void disp_init_kernel(DispStats* st, int B) {
     const int v = blockIdx.x * blockDim.x + threadIdx.x;
@@ -39,13 +41,9 @@ __device__ __forceinline__ float disp_raw(float depth, float alpha, float focal)
     return __fdiv_rn(focal, __fadd_rn(__fadd_rn(depth, __fmul_rn(alpha, 10.0f)), 1e-5f));
 }
 
-// depth_alpha: [B][2][N]; grid (blocks, B)
-__global__ void __launch_bounds__(256)
-disp_reduce_kernel(const float* __restrict__ da, const float* __restrict__ focal, int N, DispStats* st) {
-    const int v = blockIdx.y;
-    const float* depth = da + (size_t)v * 2 * N;
-    const float* alpha = depth + N;
-    const float f = focal[v];
+// One block's share of view v's statistics over its N contiguous depth and alpha values (blockDim 256, grid x strided)
+__device__ __forceinline__ void disp_reduce_view(const float* __restrict__ depth, const float* __restrict__ alpha,
+                                                 const float f, int N, DispStats* st, int v) {
     unsigned int mm = 0x7f800000u, ma = 0x7f800000u, mx = 0u, nm = 0u;
     for (int i = blockIdx.x * 256 + threadIdx.x; i < N; i += gridDim.x * 256) {
         const float a = alpha[i];
@@ -61,9 +59,22 @@ disp_reduce_kernel(const float* __restrict__ da, const float* __restrict__ focal
     }
 }
 
+// depth_alpha: [B][2][N]; grid (blocks, B)
+__global__ void __launch_bounds__(256)
+disp_reduce_kernel(const float* __restrict__ da, const float* __restrict__ focal, int N, DispStats* st) {
+    const int v = blockIdx.y;
+    const float* depth = da + (size_t)v * 2 * N;
+    disp_reduce_view(depth, depth + N, focal[v], N, st, v);
+}
+
 __device__ __forceinline__ void disp_bounds(const DispStats& s, float& m, float& M) {
     m = __uint_as_float(s.n_masked > 0 ? s.min_masked : s.min_all);
     M = __uint_as_float(s.max_all);
+}
+
+__device__ __forceinline__ float disp_norm(float d, float m, float den) {
+    const float t = __fdiv_rn(__fsub_rn(d, m), den);
+    return fminf(fmaxf(t, 0.0f), 1.0f);       // NaN (den == 0) propagates like torch.clamp
 }
 
 __global__ void __launch_bounds__(256)
@@ -78,8 +89,80 @@ disp_normalise_kernel(const float* __restrict__ da, const float* __restrict__ fo
     const float den = __fsub_rn(M, m);
     for (int i = blockIdx.x * 256 + threadIdx.x; i < N; i += gridDim.x * 256) {
         const float d = disp_raw(depth[i], alpha[i], f);
-        const float t = __fdiv_rn(__fsub_rn(d, m), den);
-        out[(size_t)v * N + i] = fminf(fmaxf(t, 0.0f), 1.0f);       // NaN (den == 0) propagates like torch.clamp
+        out[(size_t)v * N + i] = disp_norm(d, m, den);
+    }
+}
+
+// ---- 8-bit video frames (b200gsr_frames).  The views come straight from a stacked forward's outputs, color
+// [3][Hs][W] and depth_alpha [2][Hs][W]: view v's H*W pixels are contiguous from row v*Hp (Hp = Hs / B), so its
+// pixel i of channel c is at c*Hs*W + v*Hp*W + i.  The reference quantises a frame as
+//     rgb   = (clamp(color, 0, 1) * 255).round().astype(uint8)                         (float32, round half even)
+//     depth = (clamp(disp / disp.max(), 0, 1) * 255).round().astype(uint8)    disp = disp_normalise_kernel's value
+// where the cast of a NaN is undefined in numpy; here a NaN becomes 0 (fmaxf returns the non-NaN operand).
+
+// the statistics of disp_reduce_kernel over the stacked layout; grid (blocks, B)
+__global__ void __launch_bounds__(256)
+frames_stats_kernel(const float* __restrict__ da, const float* __restrict__ focal, int HW, size_t view_stride,
+                    size_t chan_stride, DispStats* st) {
+    const int v = blockIdx.y;
+    const float* depth = da + v * view_stride;
+    disp_reduce_view(depth, depth + chan_stride, focal[v], HW, st, v);
+}
+
+__device__ __forceinline__ unsigned int quantise8(float x) {
+    return (unsigned int)rintf(__fmul_rn(fminf(fmaxf(x, 0.0f), 1.0f), 255.0f));
+}
+
+// One thread per 4 consecutive pixels of the B views (flattened view-major, as rgb8 [B,H,W,3] / depth8 [B,H,W,1]):
+// three 32-bit stores of packed RGB and one of depth.  The last B*H*W % 4 pixels are stored byte by byte.
+__global__ void __launch_bounds__(256)
+frames_kernel(int B, int HW, size_t view_stride, size_t chan_stride, const float* __restrict__ color,
+              const float* __restrict__ da, const float* __restrict__ focal, const DispStats* __restrict__ st,
+              uint8_t* __restrict__ rgb8, uint8_t* __restrict__ depth8) {
+    __shared__ float s_m[B200GSR_MAX_VIEWS], s_den[B200GSR_MAX_VIEWS], s_max[B200GSR_MAX_VIEWS], s_f[B200GSR_MAX_VIEWS];
+    if (threadIdx.x < B) {
+        const int v = threadIdx.x;
+        float m, M;
+        disp_bounds(st[v], m, M);
+        const float den = __fsub_rn(M, m);
+        s_m[v] = m; s_den[v] = den; s_f[v] = focal[v];
+        // max over the view of disp_norm(d): disp_norm is non-decreasing in d and M is attained, so it is
+        // disp_norm(M) - 1 for M > m, 0 when den is 0 or NaN (every pixel is then 0, and 0 / 0 quantises to 0)
+        s_max[v] = disp_norm(M, m, den);
+    }
+    __syncthreads();
+    const int total = B * HW;
+    for (int q = blockIdx.x * blockDim.x + threadIdx.x; 4 * q < total; q += gridDim.x * blockDim.x) {
+        const int p0 = 4 * q;
+        int v = p0 / HW, i = p0 - v * HW;
+        unsigned int rgb[4], dep[4];
+        const int n = min(4, total - p0);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            rgb[k] = dep[k] = 0u;
+            if (k < n) {
+                while (i >= HW) { i -= HW; ++v; }
+                const size_t o = v * view_stride + i;
+                rgb[k] = quantise8(color[o]) | quantise8(color[o + chan_stride]) << 8 |
+                         quantise8(color[o + 2 * chan_stride]) << 16;
+                const float t = disp_norm(disp_raw(da[o], da[o + chan_stride], s_f[v]), s_m[v], s_den[v]);
+                dep[k] = quantise8(__fdiv_rn(t, s_max[v]));
+                ++i;
+            }
+        }
+        if (n == 4) {
+            uint32_t* w = reinterpret_cast<uint32_t*>(rgb8 + 12 * (size_t)q);
+            w[0] = rgb[0] | rgb[1] << 24;
+            w[1] = rgb[1] >> 8 | rgb[2] << 16;
+            w[2] = rgb[2] >> 16 | rgb[3] << 8;
+            reinterpret_cast<uint32_t*>(depth8)[q] = dep[0] | dep[1] << 8 | dep[2] << 16 | dep[3] << 24;
+        } else {
+            for (int k = 0; k < n; ++k) {
+                uint8_t* px = rgb8 + 3 * (size_t)(p0 + k);
+                px[0] = (uint8_t)rgb[k]; px[1] = (uint8_t)(rgb[k] >> 8); px[2] = (uint8_t)(rgb[k] >> 16);
+                depth8[p0 + k] = (uint8_t)dep[k];
+            }
+        }
     }
 }
 
@@ -188,6 +271,20 @@ cudaError_t gsr_launch_disparity_fwd(int B, int N, const float* da, const float*
     const int bx = max(1, min((N + 255) / 256, (num_sms * 8 + B - 1) / B));
     disp_reduce_kernel<<<dim3(bx, B), 256, 0, s>>>(da, focal, N, st);
     disp_normalise_kernel<<<dim3(bx, B), 256, 0, s>>>(da, focal, N, st, out);
+    return cudaGetLastError();
+}
+
+cudaError_t gsr_launch_frames(int B, int H, int W, int Hs, const float* color, const float* da, const float* focal,
+                              uint8_t* rgb8, uint8_t* depth8, void* stats, int num_sms, cudaStream_t s) {
+    const int HW = H * W;
+    const size_t view_stride = (size_t)(Hs / B) * W, chan_stride = (size_t)Hs * W;
+    DispStats* st = static_cast<DispStats*>(stats);
+    disp_init_kernel<<<(B + 63) / 64, 64, 0, s>>>(st, B);
+    const int bx = max(1, min((HW + 255) / 256, (num_sms * 8 + B - 1) / B));
+    frames_stats_kernel<<<dim3(bx, B), 256, 0, s>>>(da, focal, HW, view_stride, chan_stride, st);
+    const int quads = (B * HW + 3) / 4;
+    frames_kernel<<<max(1, min((quads + 255) / 256, num_sms * 8)), 256, 0, s>>>(B, HW, view_stride, chan_stride, color,
+                                                                                 da, focal, st, rgb8, depth8);
     return cudaGetLastError();
 }
 

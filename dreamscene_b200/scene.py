@@ -180,6 +180,12 @@ def _scene_groups(groups: Sequence):
     return flat, M, P
 
 
+def _refuse_reserved(groups: Sequence):
+    if any(getattr(g, "_reserved_rows", False) for g in groups):
+        raise TypeError("render_scene: a ReservedGroup holds dead rows past its live count; render group.rows() (the "
+                        "live prefixes) eagerly, or replay it with StepGraph")
+
+
 def _check_device(flat):
     if any(t.device.type != "cuda" for t in flat):
         raise RuntimeError("render_scene (b200gsr): parameters must be CUDA tensors; there is no CPU fallback")
@@ -381,9 +387,7 @@ def render_scene(groups: Sequence, settings_list: Sequence, *, shs_aug=True, sca
     -> list of B (color[3,H,W], radii[P], depth_alpha[2,H,W]); with return_scales also the augmented scales
        [B,P,3] (differentiable, for the reference's scale loss).  Every trainable group's raw leaves get their
        gradients."""
-    if any(getattr(g, "_reserved_rows", False) for g in groups):
-        raise TypeError("render_scene: a ReservedGroup holds dead rows past its live count; render group.rows() (the "
-                        "live prefixes) eagerly, or replay it with StepGraph")
+    _refuse_reserved(groups)
     from . import parallel
     B, H, W = _check_settings(settings_list)
     shs_flags = _view_flags(shs_aug, B, "shs_aug")
