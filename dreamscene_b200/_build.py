@@ -12,11 +12,13 @@ LIB = os.path.join(HERE, "libb200gsr.so")
 SOURCES = ["api.cu", "project.cu", "binning.cu", "composite.cu", "knn.cu", "assemble.cu", "postprocess.cu", "densify.cu",
            "optim.cu", "loss.cu"]
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "scene_math.cuh"), os.path.join(CSRC, "project_bwd_body.cuh"),
+           os.path.join(CSRC, "assemble_body.cuh"),
            os.path.join(HERE, "..", "include", "b200gsr.h"), os.path.join(HERE, "..", "include", "b200gsr_scene.h"),
            os.path.join(HERE, "..", "include", "b200gsr_step.h"), os.path.join(HERE, "..", "include", "b200gsr_loss.h"),
            os.path.join(HERE, "..", "include", "b200gsr_frozen.h"), os.path.join(HERE, "..", "include", "b200gsr_stats.h"),
            os.path.join(HERE, "..", "include", "b200gsr_reserve.h"),
-           os.path.join(HERE, "..", "include", "b200gsr_frames.h")]
+           os.path.join(HERE, "..", "include", "b200gsr_frames.h"),
+           os.path.join(HERE, "..", "include", "b200gsr_views_frozen.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

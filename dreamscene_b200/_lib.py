@@ -1,6 +1,6 @@
 """ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h,
 include/b200gsr_loss.h, include/b200gsr_frozen.h, include/b200gsr_stats.h,
-include/b200gsr_reserve.h, include/b200gsr_frames.h).  Fails loudly if the library is missing:
+include/b200gsr_reserve.h, include/b200gsr_frames.h, include/b200gsr_views_frozen.h).  Fails loudly if the library is missing:
 there is NO CPU or PyTorch fallback in the product path."""
 from __future__ import annotations
 
@@ -189,6 +189,22 @@ FRAMES_SIGNATURES = {
 }
 FRAMES_STATS_BYTES = 32             # B200GSR_FRAMES_STATS_BYTES: scratch per view of b200gsr_frames
 
+
+class RowRange(C.Structure):        # == b200gsr_row_range (include/b200gsr_views_frozen.h)
+    _fields_ = [("lo", C.c_int32), ("len", C.c_int32)]
+
+
+# The frozen-row backwards of include/b200gsr_views_frozen.h (same library), in that header's order: the arguments of
+# b200gsr_backward_views_ex plus the host range array and its count before the stream; those of
+# b200gsr_assemble_backward plus the uint32 frozen_groups mask before the stream.
+VIEWS_FROZEN_SIGNATURES = {
+    "b200gsr_backward_views_frozen": (C.c_int, [i32, _P(Params), _P(ViewInputs)] + [vp] * 5 +
+                                      [sz, u64, _P(ViewGrads), u32, _P(RowRange), i32, vp]),
+    "b200gsr_assemble_backward_frozen": (C.c_int, [i32, _P(Group), _P(GroupGrad), i32, i32, f32, f32, vp, vp, u64] +
+                                         [vp] * 5 + [u32, vp]),
+}
+MAX_FROZEN_RANGES = 12              # B200GSR_MAX_FROZEN_RANGES
+
 _lib = None
 ABI_VERSION = 3
 ERR_BAD_ARG = -1
@@ -219,7 +235,7 @@ def load():
     lib = C.CDLL(LIB_PATH)
     for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES, **STEP_SIGNATURES, **LOSS_SIGNATURES,
                                       **FROZEN_SIGNATURES, **STATS_SIGNATURES, **RESERVE_SIGNATURES,
-                                      **FRAMES_SIGNATURES}.items():
+                                      **FRAMES_SIGNATURES, **VIEWS_FROZEN_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:

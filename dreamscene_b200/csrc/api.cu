@@ -7,6 +7,7 @@
 #include "../../include/b200gsr_stats.h"
 #include "../../include/b200gsr_reserve.h"
 #include "../../include/b200gsr_frames.h"
+#include "../../include/b200gsr_views_frozen.h"
 
 #include <cstdarg>
 #include <cstdio>
@@ -477,12 +478,12 @@ int b200gsr_forward_views(int32_t B, const b200gsr_params* prm, const b200gsr_vi
                        saved_bytes, max_pairs, flags, host_notify, notify_seq, stream);
 }
 
-int b200gsr_backward_views_ex(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, const int32_t* radii,
-                              const float* out_depth_alpha, const float* dL_dcolor, const float* dL_ddepth_alpha,
-                              void* saved, size_t saved_bytes, uint64_t max_pairs, const b200gsr_view_grads* out,
-                              uint32_t flags, void* stream) {
-    int rc = check_views(B, prm, in);
-    if (rc) return rc;
+// b200gsr_backward_views_ex (frozen = null) and b200gsr_backward_views_frozen with ranges (validated by the caller)
+static int backward_views(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, const int32_t* radii,
+                          const float* out_depth_alpha, const float* dL_dcolor, const float* dL_ddepth_alpha,
+                          void* saved, size_t saved_bytes, uint64_t max_pairs, const b200gsr_view_grads* out,
+                          uint32_t flags, const GsrFrozenRanges* frozen, void* stream) {
+    int rc;
     const int P = prm[0].P;
     if (P == 0) return B200GSR_OK;
     if (!radii || !out_depth_alpha || !dL_dcolor || !dL_ddepth_alpha || !saved || !out)
@@ -495,6 +496,7 @@ int b200gsr_backward_views_ex(int32_t B, const b200gsr_params* prm, const b200gs
         return rc;
     set_view_inputs(a, in[0]);
     a.g_begin = 0; a.g_end = P;
+    a.frozen_rows = frozen;
     GSR_RANGE_PUSH("b200gsr.views.composite_bwd");
     rc = check_cuda(gsr_launch_composite_bwd(a), "composite_bwd");
     GSR_RANGE_POP();
@@ -510,6 +512,52 @@ int b200gsr_backward_views_ex(int32_t B, const b200gsr_params* prm, const b200gs
     }
     GSR_RANGE_POP();
     return rc;
+}
+
+int b200gsr_backward_views_ex(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, const int32_t* radii,
+                              const float* out_depth_alpha, const float* dL_dcolor, const float* dL_ddepth_alpha,
+                              void* saved, size_t saved_bytes, uint64_t max_pairs, const b200gsr_view_grads* out,
+                              uint32_t flags, void* stream) {
+    int rc = check_views(B, prm, in);
+    if (rc) return rc;
+    return backward_views(B, prm, in, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes, max_pairs,
+                          out, flags, nullptr, stream);
+}
+
+int b200gsr_backward_views_frozen(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in,
+                                  const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
+                                  const float* dL_ddepth_alpha, void* saved, size_t saved_bytes, uint64_t max_pairs,
+                                  const b200gsr_view_grads* out, uint32_t flags, const b200gsr_row_range* frozen,
+                                  int32_t num_frozen, void* stream) {
+    int rc = check_views(B, prm, in);
+    if (rc) return rc;
+    if (num_frozen < 0) return fail(B200GSR_ERR_BAD_ARG, "num_frozen %d is negative", num_frozen);
+    if (num_frozen > 0 && !frozen) return fail(B200GSR_ERR_BAD_ARG, "frozen is null with num_frozen %d", num_frozen);
+    // sorted, non-overlapping, non-empty ranges inside [0, P); touching ones merge
+    GsrFrozenRanges fr{};
+    const long long P = prm[0].P;
+    long long end = 0;
+    for (int k = 0; k < num_frozen; ++k) {
+        const long long lo = frozen[k].lo, len = frozen[k].len;
+        if (len <= 0) return fail(B200GSR_ERR_BAD_ARG, "frozen range %d is empty (len %lld)", k, len);
+        if (lo < 0 || lo + len > P)
+            return fail(B200GSR_ERR_BAD_ARG, "frozen range %d [%lld, %lld) is outside [0, P = %lld)", k, lo, lo + len, P);
+        if (k > 0 && lo < end)
+            return fail(B200GSR_ERR_BAD_ARG, "frozen range %d starts at %lld, before the end %lld of range %d: ranges "
+                        "must be sorted and must not overlap", k, lo, end, k - 1);
+        if (fr.n > 0 && lo == end) {
+            fr.len[fr.n - 1] += (uint32_t)len;
+        } else {
+            if (fr.n == B200GSR_MAX_FROZEN_RANGES)
+                return fail(B200GSR_ERR_BAD_ARG, "more than %d frozen ranges after merging touching ones",
+                            B200GSR_MAX_FROZEN_RANGES);
+            fr.lo[fr.n] = (uint32_t)lo; fr.len[fr.n] = (uint32_t)len;
+            ++fr.n;
+        }
+        end = lo + len;
+    }
+    return backward_views(B, prm, in, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes, max_pairs,
+                          out, flags, fr.n > 0 ? &fr : nullptr, stream);
 }
 
 int b200gsr_backward_views(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, const int32_t* radii,
@@ -631,16 +679,19 @@ int b200gsr_assemble_forward(int32_t num_groups, const b200gsr_group* groups, in
     return rc;
 }
 
-int b200gsr_assemble_backward(int32_t num_groups, const b200gsr_group* groups, const b200gsr_group_grad* grads,
-                              int32_t M, int32_t num_views, float shs_noise, float scale_noise, const float* z_shs,
-                              const float* z_scales, uint64_t seed, const float* d_means3D,
-                              const float* d_opacities, const float* d_scales, const float* d_rotations,
-                              const float* d_shs, void* stream) {
+// b200gsr_assemble_backward (frozen = 0) and b200gsr_assemble_backward_frozen
+static int assemble_backward(int32_t num_groups, const b200gsr_group* groups, const b200gsr_group_grad* grads,
+                             int32_t M, int32_t num_views, float shs_noise, float scale_noise, const float* z_shs,
+                             const float* z_scales, uint64_t seed, const float* d_means3D, const float* d_opacities,
+                             const float* d_scales, const float* d_rotations, const float* d_shs, uint32_t frozen,
+                             void* stream) {
     int rc = check_groups(num_groups, groups, M);
     if (rc) return rc;
+    if (frozen >> num_groups)      // num_groups <= B200GSR_MAX_GROUPS < 32 (check_groups)
+        return fail(B200GSR_ERR_BAD_ARG, "frozen mask 0x%x has bits at or above num_groups %d", frozen, num_groups);
     if (num_groups > 0 && !grads) return fail(B200GSR_ERR_BAD_ARG, "grads is null");
     for (int g = 0; g < num_groups; ++g)
-        if (groups[g].n > 0 && (!grads[g].xyz || !grads[g].opacity || !grads[g].scaling || !grads[g].rotation ||
+        if (groups[g].n > 0 && !((frozen >> g) & 1u) && (!grads[g].xyz || !grads[g].opacity || !grads[g].scaling || !grads[g].rotation ||
                                 !grads[g].f_dc || (M > 1 && !grads[g].f_rest)))
             return fail(B200GSR_ERR_BAD_ARG, "group %d: null gradient pointer", g);
     if (!d_means3D || !d_opacities || !d_scales || !d_rotations || !d_shs) return fail(B200GSR_ERR_BAD_ARG, "null gradient input");
@@ -649,9 +700,28 @@ int b200gsr_assemble_backward(int32_t num_groups, const b200gsr_group* groups, c
     rc = check_cuda(gsr_launch_assemble(true, num_groups, groups, grads, M, num_views, shs_noise, scale_noise, z_shs, z_scales, seed,
                                         const_cast<float*>(d_means3D), const_cast<float*>(d_opacities),
                                         const_cast<float*>(d_scales), const_cast<float*>(d_rotations),
-                                        const_cast<float*>(d_shs), static_cast<cudaStream_t>(stream)), "assemble_backward");
+                                        const_cast<float*>(d_shs), static_cast<cudaStream_t>(stream), frozen),
+                    "assemble_backward");
     GSR_RANGE_POP();
     return rc;
+}
+
+int b200gsr_assemble_backward(int32_t num_groups, const b200gsr_group* groups, const b200gsr_group_grad* grads,
+                              int32_t M, int32_t num_views, float shs_noise, float scale_noise, const float* z_shs,
+                              const float* z_scales, uint64_t seed, const float* d_means3D,
+                              const float* d_opacities, const float* d_scales, const float* d_rotations,
+                              const float* d_shs, void* stream) {
+    return assemble_backward(num_groups, groups, grads, M, num_views, shs_noise, scale_noise, z_shs, z_scales, seed,
+                             d_means3D, d_opacities, d_scales, d_rotations, d_shs, 0u, stream);
+}
+
+int b200gsr_assemble_backward_frozen(int32_t num_groups, const b200gsr_group* groups, const b200gsr_group_grad* grads,
+                                     int32_t M, int32_t num_views, float shs_noise, float scale_noise,
+                                     const float* z_shs, const float* z_scales, uint64_t seed, const float* d_means3D,
+                                     const float* d_opacities, const float* d_scales, const float* d_rotations,
+                                     const float* d_shs, uint32_t frozen_groups, void* stream) {
+    return assemble_backward(num_groups, groups, grads, M, num_views, shs_noise, scale_noise, z_shs, z_scales, seed,
+                             d_means3D, d_opacities, d_scales, d_rotations, d_shs, frozen_groups, stream);
 }
 
 int b200gsr_disparity_forward(int32_t B, int32_t N, const float* depth_alpha, const float* focal, float* out_disp,

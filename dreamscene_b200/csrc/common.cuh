@@ -5,6 +5,7 @@
 #include <atomic>
 
 #include "../../include/b200gsr_reserve.h"
+#include "../../include/b200gsr_views_frozen.h"
 
 #define GSR_TILE 16
 #define GSR_NEAR_Z 0.2f
@@ -281,6 +282,14 @@ struct GsrFwdArgs {
     const GsrScene* scene; // scene render: the raw leaves replace means3D .. cov3d (null otherwise)
 };
 
+// Frozen rows of a multi-view backward (b200gsr_backward_views_frozen): n sorted, merged, non-empty half-open ranges
+// [lo, lo + len) of one view's P rows, the same in every view.  composite_bwd and project_bwd run their FROZEN
+// instantiations over them.
+struct GsrFrozenRanges {
+    int n;
+    uint32_t lo[B200GSR_MAX_FROZEN_RANGES], len[B200GSR_MAX_FROZEN_RANGES];
+};
+
 struct GsrBwdArgs {
     b200gsr_params prm;
     const float *means3D, *shs, *colors, *opac, *scales, *rots, *cov3d;
@@ -300,6 +309,7 @@ struct GsrBwdArgs {
     unsigned long long* stats;   // optional device counters (b200gsr_debug_counters); selects the STATS kernels
     cudaStream_t stream;
     const GsrScene* scene;       // scene render: leaf gradients of the raw parameters (null otherwise)
+    const GsrFrozenRanges* frozen_rows;   // b200gsr_backward_views_frozen with ranges (null otherwise)
 };
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device) instead of on every
@@ -338,7 +348,8 @@ cudaError_t gsr_launch_mark_visible(int P, const float* means3D, const float* vi
 cudaError_t gsr_launch_assemble(bool backward, int num_groups, const b200gsr_group* groups,
                                 const b200gsr_group_grad* grads, int M, int B, float c_shs, float c_scale,
                                 const float* z_shs, const float* z_scales, unsigned long long seed,
-                                float* means3D, float* opac, float* scales, float* rots, float* shs, cudaStream_t s);
+                                float* means3D, float* opac, float* scales, float* rots, float* shs, cudaStream_t s,
+                                uint32_t frozen = 0u);   // backward: bit g = group g is frozen (nothing read or written)
 
 // disparity post-processing (postprocess.cu)
 cudaError_t gsr_launch_disparity_fwd(int B, int N, const float* da, const float* focal, float* out, void* stats,

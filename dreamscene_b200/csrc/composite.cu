@@ -425,8 +425,10 @@ __device__ __forceinline__ void halve2(float (&v)[10], bool hi) {
 }
 
 // Frozen groups (b200gsr_backward_scene_frozen): the packed rows of the frozen groups as merged half-open intervals
-// [lo, lo + len).  Adjacent frozen groups merge, so 24 groups give at most 12 intervals.
+// [lo, lo + len).  Adjacent frozen groups merge, so 24 groups give at most 12 intervals.  The caller's frozen row
+// ranges of b200gsr_backward_views_frozen arrive in the same form.
 constexpr int kMaxFrozenIntervals = (B200GSR_MAX_GROUPS + 1) / 2;
+static_assert(kMaxFrozenIntervals == B200GSR_MAX_FROZEN_RANGES, "b200gsr_views_frozen.h states the interval limit");
 struct NoFrozen {};
 struct FrozenRows {
     uint32_t n;                              // intervals in use
@@ -840,6 +842,15 @@ static FrozenRows frozen_rows(const GsrScene& sc, int P_view) {
     return f;
 }
 
+// The caller's frozen row ranges (b200gsr_backward_views_frozen, validated and merged by the entry point).
+static FrozenRows frozen_rows(const GsrFrozenRanges& r, int P_view) {
+    FrozenRows f{};
+    f.P_view = (uint32_t)P_view;
+    f.n = (uint32_t)r.n;
+    for (int k = 0; k < r.n; ++k) { f.lo[k] = r.lo[k]; f.len[k] = r.len[k]; }
+    return f;
+}
+
 cudaError_t gsr_launch_composite_bwd(const GsrBwdArgs& a) {
     const CompPtrs c = comp_ptrs(a.saved, a.vl, a.prm.image_height, a.prm.image_width, a.num_views, a.gy_view);
     if (c.grid.ntiles == 0) return cudaSuccess;
@@ -847,8 +858,9 @@ cudaError_t gsr_launch_composite_bwd(const GsrBwdArgs& a) {
     float* dgeom = reinterpret_cast<float*>(a.saved + a.vl.dgeom);
     // Frozen groups: the FROZEN instantiations; the instrumented kernel has no such mode and the counters are left
     // untouched, as in deterministic mode.
-    const bool frozen = a.scene != nullptr && a.scene->frozen != 0u;
-    const FrozenRows fz = frozen ? frozen_rows(*a.scene, a.P_view) : FrozenRows{};
+    const bool frozen = (a.scene != nullptr && a.scene->frozen != 0u) || a.frozen_rows != nullptr;
+    const FrozenRows fz = a.frozen_rows ? frozen_rows(*a.frozen_rows, a.P_view)
+                                        : frozen ? frozen_rows(*a.scene, a.P_view) : FrozenRows{};
     if (a.det) {
         // Deterministic mode: the default kernel with integer commits, run twice (instrumentation does not apply).
         // Pass B pops its own work queue (header words, zero between calls like the first one): no memset.

@@ -277,6 +277,9 @@ using BwdScene = std::conditional_t<
     RAW, std::conditional_t<FROZEN, SceneFrozen<std::conditional_t<DYN, SceneBwdDyn, SceneBwd>>,
                             std::conditional_t<DYN, SceneBwdDyn, SceneBwd>>,
     NoScene>;
+// The packed-input backward with frozen rows (project_bwd_rows_frozen_kernel, b200gsr_backward_views_frozen): the
+// caller's frozen row ranges of one view.  Derived from NoScene, whose fields (none) the default statements read.
+struct RowsFrozen : NoScene { GsrFrozenRanges rows; };
 // STATS (RAW, project_bwd_stats_kernel): the densification statistics of b200gsr_backward_scene[_dyn]_stats.  Per
 // group the destinations (accum null = the group gathers nothing; max_radii may be null), and the view whose launch
 // gathers: `view` by value, or *view_dev under DYN (null = none).  Derived from SceneFrozen whatever FROZEN is.
@@ -335,11 +338,21 @@ __device__ __forceinline__ ViewNoise view_noise(const S& sc, b200gsr_params& p) 
 #define GSR_C_SHS (DYN ? nz.c_shs : sc.c_shs)
 #define GSR_C_SCALE (DYN ? nz.c_scale : sc.c_scale)
 
-// FROZEN: whether active row i belongs to a frozen group.  A constant false otherwise.
+// FROZEN: whether active row i belongs to a frozen group (RAW) or lies in one of the frozen row ranges (packed
+// inputs; a loop over the ranges in use, as composite_bwd's row_frozen).  A constant false otherwise.
 template <bool FROZEN, typename S>
 __device__ __forceinline__ bool frozen_row(const S& sc, bool active, int i) {
-    if constexpr (FROZEN) return active && ((sc.frozen >> find_group(sc.tab, i)) & 1u);
-    else return false;
+    if constexpr (FROZEN && std::is_same_v<S, RowsFrozen>) {
+        if (!active) return false;
+#pragma unroll 1
+        for (int k = 0; k < sc.rows.n; ++k)
+            if ((uint32_t)i - sc.rows.lo[k] < sc.rows.len[k]) return true;
+        return false;
+    } else if constexpr (FROZEN) {
+        return active && ((sc.frozen >> find_group(sc.tab, i)) & 1u);
+    } else {
+        return false;
+    }
 }
 
 // A row's shape leaves and what the chain rule needs of them.
@@ -716,6 +729,29 @@ project_bwd_stats_kernel(b200gsr_params p, const float* __restrict__ means3D,
 #include "project_bwd_body.cuh"
 }
 
+// The packed-input backward with frozen row ranges (b200gsr_backward_views_frozen): project_bwd_kernel<MT>'s
+// statements, except that the rows in sc.rows are treated as culled - no SH staging, geometry, dgeom read-and-clear
+// or input load - and their gradient rows and d_means2D rows are written as zeros (added to under `accumulate`), so
+// every output row stays defined.  composite_bwd's FROZEN mode left their dgeom rows at zero.  A kernel of its own
+// rather than a project_bwd_kernel instantiation: a different argument type there would rename every instantiation.
+// S is RowsFrozen: a template parameter so that `sc` has a dependent type and the body's RAW statements are discarded;
+// __grid_constant__ so that the range loop reads the constant bank rather than a local copy.
+template <int MT, typename S>
+__global__ void __launch_bounds__(kBlock, 6)
+project_bwd_rows_frozen_kernel(b200gsr_params p, const float* __restrict__ means3D,
+                               const float* __restrict__ shs, const float* __restrict__ colors,
+                               const float* __restrict__ scales, const float* __restrict__ rots,
+                               const float* __restrict__ cov3d, const int32_t* __restrict__ radii,
+                               float* __restrict__ dgeom, uint32_t* __restrict__ bwd_queue,
+                               int g_base, int g_end, int dsh_coefs, int rec_base, int accumulate,
+                               float* __restrict__ d_means3D, float* __restrict__ d_means2D,
+                               float* __restrict__ d_shs, float* __restrict__ d_colors,
+                               float* __restrict__ d_opac, float* __restrict__ d_scales,
+                               float* __restrict__ d_rots, float* __restrict__ d_cov3d, const __grid_constant__ S sc) {
+    constexpr bool RAW = false, DYN = false, FROZEN = true, STATS = false, LIVE = false;
+#include "project_bwd_body.cuh"
+}
+
 __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D,
                                     const float* __restrict__ V, uint8_t* __restrict__ visible) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -821,6 +857,19 @@ static void launch_project_bwd(const GsrBwdArgs& a, int g_begin, int g_end, size
         a.d_colors, a.d_opac, a.d_scales, a.d_rots, a.d_cov3d, sc);
 }
 
+template <int MT>
+static void launch_project_bwd_rows_frozen(const GsrBwdArgs& a, int g_begin, int g_end, size_t smem) {
+    RowsFrozen sc{};
+    sc.rows = *a.frozen_rows;
+    project_bwd_rows_frozen_kernel<MT, RowsFrozen><<<(g_end - g_begin + kBlock - 1) / kBlock, kBlock, smem, a.stream>>>(
+        a.prm, a.means3D, a.shs, a.colors, a.scales, a.rots, a.cov3d, a.radii,
+        reinterpret_cast<float*>(a.saved + a.vl.dgeom),
+        reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE, g_begin, g_end,
+        a.dsh_coefs > 0 ? a.dsh_coefs : (a.dsh_coefs < 0 ? -1 : a.prm.M), a.view * a.P_view, a.accumulate, a.d_means3D,
+        a.d_means2D, a.d_shs,
+        a.d_colors, a.d_opac, a.d_scales, a.d_rots, a.d_cov3d, sc);
+}
+
 template <bool DYN, bool FROZEN, bool LIVE = false>
 static void launch_project_bwd_stats(const GsrBwdArgs& a, int g_begin, int g_end, size_t smem) {
     StatsScene<DYN, LIVE> sc{};
@@ -863,6 +912,9 @@ cudaError_t gsr_launch_project_bwd(const GsrBwdArgs& a) {
     else if (a.scene && frozen) launch_project_bwd<0, true, false, true>(a, g_begin, g_end, smem);
     else if (a.scene && a.scene->dyn_views) launch_project_bwd<0, true, true>(a, g_begin, g_end, smem);
     else if (a.scene) launch_project_bwd<0, true>(a, g_begin, g_end, smem);
+    else if (a.frozen_rows && a.shs && a.prm.M == 16) launch_project_bwd_rows_frozen<16>(a, g_begin, g_end, smem);
+    else if (a.frozen_rows && a.shs && a.prm.M == 4) launch_project_bwd_rows_frozen<4>(a, g_begin, g_end, smem);
+    else if (a.frozen_rows) launch_project_bwd_rows_frozen<0>(a, g_begin, g_end, smem);
     else if (a.shs && a.prm.M == 16) launch_project_bwd<16>(a, g_begin, g_end, smem);
     else if (a.shs && a.prm.M == 4) launch_project_bwd<4>(a, g_begin, g_end, smem);
     else launch_project_bwd<0>(a, g_begin, g_end, smem);

@@ -1,6 +1,6 @@
-// The statements of project_bwd_kernel and project_bwd_stats_kernel (project.cu), included into the body of each.
-// In scope: the kernel's parameters and the compile-time MT, RAW, DYN, FROZEN, STATS and LIVE (see project_bwd_kernel
-// and project_bwd_stats_kernel).
+// The statements of project_bwd_kernel, project_bwd_stats_kernel and project_bwd_rows_frozen_kernel (project.cu),
+// included into the body of each.  In scope: the kernel's parameters and the compile-time MT, RAW, DYN, FROZEN, STATS
+// and LIVE (see those kernels).
 extern __shared__ __align__(16) float sh_buf[];
 __shared__ uint8_t vis_s[kBlock];
 const ViewNoise nz = view_noise<DYN>(sc, p);

@@ -14,6 +14,11 @@ instead of B.
                            means2D=[m2d_0, ..., m2d_{B-1}])
     color_v, radii_v, depth_alpha_v = outs[v]
 
+Frozen rows: ``frozen_rows=[(lo, hi), ...]`` (half-open ranges of the P rows, the same in every view) are rendered as
+any other row, but the backward computes no gradient for them: their gradient rows and means2D rows are zeros, and
+the other rows' gradients are those of the call without ``frozen_rows`` (bit for bit in deterministic mode).
+``scene.frozen_rows(groups, frozen)`` gives the ranges of frozen parameter groups packed by ``scene.assemble_scene``.
+
 Every tensor argument is either ONE tensor (shared by all views) or a list of B tensors (per-view
 values, e.g. the separately augmented shs / scales of scene_render); `settings_list` holds the B
 GaussianRasterizationSettings (cameras, sh_degree, scale_modifier, bg may differ; image size and
@@ -36,9 +41,39 @@ _GRAD_FIELD = {"means3D": "d_means3D", "opacities": "d_opacities", "shs": "d_shs
                "scales": "d_scales", "rotations": "d_rotations", "cov3D_precomp": "d_cov3D"}
 
 
+def _frozen_ranges(frozen_rows, P: int):
+    """None or [(lo, hi), ...] -> the merged (lo, len) pairs that b200gsr_backward_views_frozen takes.  Refuses what
+    the library refuses: an empty, out-of-bounds, unsorted or overlapping range, or more than MAX_FROZEN_RANGES after
+    merging ranges that touch."""
+    if frozen_rows is None:
+        return ()
+    out: list = []
+    end = 0
+    for k, r in enumerate(frozen_rows):
+        if len(r) != 2:
+            raise ValueError(f"frozen_rows[{k}]: expected a (lo, hi) pair, got {r!r}")
+        lo, hi = int(r[0]), int(r[1])
+        if hi <= lo:
+            raise ValueError(f"frozen_rows[{k}] = ({lo}, {hi}) is empty")
+        if lo < 0 or hi > P:
+            raise ValueError(f"frozen_rows[{k}] = ({lo}, {hi}) is outside [0, P = {P})")
+        if k > 0 and lo < end:
+            raise ValueError(f"frozen_rows[{k}] = ({lo}, {hi}) starts before the end {end} of frozen_rows[{k - 1}]: "
+                             "the ranges must be sorted and must not overlap")
+        if out and lo == end:
+            out[-1] = (out[-1][0], out[-1][1] + hi - lo)
+        else:
+            out.append((lo, hi - lo))
+        end = hi
+    if len(out) > _lib.MAX_FROZEN_RANGES:
+        raise ValueError(f"frozen_rows: {len(out)} ranges after merging touching ones, at most "
+                         f"{_lib.MAX_FROZEN_RANGES}")
+    return tuple(out)
+
+
 class _RasterizeViews(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, settings, spec, B, *flat):
+    def forward(ctx, settings, spec, B, frozen, *flat):
         # spec[name] = None | ("shared", idx) | ("list", [idx...]) into `flat`; flat also holds the B means2D ports last
         lib = _lib.load()
         tensors = [_lib.prepare(t) for t in flat]
@@ -78,7 +113,7 @@ class _RasterizeViews(torch.autograd.Function):
 
             saved, cap = R._issue_with_capacity(d, (B, P, H, W), B * P, Hs, W, with_backward, det, score, launch, capturing,
                                                 stream.value)
-        ctx.meta = (spec, B, P, W, Hs, cap, with_backward, len(flat), det)
+        ctx.meta = (spec, B, P, W, Hs, cap, with_backward, len(flat), det, frozen)
         ctx.views = (prm, vin)            # the backward reuses the arrays; `keep` holds their device constants
         ctx.keep = keep
         ctx.saved_buf = saved
@@ -92,7 +127,7 @@ class _RasterizeViews(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_color, _g_radii, g_da, *_):
-        spec, B, P, W, Hs, cap, with_backward, nflat, det = ctx.meta
+        spec, B, P, W, Hs, cap, with_backward, nflat, det, frozen = ctx.meta
         prm, vin = ctx.views
         radii, depth_alpha = ctx.saved_tensors[:2]
         tensors = list(ctx.saved_tensors[2:])
@@ -124,20 +159,28 @@ class _RasterizeViews(torch.autograd.Function):
                 out[v].d_means2D = g2.data_ptr()
                 out[v].accumulate = acc
             ptr = _lib.ptr
-            rc = lib.b200gsr_backward_views_ex(B, prm, vin, ptr(radii), ptr(depth_alpha), ptr(g_color), ptr(g_da),
-                                               ptr(ctx.saved_buf), ctx.saved_buf.numel(), cap, out,
-                                               _lib.BWD_DETERMINISTIC if det else 0, _lib.stream(dev))
-        _lib.check(rc, "b200gsr_backward_views")
-        return (None, None, None) + tuple(grads)
+            args = (B, prm, vin, ptr(radii), ptr(depth_alpha), ptr(g_color), ptr(g_da), ptr(ctx.saved_buf),
+                    ctx.saved_buf.numel(), cap, out, _lib.BWD_DETERMINISTIC if det else 0)
+            if frozen:
+                ranges = (_lib.RowRange * len(frozen))(*[_lib.RowRange(lo, n) for lo, n in frozen])
+                rc = lib.b200gsr_backward_views_frozen(*args, ranges, len(frozen), _lib.stream(dev))
+            else:
+                rc = lib.b200gsr_backward_views_ex(*args, _lib.stream(dev))
+        _lib.check(rc, "b200gsr_backward_views_frozen" if frozen else "b200gsr_backward_views")
+        return (None, None, None, None) + tuple(grads)
 
 
 def rasterize_views(settings: Sequence[R.GaussianRasterizationSettings], means3D: TensorOrList, opacities: TensorOrList,
                     shs: TensorOrList = None, colors_precomp: TensorOrList = None, scales: TensorOrList = None,
                     rotations: TensorOrList = None, cov3D_precomp: TensorOrList = None,
-                    means2D: Optional[Sequence[torch.Tensor]] = None):
+                    means2D: Optional[Sequence[torch.Tensor]] = None,
+                    frozen_rows: Optional[Sequence[Sequence[int]]] = None):
     """-> list of B tuples (color[3,H,W], radii[P], depth_alpha[2,H,W]) (score first when score_flag), views
     into the stacked outputs.  means2D: optional list of B [P,3] tensors whose .grad receives the per-view
-    screen-space gradients (the reference's viewspace_points)."""
+    screen-space gradients (the reference's viewspace_points).  frozen_rows: None, or sorted, non-overlapping,
+    non-empty (lo, hi) ranges of the P rows (at most MAX_FROZEN_RANGES once touching ones merge) whose gradient the
+    backward does not compute: their rows of every input's gradient and of the means2D gradients are zeros, and the
+    other rows get the gradients of the call without frozen_rows."""
     B = len(settings)
     if not 1 <= B <= _lib.MAX_VIEWS:
         raise ValueError(f"need 1..{_lib.MAX_VIEWS} views")
@@ -171,7 +214,8 @@ def rasterize_views(settings: Sequence[R.GaussianRasterizationSettings], means3D
     for s in settings:
         if int(s.image_height) != H or int(s.image_width) != int(settings[0].image_width) or bool(s.score_flag) != bool(settings[0].score_flag):
             raise ValueError("all views must share the image size and score_flag")
-    res = _RasterizeViews.apply(tuple(settings), spec, B, *flat)
+    frozen = _frozen_ranges(frozen_rows, P)
+    res = _RasterizeViews.apply(tuple(settings), spec, B, frozen, *flat)
     color, radii, da = res[0], res[1], res[2]
     Hp = color.shape[1] // B
     outs = []

@@ -27,6 +27,10 @@ Noise modes
   shs_aug / scale_aug = False switch the respective augmentation off (the reference draws
   ``random.random() < ratio`` on the host for that decision: pass its outcome).
 
+Frozen groups: ``assemble_scene(groups, frozen=[...])`` gives a frozen group's leaves no gradient, and
+``rasterize_views(..., frozen_rows=frozen_rows(groups, frozen))`` skips their packed rows' gradient work, so a stage
+that trains one group pays for the backward of that group only.
+
 ``render_scene(groups, settings_list, ...)`` goes one step further: the B views of a training step rendered straight
 from the raw groups, with the activations and the Philox augmentation inside the projection kernels (no augmented copy
 of shs / scales and no per-view gradient of them is ever written); the rasterizer inputs are bit for bit those of
@@ -60,7 +64,7 @@ def _group_table(raw: Sequence[Sequence[torch.Tensor]]):
 
 class _Assemble(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, num_groups, M, B, c_shs, c_scale, z_shs, z_scales, seed, *flat):
+    def forward(ctx, num_groups, M, B, c_shs, c_scale, z_shs, z_scales, seed, frozen, *flat):
         raw = [[_lib.prepare(t.detach()) for t in flat[6 * k:6 * k + 6]] for k in range(num_groups)]
         dev = raw[0][0].device
         P = sum(int(ts[0].shape[0]) for ts in raw)
@@ -71,14 +75,14 @@ class _Assemble(torch.autograd.Function):
             rc = lib.b200gsr_assemble_forward(num_groups, _group_table(raw), M, B, c_shs, c_scale, ptr(z_shs), ptr(z_scales),
                                               seed, *[ptr(o) for o in out], _lib.stream(dev))
         _lib.check(rc, "b200gsr_assemble_forward")
-        ctx.meta = (num_groups, M, B, c_shs, c_scale, seed)
+        ctx.meta = (num_groups, M, B, c_shs, c_scale, seed, frozen)
         ctx.noise = (z_shs, z_scales)
         ctx.save_for_backward(*[t for ts in raw for t in ts])
         return tuple(out)
 
     @staticmethod
     def backward(ctx, g_means, g_opac, g_scales, g_rots, g_shs):
-        num_groups, M, B, c_shs, c_scale, seed = ctx.meta
+        num_groups, M, B, c_shs, c_scale, seed, frozen = ctx.meta
         z_shs, z_scales = ctx.noise
         saved = ctx.saved_tensors
         raw = [list(saved[6 * k:6 * k + 6]) for k in range(num_groups)]
@@ -87,22 +91,28 @@ class _Assemble(torch.autograd.Function):
         shapes = [(P, 3), (P, 1), (B, P, 3), (P, 4), (B, P, M, 3)]
         gin = [torch.zeros(s, device=dev) if g is None else _lib.prepare(g.detach())
                for g, s in zip((g_means, g_opac, g_scales, g_rots, g_shs), shapes)]
-        grads = [[torch.empty_like(t) for t in ts] for ts in raw]
+        # a frozen group gets no gradient: nothing of it is read or written
+        grads = [[None] * 6 if (frozen >> k) & 1 else [torch.empty_like(t) for t in ts] for k, ts in enumerate(raw)]
         garr = (_lib.GroupGrad * num_groups)()
         for k, ts in enumerate(grads):
             for name, t in zip(("xyz", "opacity", "scaling", "rotation", "f_dc", "f_rest"), ts):
-                setattr(garr[k], name, t.data_ptr() if t.numel() else None)
+                setattr(garr[k], name, t.data_ptr() if t is not None and t.numel() else None)
         lib, ptr = _lib.load(), _lib.ptr
+        args = (num_groups, _group_table(raw), garr, M, B, c_shs, c_scale, ptr(z_shs), ptr(z_scales), seed,
+                *[ptr(g) for g in gin])
         with torch.cuda.device(dev):
-            rc = lib.b200gsr_assemble_backward(num_groups, _group_table(raw), garr, M, B, c_shs, c_scale, ptr(z_shs),
-                                               ptr(z_scales), seed, *[ptr(g) for g in gin], _lib.stream(dev))
-        _lib.check(rc, "b200gsr_assemble_backward")
-        return (None,) * 8 + tuple(t for ts in grads for t in ts)
+            if frozen:
+                rc = lib.b200gsr_assemble_backward_frozen(*args, frozen, _lib.stream(dev))
+            else:
+                rc = lib.b200gsr_assemble_backward(*args, _lib.stream(dev))
+        _lib.check(rc, "b200gsr_assemble_backward_frozen" if frozen else "b200gsr_assemble_backward")
+        return (None,) * 9 + tuple(t for ts in grads for t in ts)
 
 
 def assemble_scene(groups: Sequence, shs_aug: bool = True, scale_aug: bool = True, noise: str = "torch",
                    seed: int | None = None, generator: torch.Generator | None = None,
-                   z_shs: torch.Tensor | None = None, z_scales: torch.Tensor | None = None, views: int = 1):
+                   z_shs: torch.Tensor | None = None, z_scales: torch.Tensor | None = None, views: int = 1,
+                   frozen: Sequence[bool] | None = None):
     """-> (means3D[P,3], opacities[P,1], scales[P,3], rotations[P,4], shs[P,M,3]) ready for
     GaussianRasterizer, differentiable w.r.t. every group's raw leaves.  z_shs [P,M,3] / z_scales [P,3]:
     explicit standard-normal draws (noise="torch" only; drawn with torch.randn when omitted).
@@ -110,11 +120,17 @@ def assemble_scene(groups: Sequence, shs_aug: bool = True, scale_aug: bool = Tru
     views = B > 1: the B views of one training step in ONE pass over the raw parameters: returns
     scales [B,P,3] and shs [B,P,M,3] (an independently augmented copy per view; index them per view for
     rasterize_views), means3D / opacities / rotations once; the backward sums the per-view gradients in the
-    kernel.  With noise="torch" the draws follow the reference's order view by view (shs, then scales)."""
+    kernel.  With noise="torch" the draws follow the reference's order view by view (shs, then scales).
+
+    frozen: None, or one bool per group, as render_scene's.  A frozen group's leaves get None as their gradient and
+    the backward reads none of its packed gradient rows; the other groups' gradients are unchanged.  Pass
+    frozen_rows(groups, frozen) to rasterize_views as well, so that its backward skips those rows too.  Explicit, not
+    inferred from requires_grad."""
     if not 1 <= len(groups) <= _lib.MAX_GROUPS:
         raise ValueError(f"need 1..{_lib.MAX_GROUPS} groups")
     if noise not in ("torch", "fused"):
         raise ValueError("noise must be 'torch' or 'fused'")
+    frozen_mask = _frozen_mask(frozen, len(groups), "assemble_scene")
     flat = [_get(g, name) for g in groups for name in _FIELDS]
     dev = flat[0].device
     if dev.type != "cuda":
@@ -147,8 +163,26 @@ def assemble_scene(groups: Sequence, shs_aug: bool = True, scale_aug: bool = Tru
             cpu_gen = generator if generator is not None and generator.device.type == "cpu" else None
             seed = int(torch.randint(0, 2 ** 62, (1,), generator=cpu_gen).item())
     m, o, sc, r, sh = _Assemble.apply(len(groups), M, B, NOISE_COEF if shs_aug else 0.0, NOISE_COEF if scale_aug else 0.0,
-                                      z_shs, z_scales, int(seed), *flat)
+                                      z_shs, z_scales, int(seed), frozen_mask, *flat)
     return (m, o, sc[0], r, sh[0]) if B == 1 else (m, o, sc, r, sh)
+
+
+def frozen_rows(groups: Sequence, frozen: Sequence[bool] | None):
+    """The packed rows of the frozen groups - in assemble_scene's order, one bool per group - as the sorted, merged
+    (lo, hi) ranges that rasterize_views(frozen_rows=) takes.  Empty groups take no rows, so frozen groups on both
+    sides of one merge.  [] when nothing is frozen."""
+    mask = _frozen_mask(frozen, len(groups), "frozen_rows")
+    out: list = []
+    row = 0
+    for k, g in enumerate(groups):
+        n = int(_get(g, "_xyz").shape[0])
+        if n > 0 and (mask >> k) & 1:
+            if out and out[-1][1] == row:
+                out[-1] = (out[-1][0], row + n)
+            else:
+                out.append((row, row + n))
+        row += n
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------------------
