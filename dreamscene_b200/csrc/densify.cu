@@ -34,6 +34,12 @@ __global__ void densify_stats_kernel(int P, const float* __restrict__ vs_grad, c
 
 __device__ __forceinline__ float sigmoidf_rn(float x) { return __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-x))); }
 
+// A split child's log-scale, log(exp(s) / (0.8 N)) (gs_renderer.py:984-992).  torch divides a CUDA tensor by a CPU
+// scalar as a multiply by the fp32 reciprocal, inv = fp32(1 / fp32(0.8 N)); a true division differs in the last bit
+// of the quotient on a fifth of the elements.  split_children_kernel stores this value and densify_classify_kernel
+// decides the children's prune on it.
+__device__ __forceinline__ float child_log_scale(float e, float inv) { return logf(__fmul_rn(e, inv)); }
+
 // Decisions of densify_and_prune(max_grad, min_opacity, extent, max_screen_size) restated per ORIGINAL point:
 //   grads = accum / denom, NaN -> 0
 //   clone : |grads| >= max_grad  and  max(exp(scaling)) <= percent_dense * extent      (appended unchanged)
@@ -49,13 +55,15 @@ __global__ void densify_classify_kernel(int P, const float* __restrict__ accum, 
     if (i >= P) return;
     float g = __fdiv_rn(accum[i], denom[i]);
     if (isnan(g)) g = 0.0f;
-    const float s = fmaxf(fmaxf(expf(scaling[3 * (size_t)i]), expf(scaling[3 * (size_t)i + 1])), expf(scaling[3 * (size_t)i + 2]));
+    const float e0 = expf(scaling[3 * (size_t)i]), e1 = expf(scaling[3 * (size_t)i + 1]), e2 = expf(scaling[3 * (size_t)i + 2]);
+    const float s = fmaxf(fmaxf(e0, e1), e2);
     const bool clone = (fabsf(g) >= max_grad) && (s <= dense_extent);
     const bool split = (g >= max_grad) && (s > dense_extent);
     const bool low = sigmoidf_rn(opacity[i]) < min_opacity;
     const bool pruned = low || (big_ws > 0.0f && s > big_ws);
-    // children: scaling_inverse(exp(scaling) / (0.8 N)) -> their activation is exp(log(s / (0.8 N)))
-    const float sc = expf(logf(__fdiv_rn(s, child_div)));
+    // the final prune sees the children's stored log-scales: max over the components of exp(child_log_scale(e_k))
+    const float inv = __fdiv_rn(1.0f, child_div);
+    const float sc = fmaxf(fmaxf(expf(child_log_scale(e0, inv)), expf(child_log_scale(e1, inv))), expf(child_log_scale(e2, inv)));
     const bool child_pruned = low || (big_ws > 0.0f && sc > big_ws);
     flags[(size_t)kKeep * P + i] = (!split && !pruned) ? 1u : 0u;
     flags[(size_t)kClone * P + i] = (clone && !pruned) ? 1u : 0u;
@@ -184,7 +192,7 @@ __global__ void gather_rows_kernel(int n_out, int row, const int32_t* __restrict
     out[e] = (kind != 0 && zero_appended) ? 0.0f : in[(size_t)s * row + c];
 }
 
-// split children: xyz = R(normalize(q)) (z * exp(scaling)) + xyz ; scaling = log(exp(scaling) / (0.8 N))
+// split children: xyz = R(normalize(q)) (z * exp(scaling)) + xyz ; scaling = child_log_scale(exp(scaling))
 // (gs_renderer.py:984-992; build_rotation normalises the quaternion: gs_renderer.py:124-147)
 __global__ void split_children_kernel(int n_out, int first_child, float child_div, const int32_t* __restrict__ src_map,
                                       const int32_t* __restrict__ child_draw, const float* __restrict__ xyz,
@@ -205,14 +213,16 @@ __global__ void split_children_kernel(int n_out, int first_child, float child_di
     xyz_out[3 * (size_t)p] = R00 * s0 + R01 * s1 + R02 * s2 + xyz[3 * (size_t)s];
     xyz_out[3 * (size_t)p + 1] = R10 * s0 + R11 * s1 + R12 * s2 + xyz[3 * (size_t)s + 1];
     xyz_out[3 * (size_t)p + 2] = R20 * s0 + R21 * s1 + R22 * s2 + xyz[3 * (size_t)s + 2];
-    const float d = child_div;
-    scaling_out[3 * (size_t)p] = logf(__fdiv_rn(e0, d));
-    scaling_out[3 * (size_t)p + 1] = logf(__fdiv_rn(e1, d));
-    scaling_out[3 * (size_t)p + 2] = logf(__fdiv_rn(e2, d));
+    const float inv = __fdiv_rn(1.0f, child_div);
+    scaling_out[3 * (size_t)p] = child_log_scale(e0, inv);
+    scaling_out[3 * (size_t)p + 1] = child_log_scale(e1, inv);
+    scaling_out[3 * (size_t)p + 2] = child_log_scale(e2, inv);
 }
 
 // ---- k-th smallest of n floats (ascending, k 0-based): 4-pass radix select on order-preserving keys ------
+// Every NaN maps to the largest key, whatever its sign bit, so NaNs sort last as in torch.sort.
 __device__ __forceinline__ uint32_t float_key(float f) {
+    if (isnan(f)) return 0xffffffffu;
     const uint32_t b = __float_as_uint(f);
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }

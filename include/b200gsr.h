@@ -364,7 +364,8 @@ int b200gsr_disparity_backward_ex(int32_t B, int32_t N, const float* depth_alpha
  *                  {kept originals, surviving clones, surviving split parents, split parents, sum};
  *                  the new point count is totals5[0] + totals5[1] + N * totals5[2].
  *                  dense_extent = percent_dense * extent; big_ws = 0.1 * extent or <= 0 (max_screen_size
- *                  is None); child_div = 0.8 * N as float32.
+ *                  is None); child_div = 0.8 * N as float32.  A split child is pruned on the max over its
+ *                  components of exp(log(exp(s_k) * fp32(1 / child_div))), the log-scale split_children stores.
  * densify_map    : src_map[int32, new count]: bits 0..29 = source row, bits 30..31 = 0 original / 1 clone /
  *                  2 split child, in the reference's output order [originals | clones | children, N blocks];
  *                  child_draw[N * totals5[2]] = row of the reference's torch.normal(std=stds) draw each
@@ -373,9 +374,11 @@ int b200gsr_disparity_backward_ex(int32_t B, int32_t N, const float* depth_alpha
  * gather_rows    : out[p, :] = in[src_map[p], :] for rows of `row_floats` floats; with zero_appended, rows
  *                  whose source is a clone/child become zeros (Adam moments, statistics).
  * split_children : xyz / log-scales of the children (rows >= first_child of the new arrays) from the
- *                  parents' raw parameters and the caller's standard-normal draws z[N * split parents, 3].
+ *                  parents' raw parameters and the caller's standard-normal draws z[N * split parents, 3];
+ *                  log-scale = log(exp(s) * fp32(1 / child_div)), torch's division by a CPU scalar.
  * kth_smallest   : *out = k-th smallest (0-based) of v[n]: the percentile threshold of prune_gaussians
- *                  without a sort.  scratch >= 1032 bytes.
+ *                  without a sort.  Orders as torch.sort: every NaN (either sign) after +inf; -0 sorts
+ *                  before +0, equal by value to torch's pick.  scratch >= 1032 bytes.
  */
 int b200gsr_densify_stats(int32_t P, const float* viewspace_grad, const int32_t* radii, float* accum,
                           float* denom, float* max_radii2D, void* stream);

@@ -33,7 +33,7 @@ def test_densify_and_prune_matches_reference_logic(P, max_screen, N):
         assert info["cloned"] > 0 and info["split_parents"] > 0 and info["kept"] < P      # every path exercised
     first_child = info["kept"] + info["cloned"]
     for k in REF.NAMES:
-        if k in ("xyz", "scaling"):
+        if k == "xyz":           # the reference forms the children's positions with torch.bmm
             assert torch.equal(got_p[k][:first_child], want_p[k][:first_child]), k
             assert torch.allclose(got_p[k][first_child:], want_p[k][first_child:], rtol=2e-6, atol=2e-6), k
         else:
