@@ -12,7 +12,7 @@ The eager loss is an L2 against a fixed target plus 0.01 * mean(disp).
 Reported per variant:
   b2b_ms         : wall time per step of `steps` back-to-back steps with one synchronize at the end (median over rounds)
   device_ms      : summed CUDA kernel and copy time per step (torch.profiler, a run of its own)
-  project_bwd_ms : within it, the project_bwd kernels (project_bwd_kernel / project_bwd_stats_kernel)
+  project_bwd_ms : within it, the project_bwd_kernel launches (plain and STATS instantiations)
   peak_mb        : peak allocated memory of building the variant and running its first two steps, above what was
                    allocated before (the graph's static buffers, statistics and optimizer state included)
 Prints one JSON line per layout with the card's name, power limit and max SM clock read in the same run.

@@ -11,8 +11,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200gsr.so")
 SOURCES = ["api.cu", "project.cu", "binning.cu", "composite.cu", "knn.cu", "assemble.cu", "postprocess.cu", "densify.cu",
            "optim.cu", "loss.cu"]
-HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "scene_math.cuh"), os.path.join(CSRC, "project_bwd_body.cuh"),
-           os.path.join(CSRC, "assemble_body.cuh"),
+HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "scene_math.cuh"),
            os.path.join(HERE, "..", "include", "b200gsr.h"), os.path.join(HERE, "..", "include", "b200gsr_scene.h"),
            os.path.join(HERE, "..", "include", "b200gsr_step.h"), os.path.join(HERE, "..", "include", "b200gsr_loss.h"),
            os.path.join(HERE, "..", "include", "b200gsr_frozen.h"), os.path.join(HERE, "..", "include", "b200gsr_stats.h"),
