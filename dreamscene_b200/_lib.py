@@ -1,6 +1,6 @@
 """ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h,
 include/b200gsr_loss.h, include/b200gsr_frozen.h, include/b200gsr_stats.h,
-include/b200gsr_reserve.h, include/b200gsr_frames.h, include/b200gsr_views_frozen.h).  Fails loudly if the library is missing:
+include/b200gsr_reserve.h, include/b200gsr_frames.h, include/b200gsr_views_frozen.h, include/b200gsr_views_stats.h).  Fails loudly if the library is missing:
 there is NO CPU or PyTorch fallback in the product path."""
 from __future__ import annotations
 
@@ -205,6 +205,19 @@ VIEWS_FROZEN_SIGNATURES = {
 }
 MAX_FROZEN_RANGES = 12              # B200GSR_MAX_FROZEN_RANGES
 
+
+class RowStats(C.Structure):        # == b200gsr_row_stats (include/b200gsr_views_stats.h)
+    _fields_ = [("lo", C.c_int32), ("len", C.c_int32)] + \
+        [(n, C.c_void_p) for n in ("xyz_gradient_accum", "denom", "max_radii2D")]
+
+
+# The statistics-gathering backward of include/b200gsr_views_stats.h (same library): the arguments of
+# b200gsr_backward_views_frozen up to num_frozen, then the host record array, its count and the view before the stream.
+VIEWS_STATS_SIGNATURES = {
+    "b200gsr_backward_views_stats": (C.c_int, [i32, _P(Params), _P(ViewInputs)] + [vp] * 5 +
+                                     [sz, u64, _P(ViewGrads), u32, _P(RowRange), i32, _P(RowStats), i32, i32, vp]),
+}
+
 _lib = None
 ABI_VERSION = 3
 ERR_BAD_ARG = -1
@@ -235,7 +248,7 @@ def load():
     lib = C.CDLL(LIB_PATH)
     for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES, **STEP_SIGNATURES, **LOSS_SIGNATURES,
                                       **FROZEN_SIGNATURES, **STATS_SIGNATURES, **RESERVE_SIGNATURES,
-                                      **FRAMES_SIGNATURES, **VIEWS_FROZEN_SIGNATURES}.items():
+                                      **FRAMES_SIGNATURES, **VIEWS_FROZEN_SIGNATURES, **VIEWS_STATS_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:

@@ -8,6 +8,7 @@
 #include "../../include/b200gsr_reserve.h"
 #include "../../include/b200gsr_frames.h"
 #include "../../include/b200gsr_views_frozen.h"
+#include "../../include/b200gsr_views_stats.h"
 
 #include <cstdarg>
 #include <cstdio>
@@ -294,9 +295,11 @@ void set_view_inputs(GsrBwdArgs& a, const b200gsr_view_inputs& in) {
     a.scales = in.scales; a.rots = in.rotations; a.cov3d = in.cov3D_precomp;
 }
 
-bool has_view_grads(const b200gsr_view_inputs& in, const b200gsr_view_grads& o) {
-    return o.d_means3D && o.d_means2D && o.d_opacities && (!in.shs || o.d_shs) && (!in.colors_precomp || o.d_colors) &&
-           (!in.cov3D_precomp || o.d_cov3D) && (in.cov3D_precomp || (o.d_scales && o.d_rotations));
+// means2D_optional: b200gsr_backward_views_stats, whose d_means2D may be null
+bool has_view_grads(const b200gsr_view_inputs& in, const b200gsr_view_grads& o, bool means2D_optional = false) {
+    return o.d_means3D && (o.d_means2D || means2D_optional) && o.d_opacities && (!in.shs || o.d_shs) &&
+           (!in.colors_precomp || o.d_colors) && (!in.cov3D_precomp || o.d_cov3D) &&
+           (in.cov3D_precomp || (o.d_scales && o.d_rotations));
 }
 
 }  // namespace
@@ -478,18 +481,20 @@ int b200gsr_forward_views(int32_t B, const b200gsr_params* prm, const b200gsr_vi
                        saved_bytes, max_pairs, flags, host_notify, notify_seq, stream);
 }
 
-// b200gsr_backward_views_ex (frozen = null) and b200gsr_backward_views_frozen with ranges (validated by the caller)
+// b200gsr_backward_views_ex (frozen = stats = null), b200gsr_backward_views_frozen with ranges and
+// b200gsr_backward_views_stats (ranges and records validated by the caller)
 static int backward_views(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, const int32_t* radii,
                           const float* out_depth_alpha, const float* dL_dcolor, const float* dL_ddepth_alpha,
                           void* saved, size_t saved_bytes, uint64_t max_pairs, const b200gsr_view_grads* out,
-                          uint32_t flags, const GsrFrozenRanges* frozen, void* stream) {
+                          uint32_t flags, const GsrFrozenRanges* frozen, const GsrRowStats* stats, void* stream) {
     int rc;
     const int P = prm[0].P;
     if (P == 0) return B200GSR_OK;
     if (!radii || !out_depth_alpha || !dL_dcolor || !dL_ddepth_alpha || !saved || !out)
         return fail(B200GSR_ERR_BAD_ARG, "null saved-state/gradient pointer");
     for (int v = 0; v < B; ++v)     // before any launch: composite_bwd consumes the work lists project_bwd needs
-        if (!has_view_grads(in[v], out[v])) return fail(B200GSR_ERR_BAD_ARG, "view %d: null gradient output pointer", v);
+        if (!has_view_grads(in[v], out[v], stats != nullptr))
+            return fail(B200GSR_ERR_BAD_ARG, "view %d: null gradient output pointer", v);
     GsrBwdArgs a;
     if ((rc = setup_backward(true, B, prm, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes,
                              max_pairs, (flags & B200GSR_BWD_DETERMINISTIC) != 0, stream, a)))
@@ -497,6 +502,7 @@ static int backward_views(int32_t B, const b200gsr_params* prm, const b200gsr_vi
     set_view_inputs(a, in[0]);
     a.g_begin = 0; a.g_end = P;
     a.frozen_rows = frozen;
+    a.row_stats = stats;
     GSR_RANGE_PUSH("b200gsr.views.composite_bwd");
     rc = check_cuda(gsr_launch_composite_bwd(a), "composite_bwd");
     GSR_RANGE_POP();
@@ -521,21 +527,15 @@ int b200gsr_backward_views_ex(int32_t B, const b200gsr_params* prm, const b200gs
     int rc = check_views(B, prm, in);
     if (rc) return rc;
     return backward_views(B, prm, in, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes, max_pairs,
-                          out, flags, nullptr, stream);
+                          out, flags, nullptr, nullptr, stream);
 }
 
-int b200gsr_backward_views_frozen(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in,
-                                  const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
-                                  const float* dL_ddepth_alpha, void* saved, size_t saved_bytes, uint64_t max_pairs,
-                                  const b200gsr_view_grads* out, uint32_t flags, const b200gsr_row_range* frozen,
-                                  int32_t num_frozen, void* stream) {
-    int rc = check_views(B, prm, in);
-    if (rc) return rc;
+// The frozen ranges of b200gsr_backward_views_frozen / _stats: sorted, non-overlapping, non-empty ranges inside
+// [0, P); touching ones merge, and at most B200GSR_MAX_FROZEN_RANGES may remain.
+static int frozen_ranges(long long P, const b200gsr_row_range* frozen, int32_t num_frozen, GsrFrozenRanges& fr) {
     if (num_frozen < 0) return fail(B200GSR_ERR_BAD_ARG, "num_frozen %d is negative", num_frozen);
     if (num_frozen > 0 && !frozen) return fail(B200GSR_ERR_BAD_ARG, "frozen is null with num_frozen %d", num_frozen);
-    // sorted, non-overlapping, non-empty ranges inside [0, P); touching ones merge
-    GsrFrozenRanges fr{};
-    const long long P = prm[0].P;
+    fr = GsrFrozenRanges{};
     long long end = 0;
     for (int k = 0; k < num_frozen; ++k) {
         const long long lo = frozen[k].lo, len = frozen[k].len;
@@ -556,8 +556,70 @@ int b200gsr_backward_views_frozen(int32_t B, const b200gsr_params* prm, const b2
         }
         end = lo + len;
     }
+    return B200GSR_OK;
+}
+
+int b200gsr_backward_views_frozen(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in,
+                                  const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
+                                  const float* dL_ddepth_alpha, void* saved, size_t saved_bytes, uint64_t max_pairs,
+                                  const b200gsr_view_grads* out, uint32_t flags, const b200gsr_row_range* frozen,
+                                  int32_t num_frozen, void* stream) {
+    int rc = check_views(B, prm, in);
+    if (rc) return rc;
+    GsrFrozenRanges fr;
+    if ((rc = frozen_ranges(prm[0].P, frozen, num_frozen, fr))) return rc;
     return backward_views(B, prm, in, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes, max_pairs,
-                          out, flags, fr.n > 0 ? &fr : nullptr, stream);
+                          out, flags, fr.n > 0 ? &fr : nullptr, nullptr, stream);
+}
+
+int b200gsr_backward_views_stats(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in,
+                                 const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
+                                 const float* dL_ddepth_alpha, void* saved, size_t saved_bytes, uint64_t max_pairs,
+                                 const b200gsr_view_grads* out, uint32_t flags, const b200gsr_row_range* frozen,
+                                 int32_t num_frozen, const b200gsr_row_stats* stats, int32_t num_stats,
+                                 int32_t stats_view, void* stream) {
+    int rc = check_views(B, prm, in);
+    if (rc) return rc;
+    GsrFrozenRanges fr;
+    if ((rc = frozen_ranges(prm[0].P, frozen, num_frozen, fr))) return rc;
+    if (stats_view < -1 || stats_view >= B)
+        return fail(B200GSR_ERR_BAD_ARG, "stats_view %d is outside [-1, B = %d)", stats_view, B);
+    if (num_stats < 0 || num_stats > B200GSR_MAX_GROUPS)
+        return fail(B200GSR_ERR_BAD_ARG, "num_stats %d is outside [0, %d]", num_stats, B200GSR_MAX_GROUPS);
+    if (num_stats > 0 && !stats) return fail(B200GSR_ERR_BAD_ARG, "stats is null with num_stats %d", num_stats);
+    // sorted, non-overlapping, non-empty records inside [0, P), none overlapping a frozen range; the records that
+    // gather nothing are dropped
+    GsrRowStats rs{};
+    rs.view = stats_view;
+    const long long P = prm[0].P;
+    long long end = 0;
+    for (int k = 0; k < num_stats; ++k) {
+        const b200gsr_row_stats& r = stats[k];
+        const long long lo = r.lo, len = r.len;
+        if (len <= 0) return fail(B200GSR_ERR_BAD_ARG, "stats record %d is empty (len %lld)", k, len);
+        if (lo < 0 || lo + len > P)
+            return fail(B200GSR_ERR_BAD_ARG, "stats record %d [%lld, %lld) is outside [0, P = %lld)", k, lo, lo + len, P);
+        if (k > 0 && lo < end)
+            return fail(B200GSR_ERR_BAD_ARG, "stats record %d starts at %lld, before the end %lld of record %d: records "
+                        "must be sorted and must not overlap", k, lo, end, k - 1);
+        end = lo + len;
+        if ((r.xyz_gradient_accum != nullptr) != (r.denom != nullptr))
+            return fail(B200GSR_ERR_BAD_ARG, "stats record %d: xyz_gradient_accum and denom must both be set or both "
+                        "be null", k);
+        if (r.max_radii2D && !r.xyz_gradient_accum)
+            return fail(B200GSR_ERR_BAD_ARG, "stats record %d: max_radii2D without xyz_gradient_accum and denom", k);
+        for (int j = 0; j < fr.n; ++j)
+            if (lo < (long long)fr.lo[j] + fr.len[j] && (long long)fr.lo[j] < lo + len)
+                return fail(B200GSR_ERR_BAD_ARG, "stats record %d [%lld, %lld) overlaps the frozen rows [%u, %u): a "
+                            "frozen row would still count in denom", k, lo, lo + len, fr.lo[j], fr.lo[j] + fr.len[j]);
+        if (!r.xyz_gradient_accum) continue;
+        rs.lo[rs.n] = (uint32_t)lo; rs.len[rs.n] = (uint32_t)len;
+        rs.accum[rs.n] = r.xyz_gradient_accum; rs.denom[rs.n] = r.denom; rs.max_radii[rs.n] = r.max_radii2D;
+        ++rs.n;
+    }
+    if (rs.n == 0) rs.view = -1;        // nothing gathers: only the launches without d_means2D run the STATS kernels
+    return backward_views(B, prm, in, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes, max_pairs,
+                          out, flags, fr.n > 0 ? &fr : nullptr, &rs, stream);
 }
 
 int b200gsr_backward_views(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in, const int32_t* radii,

@@ -6,6 +6,7 @@
 
 #include "../../include/b200gsr_reserve.h"
 #include "../../include/b200gsr_views_frozen.h"
+#include "../../include/b200gsr_views_stats.h"
 
 #define GSR_TILE 16
 #define GSR_NEAR_Z 0.2f
@@ -290,6 +291,19 @@ struct GsrFrozenRanges {
     uint32_t lo[B200GSR_MAX_FROZEN_RANGES], len[B200GSR_MAX_FROZEN_RANGES];
 };
 
+// Densification statistics of a multi-view backward (b200gsr_backward_views_stats): n sorted, non-overlapping,
+// non-empty row ranges [lo, lo + len) of one view's P rows with their destinations (accum null = the record gathers
+// nothing; max_radii may be null), and the view whose launch gathers (-1 = none).  project_bwd runs its packed STATS
+// instantiation in that launch, and in every launch whose d_means2D is null.
+struct GsrRowStats {
+    int n;
+    int32_t view;
+    uint32_t lo[B200GSR_MAX_GROUPS], len[B200GSR_MAX_GROUPS];
+    float* accum[B200GSR_MAX_GROUPS];
+    float* denom[B200GSR_MAX_GROUPS];
+    float* max_radii[B200GSR_MAX_GROUPS];
+};
+
 struct GsrBwdArgs {
     b200gsr_params prm;
     const float *means3D, *shs, *colors, *opac, *scales, *rots, *cov3d;
@@ -310,6 +324,7 @@ struct GsrBwdArgs {
     cudaStream_t stream;
     const GsrScene* scene;       // scene render: leaf gradients of the raw parameters (null otherwise)
     const GsrFrozenRanges* frozen_rows;   // b200gsr_backward_views_frozen with ranges (null otherwise)
+    const GsrRowStats* row_stats;         // b200gsr_backward_views_stats (null otherwise)
 };
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device) instead of on every

@@ -275,6 +275,13 @@ struct SceneFrozen : S { uint32_t frozen; };
 // FROZEN without RAW, the packed-input backward with frozen rows (b200gsr_backward_views_frozen): the caller's frozen
 // row ranges of one view.  Derived from NoScene, whose fields (none) the default statements read.
 struct RowsFrozen : NoScene { GsrFrozenRanges rows; };
+// STATS without RAW, the packed-input backward with the densification statistics (b200gsr_backward_views_stats): the
+// records' row ranges and destinations, the view whose launch gathers (st.view), and this launch's view.  Derived from
+// RowsFrozen whatever FROZEN is (rows.n = 0 when nothing is frozen).
+struct RowsStats : RowsFrozen {
+    GsrRowStats st;
+    int32_t view;
+};
 // STATS (with RAW): the densification statistics of b200gsr_backward_scene[_dyn]_stats.  Per group the destinations
 // (accum null = the group gathers nothing; max_radii may be null), and the view whose launch gathers: `view` by value,
 // or *view_dev under DYN (null = none).  Derived from SceneFrozen whatever FROZEN is.
@@ -296,7 +303,7 @@ using FwdSceneLive = std::conditional_t<LIVE, SceneLive<SceneFwdDyn>, FwdScene<R
 // project_bwd_kernel's argument type for each mode.
 template <bool RAW, bool DYN, bool FROZEN, bool STATS, bool LIVE>
 using BwdScene = std::conditional_t<
-    STATS, std::conditional_t<LIVE, SceneLive<SceneStats<DYN>>, SceneStats<DYN>>,
+    STATS, std::conditional_t<RAW, std::conditional_t<LIVE, SceneLive<SceneStats<DYN>>, SceneStats<DYN>>, RowsStats>,
     std::conditional_t<
         RAW, std::conditional_t<FROZEN, SceneFrozen<std::conditional_t<DYN, SceneBwdDyn, SceneBwd>>,
                                 std::conditional_t<DYN, SceneBwdDyn, SceneBwd>>,
@@ -343,7 +350,7 @@ __device__ __forceinline__ ViewNoise view_noise(const S& sc, b200gsr_params& p) 
 // inputs; a loop over the ranges in use, as composite_bwd's row_frozen).  A constant false otherwise.
 template <bool FROZEN, typename S>
 __device__ __forceinline__ bool frozen_row(const S& sc, bool active, int i) {
-    if constexpr (FROZEN && std::is_same_v<S, RowsFrozen>) {
+    if constexpr (FROZEN && std::is_base_of_v<RowsFrozen, S>) {
         if (!active) return false;
 #pragma unroll 1
         for (int k = 0; k < sc.rows.n; ++k)
@@ -693,6 +700,9 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
 // may be null (nothing stored), and in the launch of the statistics view (sc.st) each visible row of a group with
 // statistics adds its screen-space gradient's norm, 1 and its radius to the group's accum / denom / max_radii row -
 // the arithmetic of densify_stats_kernel on the d_means2D row this launch computes.  One thread per row: no atomics.
+// STATS without RAW (b200gsr_backward_views_stats): d_means2D may be null, and in the launch of the statistics view
+// (sc.st.view == sc.view) each visible row inside one of the records adds the same three values to the record's row
+// (row - lo); the thread that computed the row's screen-space gradient does it, so again no atomics.
 // LIVE (with STATS and DYN, b200gsr_backward_scene_dyn_live): dead rows get zero gradients and no statistics, and
 // read no leaf.
 // S is the mode's BwdScene: a template parameter, so that `sc` has a dependent type and the statements of the other
@@ -1077,7 +1087,27 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
     if (active) {
         GSR_OUT(d_means3D + 3 * (size_t)i, dmean[0], 1); GSR_OUT(d_means3D + 3 * (size_t)i + 1, dmean[1], 1);
         GSR_OUT(d_means3D + 3 * (size_t)i + 2, dmean[2], 1);
-        d_means2D[3 * (size_t)i] = dm2[0]; d_means2D[3 * (size_t)i + 1] = dm2[1]; d_means2D[3 * (size_t)i + 2] = 0.f;
+        if (!STATS || d_means2D != nullptr) {
+            d_means2D[3 * (size_t)i] = dm2[0]; d_means2D[3 * (size_t)i + 1] = dm2[1]; d_means2D[3 * (size_t)i + 2] = 0.f;
+        }
+        if constexpr (STATS && !RAW) {
+            // visible = radii > 0 (no record overlaps a frozen range: refused on the host); the records are sorted
+            // and disjoint, so at most one holds row i
+            if (vis && sc.st.view == sc.view) {
+#pragma unroll 1
+                for (int k = 0; k < sc.st.n; ++k) {
+                    const uint32_t loc = (uint32_t)i - sc.st.lo[k];
+                    if (loc < sc.st.len[k]) {
+                        const int r = __ldg(radii + rec_base + i);
+                        sc.st.accum[k][loc] += gsr_screen_grad_norm(dm2[0], dm2[1]);
+                        sc.st.denom[k][loc] += 1.0f;
+                        float* pm = sc.st.max_radii[k];
+                        if (pm != nullptr) pm[loc] = fmaxf(pm[loc], (float)r);
+                        break;
+                    }
+                }
+            }
+        }
         GSR_OUT(d_opac + i, dop, 2);
         if (cov3d != nullptr) {
 #pragma unroll
@@ -1262,7 +1292,11 @@ static void launch_project_bwd(const GsrBwdArgs& a, int g_begin, int g_end, size
     if constexpr (DYN) sc.dyn = SceneDyn{a.scene->dyn_views, a.scene->dyn_seed};
     if constexpr (RAW && (FROZEN || STATS)) sc.frozen = a.scene->frozen;
     if constexpr (!RAW && FROZEN) sc.rows = *a.frozen_rows;
-    if constexpr (STATS) {
+    if constexpr (!RAW && STATS) {
+        sc.st = *a.row_stats;
+        sc.view = a.view;
+    }
+    if constexpr (RAW && STATS) {
         const GsrScene& s = *a.scene;
         for (int g = 0; g < s.num_groups && s.stats; ++g) {
             sc.st.accum[g] = s.stats[g].xyz_gradient_accum;
@@ -1301,6 +1335,15 @@ cudaError_t gsr_launch_project_bwd(const GsrBwdArgs& a) {
     else if (a.scene && frozen) launch_project_bwd<0, true, false, true>(a, g_begin, g_end, smem);
     else if (a.scene && a.scene->dyn_views) launch_project_bwd<0, true, true>(a, g_begin, g_end, smem);
     else if (a.scene) launch_project_bwd<0, true>(a, g_begin, g_end, smem);
+    else if (a.row_stats && (a.view == a.row_stats->view || !a.d_means2D)) {
+        // b200gsr_backward_views_stats: the launch that gathers, and every launch that stores no d_means2D
+        if (a.frozen_rows && a.shs && a.prm.M == 16) launch_project_bwd<16, false, false, true, true>(a, g_begin, g_end, smem);
+        else if (a.frozen_rows && a.shs && a.prm.M == 4) launch_project_bwd<4, false, false, true, true>(a, g_begin, g_end, smem);
+        else if (a.frozen_rows) launch_project_bwd<0, false, false, true, true>(a, g_begin, g_end, smem);
+        else if (a.shs && a.prm.M == 16) launch_project_bwd<16, false, false, false, true>(a, g_begin, g_end, smem);
+        else if (a.shs && a.prm.M == 4) launch_project_bwd<4, false, false, false, true>(a, g_begin, g_end, smem);
+        else launch_project_bwd<0, false, false, false, true>(a, g_begin, g_end, smem);
+    }
     else if (a.frozen_rows && a.shs && a.prm.M == 16) launch_project_bwd<16, false, false, true>(a, g_begin, g_end, smem);
     else if (a.frozen_rows && a.shs && a.prm.M == 4) launch_project_bwd<4, false, false, true>(a, g_begin, g_end, smem);
     else if (a.frozen_rows) launch_project_bwd<0, false, false, true>(a, g_begin, g_end, smem);

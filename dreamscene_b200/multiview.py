@@ -19,6 +19,11 @@ any other row, but the backward computes no gradient for them: their gradient ro
 the other rows' gradients are those of the call without ``frozen_rows`` (bit for bit in deterministic mode).
 ``scene.frozen_rows(groups, frozen)`` gives the ranges of frozen parameter groups packed by ``scene.assemble_scene``.
 
+Densification statistics: ``densify_stats=[(lo, hi, xyz_gradient_accum, denom, max_radii2D or None), ...]`` makes the
+backward do the reference's add_densification_stats for rows [lo, hi) of view ``stats_view`` itself, in place, in the
+launch that computes that view's screen-space gradient.  Without ``means2D`` no screen-space gradient is then stored
+at all.  ``scene.stats_rows(groups, stats)`` gives the records of the groups packed by ``scene.assemble_scene``.
+
 Every tensor argument is either ONE tensor (shared by all views) or a list of B tensors (per-view
 values, e.g. the separately augmented shs / scales of scene_render); `settings_list` holds the B
 GaussianRasterizationSettings (cameras, sh_degree, scale_modifier, bg may differ; image size and
@@ -71,10 +76,53 @@ def _frozen_ranges(frozen_rows, P: int):
     return tuple(out)
 
 
+def _stats_records(densify_stats, P: int, dev, frozen):
+    """None or [(lo, hi, accum, denom, max_radii2D or None), ...] -> the validated (lo, len, accum, denom, max_radii2D)
+    records that b200gsr_backward_views_stats takes.  Refuses what the library refuses - an empty, out-of-bounds,
+    unsorted or overlapping record, more than MAX_GROUPS records, a record that overlaps the merged frozen ranges
+    `frozen` - and statistics tensors that are not contiguous float32 tensors of hi - lo elements on `dev`."""
+    if densify_stats is None:
+        return None
+    out: list = []
+    end = 0
+    entries = list(densify_stats)
+    if len(entries) > _lib.MAX_GROUPS:
+        raise ValueError(f"densify_stats: {len(entries)} records, at most {_lib.MAX_GROUPS}")
+    for k, e in enumerate(entries):
+        if len(e) != 5 or e[2] is None or e[3] is None:
+            raise ValueError(f"densify_stats[{k}] must be (lo, hi, xyz_gradient_accum, denom, max_radii2D or None)")
+        lo, hi = int(e[0]), int(e[1])
+        if hi <= lo:
+            raise ValueError(f"densify_stats[{k}] = ({lo}, {hi}) is empty")
+        if lo < 0 or hi > P:
+            raise ValueError(f"densify_stats[{k}] = ({lo}, {hi}) is outside [0, P = {P})")
+        if k > 0 and lo < end:
+            raise ValueError(f"densify_stats[{k}] = ({lo}, {hi}) starts before the end {end} of densify_stats[{k - 1}]: "
+                             "the records must be sorted and must not overlap")
+        end = hi
+        for flo, flen in frozen:
+            if lo < flo + flen and flo < hi:
+                raise ValueError(f"densify_stats[{k}] = ({lo}, {hi}) overlaps the frozen rows ({flo}, {flo + flen}): "
+                                 "the reference gathers statistics for the trained rows only")
+        for name, t in zip(("xyz_gradient_accum", "denom", "max_radii2D"), e[2:]):
+            if t is None:
+                continue
+            if not torch.is_tensor(t) or t.dtype != torch.float32 or not t.is_contiguous():
+                raise ValueError(f"densify_stats[{k}] {name} must be a contiguous float32 tensor")
+            if t.numel() != hi - lo:
+                raise ValueError(f"densify_stats[{k}] {name} has {t.numel()} elements, rows ({lo}, {hi}) are {hi - lo}")
+            if t.device != dev:
+                raise ValueError(f"densify_stats[{k}] {name} must be on the inputs' device ({dev})")
+        out.append((lo, hi - lo, e[2], e[3], e[4]))
+    return tuple(out)
+
+
 class _RasterizeViews(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, settings, spec, B, frozen, *flat):
-        # spec[name] = None | ("shared", idx) | ("list", [idx...]) into `flat`; flat also holds the B means2D ports last
+    def forward(ctx, settings, spec, B, frozen, stats, ports, *flat):
+        # spec[name] = None | ("shared", idx) | ("list", [idx...]) into `flat`; flat also holds the `ports` means2D
+        # ports last: B, or 0 when `stats` = (records, view) is given without them (then no screen-space gradient is
+        # stored)
         lib = _lib.load()
         tensors = [_lib.prepare(t) for t in flat]
         get = lambda name, v: None if spec[name] is None else tensors[spec[name][1] if spec[name][0] == "shared" else spec[name][1][v]]
@@ -114,6 +162,8 @@ class _RasterizeViews(torch.autograd.Function):
             saved, cap = R._issue_with_capacity(d, (B, P, H, W), B * P, Hs, W, with_backward, det, score, launch, capturing,
                                                 stream.value)
         ctx.meta = (spec, B, P, W, Hs, cap, with_backward, len(flat), det, frozen)
+        ctx.stats = stats
+        ctx.ports = ports
         ctx.views = (prm, vin)            # the backward reuses the arrays; `keep` holds their device constants
         ctx.keep = keep
         ctx.saved_buf = saved
@@ -139,7 +189,7 @@ class _RasterizeViews(torch.autograd.Function):
         g_color = torch.zeros(3, Hs, W, device=dev) if g_color is None else _lib.prepare(g_color)
         g_da = torch.zeros(2, Hs, W, device=dev) if g_da is None else _lib.prepare(g_da)
         grads: List[Optional[torch.Tensor]] = [None] * nflat
-        m2d_base = nflat - B
+        m2d_base = nflat - ctx.ports
         with torch.cuda.device(dev):
             out = (_lib.ViewGrads * B)()
             for v in range(B):
@@ -154,33 +204,55 @@ class _RasterizeViews(torch.autograd.Function):
                     else:
                         acc |= _ACC_BIT[name]                      # shared with an earlier view: accumulate in the kernel
                     setattr(out[v], _GRAD_FIELD[name], grads[idx].data_ptr())
-                g2 = torch.empty(P, 3, dtype=torch.float32, device=dev)
-                grads[m2d_base + v] = g2
-                out[v].d_means2D = g2.data_ptr()
+                if ctx.ports:
+                    g2 = torch.empty(P, 3, dtype=torch.float32, device=dev)
+                    grads[m2d_base + v] = g2
+                    out[v].d_means2D = g2.data_ptr()
                 out[v].accumulate = acc
             ptr = _lib.ptr
             args = (B, prm, vin, ptr(radii), ptr(depth_alpha), ptr(g_color), ptr(g_da), ptr(ctx.saved_buf),
                     ctx.saved_buf.numel(), cap, out, _lib.BWD_DETERMINISTIC if det else 0)
-            if frozen:
-                ranges = (_lib.RowRange * len(frozen))(*[_lib.RowRange(lo, n) for lo, n in frozen])
+            ranges = (_lib.RowRange * len(frozen))(*[_lib.RowRange(lo, n) for lo, n in frozen]) if frozen else None
+            if ctx.stats is not None:
+                records, view = ctx.stats
+                rec = (_lib.RowStats * len(records))(*[_lib.RowStats(lo, n, *[ptr(t) for t in ts])
+                                                       for lo, n, *ts in records]) if records else None
+                name = "b200gsr_backward_views_stats"
+                rc = lib.b200gsr_backward_views_stats(*args, ranges, len(frozen), rec, len(records), view,
+                                                      _lib.stream(dev))
+            elif frozen:
+                name = "b200gsr_backward_views_frozen"
                 rc = lib.b200gsr_backward_views_frozen(*args, ranges, len(frozen), _lib.stream(dev))
             else:
+                name = "b200gsr_backward_views"
                 rc = lib.b200gsr_backward_views_ex(*args, _lib.stream(dev))
-        _lib.check(rc, "b200gsr_backward_views_frozen" if frozen else "b200gsr_backward_views")
-        return (None, None, None, None) + tuple(grads)
+        _lib.check(rc, name)
+        return (None,) * 6 + tuple(grads)
 
 
 def rasterize_views(settings: Sequence[R.GaussianRasterizationSettings], means3D: TensorOrList, opacities: TensorOrList,
                     shs: TensorOrList = None, colors_precomp: TensorOrList = None, scales: TensorOrList = None,
                     rotations: TensorOrList = None, cov3D_precomp: TensorOrList = None,
                     means2D: Optional[Sequence[torch.Tensor]] = None,
-                    frozen_rows: Optional[Sequence[Sequence[int]]] = None):
+                    frozen_rows: Optional[Sequence[Sequence[int]]] = None,
+                    densify_stats: Optional[Sequence] = None, stats_view: int = -1):
     """-> list of B tuples (color[3,H,W], radii[P], depth_alpha[2,H,W]) (score first when score_flag), views
     into the stacked outputs.  means2D: optional list of B [P,3] tensors whose .grad receives the per-view
     screen-space gradients (the reference's viewspace_points).  frozen_rows: None, or sorted, non-overlapping,
     non-empty (lo, hi) ranges of the P rows (at most MAX_FROZEN_RANGES once touching ones merge) whose gradient the
     backward does not compute: their rows of every input's gradient and of the means2D gradients are zeros, and the
-    other rows get the gradients of the call without frozen_rows."""
+    other rows get the gradients of the call without frozen_rows.
+
+    densify_stats: None, or sorted, non-overlapping, non-empty records (lo, hi, xyz_gradient_accum, denom, max_radii2D
+    or None) of the P rows (at most MAX_GROUPS, none overlapping frozen_rows), each tensor a contiguous float32 tensor
+    of hi - lo elements on the inputs' device.  The backward then does the reference's add_densification_stats for
+    view `stats_view` inside the render backward, in place: for each row of a record whose radius in that view is
+    positive, xyz_gradient_accum[row - lo] += |screen-space gradient[:2]|, denom[row - lo] += 1, max_radii2D[row - lo]
+    = max(max_radii2D[row - lo], radius) - bit for bit what densify.add_densification_stats does with that view's
+    means2D gradient and radii.  Each backward adds once (a retain_graph second backward adds again); no backward, no
+    statistics.  Without means2D no screen-space gradient is stored at all; with it both are produced.
+    scene.stats_rows(groups, stats) gives the records of assemble_scene's packed groups.
+    stats_view: the view whose statistics are gathered: -1 (default) is the last view, B - 1, as render_scene's."""
     B = len(settings)
     if not 1 <= B <= _lib.MAX_VIEWS:
         raise ValueError(f"need 1..{_lib.MAX_VIEWS} views")
@@ -206,8 +278,9 @@ def rasterize_views(settings: Sequence[R.GaussianRasterizationSettings], means3D
     P = int((means3D if torch.is_tensor(means3D) else means3D[0]).shape[0])
     dev = (means3D if torch.is_tensor(means3D) else means3D[0]).device
     if means2D is None:
-        means2D = [torch.zeros(P, 3, device=dev) for _ in range(B)]
-    if len(means2D) != B:
+        # with densify_stats no port is needed: the backward then writes no screen-space gradient
+        means2D = [] if densify_stats is not None else [torch.zeros(P, 3, device=dev) for _ in range(B)]
+    elif len(means2D) != B:
         raise ValueError(f"means2D: expected {B} per-view tensors")
     flat.extend(means2D)
     H = int(settings[0].image_height)
@@ -215,7 +288,13 @@ def rasterize_views(settings: Sequence[R.GaussianRasterizationSettings], means3D
         if int(s.image_height) != H or int(s.image_width) != int(settings[0].image_width) or bool(s.score_flag) != bool(settings[0].score_flag):
             raise ValueError("all views must share the image size and score_flag")
     frozen = _frozen_ranges(frozen_rows, P)
-    res = _RasterizeViews.apply(tuple(settings), spec, B, frozen, *flat)
+    stats = None
+    if densify_stats is not None:
+        sv = int(stats_view)
+        if not -1 <= sv < B:
+            raise ValueError(f"rasterize_views: stats_view must be -1 (the last view) or in 0..{B - 1}, got {stats_view}")
+        stats = (_stats_records(densify_stats, P, dev, frozen), B - 1 if sv == -1 else sv)
+    res = _RasterizeViews.apply(tuple(settings), spec, B, frozen, stats, len(means2D), *flat)
     color, radii, da = res[0], res[1], res[2]
     Hp = color.shape[1] // B
     outs = []

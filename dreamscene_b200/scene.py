@@ -29,7 +29,8 @@ Noise modes
 
 Frozen groups: ``assemble_scene(groups, frozen=[...])`` gives a frozen group's leaves no gradient, and
 ``rasterize_views(..., frozen_rows=frozen_rows(groups, frozen))`` skips their packed rows' gradient work, so a stage
-that trains one group pays for the backward of that group only.
+that trains one group pays for the backward of that group only.  ``rasterize_views(..., densify_stats=stats_rows(groups,
+stats))`` gathers the trained groups' densification statistics inside that backward, as render_scene's densify_stats.
 
 ``render_scene(groups, settings_list, ...)`` goes one step further: the B views of a training step rendered straight
 from the raw groups, with the activations and the Philox augmentation inside the projection kernels (no augmented copy
@@ -181,6 +182,23 @@ def frozen_rows(groups: Sequence, frozen: Sequence[bool] | None):
                 out[-1] = (out[-1][0], row + n)
             else:
                 out.append((row, row + n))
+        row += n
+    return out
+
+
+def stats_rows(groups: Sequence, stats: Sequence):
+    """The densification statistics records of the packed rows - `stats` holds, in assemble_scene's order, one entry
+    per group: None, or the reference's (xyz_gradient_accum, denom, max_radii2D or None) of that group - as the
+    sorted (lo, hi, xyz_gradient_accum, denom, max_radii2D) records that rasterize_views(densify_stats=) takes.  The
+    tensors are the group's own (float32, contiguous, one element per row), updated in place by the backward.  Empty
+    groups take no rows and give no record.  [] when no group gathers."""
+    entries = _densify_stats(stats, groups, 0, "stats_rows")
+    out: list = []
+    row = 0
+    for g, e in zip(groups, entries or ()):
+        n = int(_get(g, "_xyz").shape[0])
+        if n > 0 and e is not None:
+            out.append((row, row + n) + tuple(e))
         row += n
     return out
 
