@@ -3,7 +3,7 @@
 all of them, with the frozen groups' backward skipped (frozen=) against the plain backward that computes every
 group's gradients and steps only the trained groups' optimizers.
 
-Layout: benchmarks/scene_step.py::build_scene (env 2.0 M, floor 0.3 M, 4 objects of 0.08 M; M = 4, sh_degree 1),
+Layout: harness/room.py::build_scene (env 2.0 M, floor 0.3 M, 4 objects of 0.08 M; M = 4, sh_degree 1),
 4 views of 512 x 512.  Configurations, after DreamScene's scene stages:
   all   : every group trains (scene_optim); frozen=[False] * 6 is the plain backward
   env   : stage 1, only env trains

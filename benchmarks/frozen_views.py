@@ -2,7 +2,7 @@
 """Frozen groups on the two-step scene route: assemble_scene(frozen=) + rasterize_views(frozen_rows=) against the same
 two ops without freezing, forward + backward of one training step's views.
 
-Layout: benchmarks/scene_step.py::build_scene (env 2.0 M, floor 0.3 M, 4 objects of 0.08 M; M = 4, sh_degree 1),
+Layout: harness/room.py::build_scene (env 2.0 M, floor 0.3 M, 4 objects of 0.08 M; M = 4, sh_degree 1),
 4 views of 512 x 512 inside the room, SH and scale augmentation on in every view.  Configurations, after DreamScene's
 scene stages (benchmarks/frozen_step.py):
   all   : every group trains; frozen = [False] * 6, which runs the plain kernels

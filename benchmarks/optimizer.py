@@ -4,7 +4,7 @@ dreamscene_b200.GaussianAdam on two parameter layouts, timed in one process with
 
   object : one GaussianModel of 1.2 M Gaussians at M = 16 with the reference's seven groups (background without a
            gradient, as in training): 59 floats per Gaussian, 70.8 M elements per step.
-  scene  : the scene of benchmarks/scene_step.py (walls + ceiling, floor, four objects; 2.63 M Gaussians, M = 4),
+  scene  : the scene of harness/room.py (walls + ceiling, floor, four objects; 2.63 M Gaussians, M = 4),
            one optimizer per GaussianModel as in the reference: six step() calls per training step.
 
 Each variant owns a copy of the parameters, moments and (fixed, random) gradients.  One repetition times --steps
@@ -43,7 +43,7 @@ def object_models(dev, P=1_200_000, M=16):
 
 
 def scene_models(dev):
-    from scene_step import build_scene
+    from harness.room import build_scene
     shapes = [{k: tuple(v.shape) for k, v in g.items()} for g in build_scene(dev)]
     for s in shapes:
         s["background"] = (3, 1, 1)

@@ -10,7 +10,7 @@ and StepGraph in target mode (the loss inside the render graph).
 The pseudo ground truth is G = 18 float16 images of 512 x 512 (the object stage's 18 views).  Every step changes the
 camera, the target index and the xyz lr, as the refine loop does.  Layouts (benchmarks/scene_render.py):
   object : 1.2 M Gaussians in one group, M = 16
-  scene  : benchmarks/scene_step.py::build_scene (cfg5: 2.63 M Gaussians in 6 groups, M = 4)
+  scene  : harness/room.py::build_scene (cfg5: 2.63 M Gaussians in 6 groups, M = 4)
 
 Per variant, alternating the variants in rounds:
   sync_ms    : median wall time of one step followed by torch.cuda.synchronize()

@@ -7,7 +7,7 @@
 
 Both with SH and scale augmentation on in every view and the same seed, so both render the same images.  Layouts:
   object : 1.2 M Gaussians in one group, M = 16 (sh_degree 3), 4 views of 512 x 512 (object_render)
-  scene  : benchmarks/scene_step.py::build_scene (2.63 M Gaussians in 6 groups, M = 4, sh_degree 1), 4 views of
+  scene  : harness/room.py::build_scene (2.63 M Gaussians in 6 groups, M = 4, sh_degree 1), 4 views of
            512 x 512 inside the room (scene_render)
 
 Per layout the variants alternate step by step; a step is timed with CUDA events from the first op of the forward
@@ -34,8 +34,7 @@ sys.path.insert(0, HERE)
 from dreamscene_b200 import GaussianRasterizationSettings, _lib  # noqa: E402
 from dreamscene_b200.multiview import rasterize_views  # noqa: E402
 from dreamscene_b200.scene import assemble_scene, render_scene  # noqa: E402
-from harness import cameras  # noqa: E402
-import scene_step  # noqa: E402
+from harness import cameras, room  # noqa: E402
 
 NAMES = ("_xyz", "_opacity", "_scaling", "_rotation", "_features_dc", "_features_rest")
 
@@ -44,18 +43,15 @@ def object_layout(dev, P=1_200_000, M=16, seed=0):
     rng = np.random.RandomState(seed)
     d = rng.normal(size=(P, 3)); d /= np.linalg.norm(d, axis=1, keepdims=True)
     xyz = 0.5 * np.cbrt(rng.random_sample((P, 1))) * d
-    g = scene_step.make_group(xyz, rng, M, dev, scale=0.004)
-    group = {"_xyz": g["xyz"], "_opacity": g["opacity"], "_scaling": g["scaling"], "_rotation": g["rotation"],
-             "_features_dc": g["f_dc"], "_features_rest": g["f_rest"]}
+    group = room.named_groups([room.make_group(xyz, rng, M, dev, scale=0.004)])[0]
     cams = lambda it: [cameras.orbit_camera(radius=2.5, theta_deg=60.0 + 10 * math.sin(it + k), phi_deg=90.0 * k + 13 * it,
                                             fovx=0.8, height=512, width=512, device=dev) for k in range(4)]
     return [group], cams, 3
 
 
 def scene_layout(dev):
-    groups = [{"_xyz": g["xyz"], "_opacity": g["opacity"], "_scaling": g["scaling"], "_rotation": g["rotation"],
-               "_features_dc": g["f_dc"], "_features_rest": g["f_rest"]} for g in scene_step.build_scene(dev)]
-    cams = lambda it: [scene_step.scene_camera(it * 4 + k, 512, dev) for k in range(4)]
+    groups = room.named_groups(room.build_scene(dev))
+    cams = lambda it: [room.scene_camera(it * 4 + k, 512, dev) for k in range(4)]
     return groups, cams, 1
 
 

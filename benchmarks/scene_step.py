@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """BASELINE.json config 5 re-enactment: the call pattern of DreamScene's scene_train_step
 (/root/reference/training/scene_trainer.py:699-1080 -> scene_gaussian.py:673-893) with the SDS
-guidance replaced by an L2 loss, on a synthetic indoor scene built with the reference's init
-recipes (gs_renderer.py:218-248 walls, 279-296 floor; configs/scenes/sample_indoor.yaml box).
+guidance replaced by an L2 loss, on the synthetic indoor scene of harness/room.py, built with the
+reference's init recipes (gs_renderer.py:218-248 walls, 279-296 floor; configs/scenes/sample_indoor.yaml box).
 The reference modules cannot be imported on the GPU box (absent + missing deps), so the loop is
 restated here: per view  torch.cat(env, floor, objects) -> SH/scale augmentation -> rasterizer ->
 depth/alpha post-processing; 4 views per step (C_batch_size, config.py:163); one backward.
@@ -28,60 +28,8 @@ from dreamscene_b200 import GaussianRasterizationSettings, GaussianRasterizer  #
 from dreamscene_b200.multiview import rasterize_views  # noqa: E402
 from dreamscene_b200.postprocess import disparity_from_depth_alpha  # noqa: E402
 from dreamscene_b200.scene import assemble_scene, render_scene  # noqa: E402
-from harness import cameras  # noqa: E402
+from harness.room import build_scene, named_groups, scene_camera  # noqa: E402
 from harness.scene_ref import reference_assemble  # noqa: E402
-
-SH_C0 = 0.28209479177387814
-
-
-def plane_points(n, origin, u, v, rng):
-    a, b = rng.random_sample((n, 1)), rng.random_sample((n, 1))
-    return origin[None] + a * u[None] + b * v[None]
-
-
-def make_group(xyz, rng, M, dev, scale):
-    P = xyz.shape[0]
-    t = lambda a: torch.tensor(np.ascontiguousarray(a, dtype=np.float32), device=dev)
-    return dict(
-        xyz=t(xyz).requires_grad_(True),
-        f_dc=t((rng.random_sample((P, 1, 3)) - 0.5) / SH_C0).requires_grad_(True),
-        f_rest=t(rng.normal(0, 0.02, (P, M - 1, 3))).requires_grad_(True),
-        scaling=t(np.log(np.full((P, 3), scale) * np.exp(rng.normal(0, 0.2, (P, 3))))).requires_grad_(True),
-        rotation=t(np.tile([1.0, 0, 0, 0], (P, 1)) + rng.normal(0, 0.05, (P, 4))).requires_grad_(True),
-        opacity=t(np.full((P, 1), math.log(0.1 / 0.9))).requires_grad_(True))
-
-
-def build_scene(dev, M=4, n_wall=400_000, n_floor=300_000, n_obj=81_920, seed=0):
-    rng = np.random.RandomState(seed)
-    L, Wd, Hh = 6.0, 5.0, 2.8          # room box (m)
-    o = np.array([-L / 2, -Wd / 2, 0.0])
-    ex, ey, ez = np.array([L, 0, 0.0]), np.array([0, Wd, 0.0]), np.array([0, 0, Hh])
-    walls = [plane_points(n_wall, o, ex, ez, rng), plane_points(n_wall, o + ey, ex, ez, rng),
-             plane_points(n_wall, o, ey, ez, rng), plane_points(n_wall, o + ex, ey, ez, rng),
-             plane_points(n_wall, o + ez, ex, ey, rng)]                     # 4 walls + ceiling
-    env = make_group(np.concatenate(walls), rng, M, dev, scale=0.008)
-    floor = make_group(plane_points(n_floor, o, ex, ey, rng), rng, M, dev, scale=0.008)
-    objs = []
-    for c in ([1.0, 0.8, 0.5], [-1.2, -0.6, 0.4], [0.3, -1.3, 0.45], [-0.5, 1.2, 0.6]):
-        d = rng.normal(size=(n_obj, 3)); d /= np.linalg.norm(d, axis=1, keepdims=True)
-        xyz = np.array(c)[None] + 0.35 * np.cbrt(rng.random_sample((n_obj, 1))) * d
-        objs.append(make_group(xyz, rng, M, dev, scale=0.006))
-    return [env, floor] + objs
-
-
-def scene_camera(k, size, dev):
-    # camera inside the room, looking roughly horizontally (Stage1_Indoor-like), FoV 0.96
-    ang = 2 * math.pi * (k * 0.37 % 1.0)
-    eye = np.array([0.8 * math.cos(ang * 1.7), 0.6 * math.sin(ang * 1.3), 1.4], np.float32)
-    fwd = np.array([math.cos(ang), math.sin(ang), -0.1], np.float32); fwd /= np.linalg.norm(fwd)
-    up = np.array([0, 0, 1], np.float32)
-    right = np.cross(fwd, up); right /= np.linalg.norm(right)
-    up = np.cross(right, fwd)
-    pose = np.eye(4, dtype=np.float32)
-    pose[:3, :3] = np.stack((-right, up, -fwd), axis=-1)    # same axes convention as cameras.orbit_pose
-    pose[:3, 3] = eye
-    return cameras.camera_from_pose(pose, 0.96, size, size, device=dev)
-
 
 def render(groups, cam, dev, bg, aug=True, glue="torch"):
     """scene_gaussian.py:673-893 restated.  glue="torch": the reference's own PyTorch expressions
@@ -91,8 +39,7 @@ def render(groups, cam, dev, bg, aug=True, glue="torch"):
         image_height=cam.image_height, image_width=cam.image_width, tanfovx=cam.tanfovx, tanfovy=cam.tanfovy,
         bg=bg, scale_modifier=1.0, viewmatrix=cam.world_view_transform, projmatrix=cam.full_proj_transform,
         sh_degree=1, campos=cam.camera_center, prefiltered=False, score_flag=False)
-    named = [{"_xyz": g["xyz"], "_opacity": g["opacity"], "_scaling": g["scaling"], "_rotation": g["rotation"],
-              "_features_dc": g["f_dc"], "_features_rest": g["f_rest"]} for g in groups]
+    named = named_groups(groups)
     if glue == "torch":
         P = sum(g["xyz"].shape[0] for g in groups)
         M = 1 + groups[0]["f_rest"].shape[1]
@@ -129,8 +76,7 @@ def render_views(groups, cams, dev, bg, aug=True, scene=False):
     (in-kernel Philox noise), shared positions / opacities / rotations, batched fused disparity.  scene=True:
     dreamscene_b200.scene.render_scene renders them straight from the raw groups (the activations and the
     augmentation happen inside the projection kernels; the rasterizer time then includes them)."""
-    named = [{"_xyz": g["xyz"], "_opacity": g["opacity"], "_scaling": g["scaling"], "_rotation": g["rotation"],
-              "_features_dc": g["f_dc"], "_features_rest": g["f_rest"]} for g in groups]
+    named = named_groups(groups)
     if not scene:
         xyz, opacity, scales_v, rots, shs_v = assemble_scene(named, shs_aug=aug, scale_aug=aug, noise="fused",
                                                              views=len(cams))

@@ -18,7 +18,7 @@ lambda_tv 1, lambda_tv_depth 1 (object) / 0 (scene), lambda_scale 1 (object) / 0
 term of weight 0 (the reference computes 0 * tv_loss(depths)); reg leaves it out.  Every step changes the cameras,
 flags, seed and xyz lr.  Layouts as benchmarks/step_graph.py:
   object : 1.2 M Gaussians in one group, M = 16, 4 views of 512 x 512
-  scene  : benchmarks/scene_step.py::build_scene (cfg5: 2.63 M Gaussians in 6 groups, M = 4), 4 views of 512 x 512
+  scene  : harness/room.py::build_scene (cfg5: 2.63 M Gaussians in 6 groups, M = 4), 4 views of 512 x 512
 
 Per variant, alternating the variants in rounds:
   sync_ms    : median wall time of one step followed by torch.cuda.synchronize()

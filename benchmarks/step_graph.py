@@ -8,7 +8,7 @@
 The loss is an L2 against a fixed target, a total-variation term, a disparity term and the scale loss.  Both variants
 change the cameras, flags, seed and the xyz lr every step, as a schedule does.  Layouts (benchmarks/scene_render.py):
   object : 1.2 M Gaussians in one group, M = 16, 4 views of 512 x 512
-  scene  : benchmarks/scene_step.py::build_scene (cfg5: 2.63 M Gaussians in 6 groups, M = 4), 4 views of 512 x 512
+  scene  : harness/room.py::build_scene (cfg5: 2.63 M Gaussians in 6 groups, M = 4), 4 views of 512 x 512
 
 Per variant, alternating the variants in rounds:
   sync_ms    : median wall time of one step followed by torch.cuda.synchronize()

@@ -9,7 +9,7 @@
   render_frames : dreamscene_b200.video.render_frames (stacked forward-only passes of 16 views, frames quantised on
                   the device, copied into pinned memory while the next pass renders).
 
-Layouts (512 x 512): scene = benchmarks/scene_step.py::build_scene (cfg5: 2.63 M Gaussians in 6 groups, M = 4,
+Layouts (512 x 512): scene = harness/room.py::build_scene (cfg5: 2.63 M Gaussians in 6 groups, M = 4,
 sh_degree 1; cameras inside the room); object = benchmarks/scene_render.py::object_layout (1.2 M Gaussians, M = 16,
 sh_degree 3; orbit cameras).  Frame counts: 240 (one Circle(): 120 views around, 120 at 45 degrees) and 1440 (the
 scene's inference cameras with K = 5 objects, 240 (K + 1)); the 240 are the first 240 of the 1440.
@@ -42,9 +42,8 @@ sys.path.insert(0, os.path.dirname(HERE))
 sys.path.insert(0, HERE)
 from dreamscene_b200 import GaussianRasterizationSettings, GaussianRasterizer  # noqa: E402
 from dreamscene_b200.video import render_frames  # noqa: E402
-from harness import cameras, video_ref  # noqa: E402
+from harness import cameras, room, video_ref  # noqa: E402
 import scene_render  # noqa: E402
-import scene_step  # noqa: E402
 
 
 def card():
@@ -66,7 +65,7 @@ def circle(n, dev, radius=2.5):
 def layouts(dev, n):
     if "scene" in LAYOUTS:
         groups, _, deg = scene_render.scene_layout(dev)
-        yield "scene", groups, [scene_step.scene_camera(k, 512, dev) for k in range(n)], deg
+        yield "scene", groups, [room.scene_camera(k, 512, dev) for k in range(n)], deg
     if "object" in LAYOUTS:
         groups, _, deg = scene_render.object_layout(dev)
         cams = [c for r in range(n // 240) for c in circle(240, dev, radius=2.5 + 0.25 * r)]

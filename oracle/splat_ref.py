@@ -127,7 +127,11 @@ def preprocess(S: Settings, means3D, opacities, shs=None, colors_precomp=None, s
     """Per-Gaussian stage (SURVEY.md A.1-A.5).  Differentiable.  Returns a dict.
 
     ``decisions``: integer decisions (visible/radii/rect) from another run (used to evaluate
-    the fp64 gradient reference on exactly the fp32 pair lists)."""
+    the fp64 gradient reference on exactly the fp32 pair lists).  When they also hold the branch
+    flags ``in_x`` / ``in_y`` (EWA clamp) and ``clamped`` (SH colour clamp), those are used in
+    place of the flags this run would compute in its own dtype: a Gaussian whose t.x/t.z lies
+    within an ulp of the clamp limit, or whose colour lies within an ulp of 0, would otherwise take
+    the other gradient branch in fp64 (identity vs zero) than in the fp32 run it is compared with."""
     P = means3D.shape[0]
     H, W = int(S.image_height), int(S.image_width)
     V = S.viewmatrix.detach().to("cpu", dtype).reshape(16)
@@ -166,8 +170,11 @@ def preprocess(S: Settings, means3D, opacities, shs=None, colors_precomp=None, s
     with torch.no_grad():
         tz_safe = torch.where(tz == 0, torch.ones_like(tz), tz)
         txtz, tytz = tx / tz_safe, ty / tz_safe
-        in_x = (txtz >= -limx) & (txtz <= limx)
-        in_y = (tytz >= -limy) & (tytz <= limy)
+        if decisions is not None and "in_x" in decisions:
+            in_x, in_y = decisions["in_x"], decisions["in_y"]
+        else:
+            in_x = (txtz >= -limx) & (txtz <= limx)
+            in_y = (tytz >= -limy) & (tytz <= limy)
         cx_val = torch.minimum(limx, torch.maximum(-limx, txtz)) * tz
         cy_val = torch.minimum(limy, torch.maximum(-limy, tytz)) * tz
     # value = clamp(t.x/t.z)*t.z ; gradient = identity when unclamped, constant when clamped
@@ -226,14 +233,18 @@ def preprocess(S: Settings, means3D, opacities, shs=None, colors_precomp=None, s
         dn = torch.where(dn.detach() == 0, torch.ones_like(dn), dn)
         d = d / dn[:, None]
         raw = eval_sh_basis_dot(int(S.sh_degree), shs, d) + 0.5
-        clamped = (raw.detach() < 0)
-        rgb = torch.clamp_min(raw, 0.0)
+        if decisions is not None and decisions.get("clamped") is not None:
+            clamped = decisions["clamped"]
+        else:
+            clamped = (raw.detach() < 0)
+        # = clamp_min(raw, 0) in value and gradient when `clamped` is this run's own mask
+        rgb = torch.where(clamped, torch.zeros_like(raw), raw)
     else:
         rgb = colors_precomp
 
     return dict(depth=tz, px=px, py=py, conic=(con_a, con_b, con_c), opacity=opacities.reshape(P),
                 rgb=rgb, cov2d=(a, b, c), cov3D=cov3D, radii=radii, rect=rect, touched=touched,
-                visible=visible, clamped=clamped, grid=(gx, gy))
+                visible=visible, in_x=in_x, in_y=in_y, clamped=clamped, grid=(gx, gy))
 
 
 def bin_and_sort(pre, S: Settings):
@@ -367,7 +378,9 @@ def rasterize(S: Settings, means3D, opacities, shs=None, colors_precomp=None, sc
     """Full forward.  Returns dict(color, depth_alpha, radii, score, + intermediates).
 
     ``decisions`` (optional) = {'visible','radii','rect','touched','point_list','ranges'} from a
-    previous fp32 run; lets an fp64 run use the bit-exact fp32 pair lists."""
+    previous fp32 run; lets an fp64 run use the bit-exact fp32 pair lists.  The decisions this
+    returns also carry the branch flags 'in_x', 'in_y' and 'clamped' (see ``preprocess``), so an
+    fp64 run given them takes the fp32 run's gradient branch on every Gaussian."""
     if (shs is None) == (colors_precomp is None):
         raise Exception("Please provide excatly one of either SHs or precomputed colors!")
     if ((scales is None or rotations is None) and cov3D_precomp is None) or \
@@ -388,4 +401,5 @@ def rasterize(S: Settings, means3D, opacities, shs=None, colors_precomp=None, sc
                 n_contrib=ncon, keys=keys, point_list=point_list, ranges=ranges, pre=pre,
                 decisions=dict(visible=pre["visible"], radii=pre["radii"], rect=pre["rect"],
                                touched=pre["touched"], point_list=point_list, ranges=ranges,
+                               in_x=pre["in_x"], in_y=pre["in_y"], clamped=pre["clamped"],
                                **({"blend": record_blend} if record_blend is not None else {})))

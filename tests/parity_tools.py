@@ -72,14 +72,15 @@ def tile_mask(tiles, H, W):
 
 
 def oracle_lists(sc, cam, deg, scale_modifier=1.0):
-    """fp32 per-Gaussian stage + binning/sort (bit-exact integers) without blending anything."""
+    """fp32 per-Gaussian stage + binning/sort (bit-exact integers) without blending anything.  The
+    returned decisions also hold the fp32 EWA-clamp and colour-clamp flags for an fp64 replay."""
     S = U.oracle_settings(cam, deg, scale_modifier=scale_modifier)
     with torch.no_grad():
         pre = O.preprocess(S, sc["means3D"], sc["opacities"], shs=sc["shs"], scales=sc["scales"],
                            rotations=sc["rotations"])
         keys, pl, ranges = O.bin_and_sort(pre, S)
     dec = dict(visible=pre["visible"], radii=pre["radii"], rect=pre["rect"], touched=pre["touched"],
-               point_list=pl, ranges=ranges)
+               point_list=pl, ranges=ranges, in_x=pre["in_x"], in_y=pre["in_y"], clamped=pre["clamped"])
     return S, pre, keys, pl, ranges, dec
 
 
