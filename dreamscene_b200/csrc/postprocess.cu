@@ -1,14 +1,16 @@
 // Depth/alpha -> normalised disparity (SURVEY.md 8 f1, second half): the post-processing DreamScene runs
-// after every render (/root/reference/scene_gaussian.py:871-881)
+// after every render (DreamScene's scene_gaussian.py:871-881)
 //     depth, alpha = chunk(depth_alpha, 2)
 //     disp  = focal / (depth + alpha * 10 + 1e-5)
 //     min_d = disp[alpha <= 0.1].min()        # falls back to disp.min() when no pixel is opaque
 //     disp  = clamp((disp - min_d) / (disp.max() - min_d), 0, 1)
 // as two small kernels forward and two backward, for a batch of views, with NO host synchronisation
 // (the boolean-mask indexing above forces a device->host copy of the mask population per view).
-// Gradients follow torch autograd exactly: through the quotient, through min_d and disp.max()
-// (evenly distributed over ties, as torch.min()/max() do) and through the clamp (pass-through on
-// the closed interval).
+// Every value is rounded as torch rounds it on CUDA: focal / x is Tensor.__rdiv__, x.reciprocal() * focal (two
+// roundings); the quotient by the 0-dim (max - min_d) is a true division; clamp lets a NaN through (a view whose
+// max equals min_d normalises to 0 / 0).  Gradients follow torch autograd: per pixel, the fp32 chain of Clamp-,
+// Div-, Mul- and ReciprocalBackward in torch's order, bit for bit; through min_d and disp.max() evenly distributed
+// over the ties, as torch.min()/max() do (a sum over the view: equal to torch's within its rounding).
 #include "common.cuh"
 #include "../../include/b200gsr_frames.h"
 
@@ -37,8 +39,13 @@ __global__ void disp_init_kernel(DispStats* st, int B) {
     }
 }
 
+// r = 1 / x, x = depth + 10 alpha + 1e-5; the disparity is r * focal, as torch evaluates focal / x
+__device__ __forceinline__ float disp_rcp(float depth, float alpha) {
+    return __frcp_rn(__fadd_rn(__fadd_rn(depth, __fmul_rn(alpha, 10.0f)), 1e-5f));
+}
+
 __device__ __forceinline__ float disp_raw(float depth, float alpha, float focal) {
-    return __fdiv_rn(focal, __fadd_rn(__fadd_rn(depth, __fmul_rn(alpha, 10.0f)), 1e-5f));
+    return __fmul_rn(disp_rcp(depth, alpha), focal);
 }
 
 // One block's share of view v's statistics over its N contiguous depth and alpha values (blockDim 256, grid x strided)
@@ -74,7 +81,13 @@ __device__ __forceinline__ void disp_bounds(const DispStats& s, float& m, float&
 
 __device__ __forceinline__ float disp_norm(float d, float m, float den) {
     const float t = __fdiv_rn(__fsub_rn(d, m), den);
-    return fminf(fmaxf(t, 0.0f), 1.0f);       // NaN (den == 0) propagates like torch.clamp
+    return t != t ? t : fminf(fmaxf(t, 0.0f), 1.0f);    // NaN (0 / 0 when den == 0) passes, as torch.clamp lets it
+}
+
+// ClampBackward's gate: the gradient passes where the normalised value lies in [0, 1] (never for a NaN)
+__device__ __forceinline__ bool disp_gate(float d, float m, float den) {
+    const float t = __fdiv_rn(__fsub_rn(d, m), den);
+    return t >= 0.0f && t <= 1.0f;
 }
 
 __global__ void __launch_bounds__(256)
@@ -98,7 +111,7 @@ disp_normalise_kernel(const float* __restrict__ da, const float* __restrict__ fo
 // pixel i of channel c is at c*Hs*W + v*Hp*W + i.  The reference quantises a frame as
 //     rgb   = (clamp(color, 0, 1) * 255).round().astype(uint8)                         (float32, round half even)
 //     depth = (clamp(disp / disp.max(), 0, 1) * 255).round().astype(uint8)    disp = disp_normalise_kernel's value
-// where the cast of a NaN is undefined in numpy; here a NaN becomes 0 (fmaxf returns the non-NaN operand).
+// where the cast of a NaN is undefined in numpy; here a NaN becomes 0 (quantise8: fmaxf returns the non-NaN operand).
 
 // the statistics of disp_reduce_kernel over the stacked layout; grid (blocks, B)
 __global__ void __launch_bounds__(256)
@@ -127,7 +140,8 @@ frames_kernel(int B, int HW, size_t view_stride, size_t chan_stride, const float
         const float den = __fsub_rn(M, m);
         s_m[v] = m; s_den[v] = den; s_f[v] = focal[v];
         // max over the view of disp_norm(d): disp_norm is non-decreasing in d and M is attained, so it is
-        // disp_norm(M) - 1 for M > m, 0 when den is 0 or NaN (every pixel is then 0, and 0 / 0 quantises to 0)
+        // disp_norm(M) = 1 for M > m, NaN when den is 0 (as torch's max over a view holding a NaN): every pixel's
+        // t / NaN then quantises to 0
         s_max[v] = disp_norm(M, m, den);
     }
     __syncthreads();
@@ -186,8 +200,7 @@ disp_bwd_reduce_kernel(const float* __restrict__ da, const float* __restrict__ f
     for (int i = blockIdx.x * 256 + threadIdx.x; i < N; i += gridDim.x * 256) {
         const float a = alpha[i];
         const float d = disp_raw(depth[i], a, f);
-        const float t = (d - m) / den;
-        const float dt = (t >= 0.0f && t <= 1.0f) ? g_out[(size_t)v * N + i] : 0.0f;
+        const float dt = disp_gate(d, m, den) ? g_out[(size_t)v * N + i] : 0.0f;
         sm += dt * (d - M) * inv2;
         sM -= dt * (d - m) * inv2;
         if (d == m && (!masked_min || a <= 0.1f)) ++tm;
@@ -232,8 +245,9 @@ disp_bwd_sum_kernel(int nblk, const float* __restrict__ part, DispStats* st) {
     if (lane == 0) { st[v].sum_min += sm; st[v].sum_max += sM; }
 }
 
-// backward pass 2: d depth_alpha = chain through d = focal / x, x = depth + 10 alpha + 1e-5 (+ the caller's own
-// gradient on the alpha channel, which is returned alongside the disparity)
+// backward pass 2: d depth_alpha = chain through d = r * focal, r = 1 / x, x = depth + 10 alpha + 1e-5 (+ the
+// caller's own gradient on the alpha channel, which is returned alongside the disparity).  Each step is one rounded
+// fp32 operation in the order of torch's backward nodes, so that outside the tie sets the result is autograd's.
 __global__ void __launch_bounds__(256)
 disp_bwd_apply_kernel(const float* __restrict__ da, const float* __restrict__ focal, int N,
                       const float* __restrict__ g_out, const float* __restrict__ g_alpha,
@@ -245,19 +259,22 @@ disp_bwd_apply_kernel(const float* __restrict__ da, const float* __restrict__ fo
     disp_bounds(st[v], m, M);
     const bool masked_min = st[v].n_masked > 0;
     const float f = focal[v];
-    const float den = M - m, inv = 1.0f / den;
-    const float gmin = st[v].ties_min ? st[v].sum_min / (float)st[v].ties_min : 0.0f;
-    const float gmax = st[v].ties_max ? st[v].sum_max / (float)st[v].ties_max : 0.0f;
+    const float den = __fsub_rn(M, m);
+    const float gmin = st[v].ties_min ? __fdiv_rn(st[v].sum_min, (float)st[v].ties_min) : 0.0f;
+    const float gmax = st[v].ties_max ? __fdiv_rn(st[v].sum_max, (float)st[v].ties_max) : 0.0f;
     for (int i = blockIdx.x * 256 + threadIdx.x; i < N; i += gridDim.x * 256) {
         const float a = alpha[i];
-        const float d = disp_raw(depth[i], a, f);
-        const float t = (d - m) * inv;
-        float gd = (t >= 0.0f && t <= 1.0f) ? g_out[(size_t)v * N + i] * inv : 0.0f;
-        if (d == m && (!masked_min || a <= 0.1f)) gd += gmin;
-        if (d == M) gd += gmax;
-        const float gx = -gd * d * d / f;                     // d(focal/x)/dx = -d^2/focal
+        const float r = disp_rcp(depth[i], a);
+        const float d = __fmul_rn(r, f);
+        // ClampBackward then DivBackward: the gated gradient over den (0 / 0 = NaN on every pixel when den == 0)
+        float gd = __fdiv_rn(disp_gate(d, m, den) ? g_out[(size_t)v * N + i] : 0.0f, den);
+        if (d == m && (!masked_min || a <= 0.1f)) gd = __fadd_rn(gd, gmin);
+        if (d == M) gd = __fadd_rn(gd, gmax);
+        // MulBackward (* focal), then ReciprocalBackward: -(g) * (r * r)
+        const float gx = -__fmul_rn(__fmul_rn(gd, f), __fmul_rn(r, r));
+        const float ga = __fmul_rn(gx, 10.0f);                // MulBackward of alpha * 10
         d_da[(size_t)v * 2 * N + i] = gx;
-        d_da[(size_t)v * 2 * N + N + i] = 10.0f * gx + (g_alpha ? g_alpha[(size_t)v * N + i] : 0.0f);
+        d_da[(size_t)v * 2 * N + N + i] = g_alpha ? __fadd_rn(ga, g_alpha[(size_t)v * N + i]) : ga;
     }
 }
 

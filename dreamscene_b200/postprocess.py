@@ -1,6 +1,6 @@
 """Fused depth/alpha -> normalised disparity (SURVEY.md section 8 f1, post-processing half).
 
-``disparity_from_depth_alpha(depth_alpha, focal)`` replaces /root/reference/scene_gaussian.py:871-881
+``disparity_from_depth_alpha(depth_alpha, focal)`` replaces DreamScene's scene_gaussian.py:871-881
 
     depth, alpha = torch.chunk(depth_alpha, 2)
     disp  = focal / (depth + (alpha * 10) + 1e-5)
@@ -10,8 +10,11 @@
 
 for one view ([2,H,W]) or a batch ([B,2,H,W]) with two small kernels each way and NO host
 synchronisation (the boolean-mask indexing above copies the mask population to the host per view).
-Returns (disp [.,1,H,W], alpha [.,1,H,W]); differentiable exactly like the PyTorch expression,
-including the paths through min_d and disp.max().
+Returns (disp [.,1,H,W], alpha [.,1,H,W]), equal bit for bit to torch's evaluation of the expression on CUDA:
+`focal / x` rounded as torch's ``x.reciprocal() * focal``, and NaN wherever torch's is NaN (a view whose
+``disp.max()`` equals ``min_d`` divides 0 by 0).  Differentiable like the PyTorch expression: outside the pixels
+that tie for min_d or disp.max() the gradient is autograd's bit for bit; on those ties it carries the paths through
+min_d and disp.max(), sums over the view that agree with autograd's within fp32 rounding.
 """
 from __future__ import annotations
 

@@ -338,6 +338,8 @@ int b200gsr_assemble_backward(int32_t num_groups, const b200gsr_group* groups, c
  * /root/reference/scene_gaussian.py:871-881 for a batch of B views without any host synchronisation.
  *   depth_alpha [B,2,N] (N = H*W; channel 1 = transmittance), focal [B] (device), out_disp [B,N],
  *   stats = 32*B bytes of device scratch that must be kept for the backward.
+ * out_disp is torch's evaluation of the expression on CUDA bit for bit; in a view whose max equals min_d
+ * (e.g. one that sees nothing) the pixels at min_d are 0 / 0 = NaN and every gradient is NaN, as in torch.
  * Backward: g_disp [B,N] = dL/d out_disp, g_alpha [B,N] or NULL = dL/d alpha from other consumers of the
  * alpha channel; d_depth_alpha [B,2,N] is fully overwritten.  `stats` is updated in place (pass a copy
  * of the forward's record if the backward may run more than once).

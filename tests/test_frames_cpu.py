@@ -97,7 +97,8 @@ def _kernel_quantise(x):
 
 def _disp_norm(d, m, den):
     with np.errstate(divide="ignore", invalid="ignore"):
-        return np.fmin(np.fmax((d - m) / den, F0), F1)
+        t = (d - m) / den
+    return np.where(np.isnan(t), t, np.fmin(np.fmax(t, F0), F1))          # NaN passes, as in torch.clamp
 
 
 def _kernel_depth(d, m, M):
