@@ -559,6 +559,16 @@ static int frozen_ranges(long long P, const b200gsr_row_range* frozen, int32_t n
     return B200GSR_OK;
 }
 
+// The destinations of statistics record k (`what`: "group" or "stats record"): accum and denom both set or both null,
+// max_radii only beside them.
+static int check_stats_dests(const char* what, int k, const float* accum, const float* denom, const float* max_radii) {
+    if ((accum == nullptr) != (denom == nullptr))
+        return fail(B200GSR_ERR_BAD_ARG, "%s %d: xyz_gradient_accum and denom must both be set or both be null", what, k);
+    if (max_radii && !accum)
+        return fail(B200GSR_ERR_BAD_ARG, "%s %d: max_radii2D without xyz_gradient_accum and denom", what, k);
+    return B200GSR_OK;
+}
+
 int b200gsr_backward_views_frozen(int32_t B, const b200gsr_params* prm, const b200gsr_view_inputs* in,
                                   const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
                                   const float* dL_ddepth_alpha, void* saved, size_t saved_bytes, uint64_t max_pairs,
@@ -603,11 +613,7 @@ int b200gsr_backward_views_stats(int32_t B, const b200gsr_params* prm, const b20
             return fail(B200GSR_ERR_BAD_ARG, "stats record %d starts at %lld, before the end %lld of record %d: records "
                         "must be sorted and must not overlap", k, lo, end, k - 1);
         end = lo + len;
-        if ((r.xyz_gradient_accum != nullptr) != (r.denom != nullptr))
-            return fail(B200GSR_ERR_BAD_ARG, "stats record %d: xyz_gradient_accum and denom must both be set or both "
-                        "be null", k);
-        if (r.max_radii2D && !r.xyz_gradient_accum)
-            return fail(B200GSR_ERR_BAD_ARG, "stats record %d: max_radii2D without xyz_gradient_accum and denom", k);
+        if ((rc = check_stats_dests("stats record", k, r.xyz_gradient_accum, r.denom, r.max_radii2D))) return rc;
         for (int j = 0; j < fr.n; ++j)
             if (lo < (long long)fr.lo[j] + fr.len[j] && (long long)fr.lo[j] < lo + len)
                 return fail(B200GSR_ERR_BAD_ARG, "stats record %d [%lld, %lld) overlaps the frozen rows [%u, %u): a "
@@ -1142,31 +1148,55 @@ int b200gsr_forward_scene_dyn(int32_t B, const b200gsr_params* prm, int32_t num_
 }
 
 // The statistics arguments of b200gsr_backward_scene[_dyn]_stats (include/b200gsr_stats.h), after check_scene and the
-// frozen mask's check.  -> whether any group gathers.
-static int check_stats(int32_t B, int32_t num_groups, uint32_t frozen, const b200gsr_group_stats* stats, bool dyn,
-                       int32_t stats_view, const int32_t* dyn_stats_view, bool& any) {
-    any = false;
+// frozen mask's check, as the records of b200gsr_backward_views_stats: one per group that gathers, over its packed rows.
+static int scene_stats(int32_t B, int32_t num_groups, const b200gsr_group* groups, uint32_t frozen,
+                       const b200gsr_group_stats* stats, bool dyn, int32_t stats_view, const int32_t* dyn_stats_view,
+                       GsrRowStats& rs) {
+    rs = GsrRowStats{};
     if (!dyn && (stats_view < -1 || stats_view >= B))
         return fail(B200GSR_ERR_BAD_ARG, "stats_view %d not in -1..%d", stats_view, B - 1);
-    for (int g = 0; g < num_groups && stats; ++g) {
+    int rc;
+    uint32_t row = 0;
+    for (int g = 0; g < num_groups && stats; row += (uint32_t)groups[g].n, ++g) {
         const b200gsr_group_stats& st = stats[g];
-        if ((st.xyz_gradient_accum == nullptr) != (st.denom == nullptr))
-            return fail(B200GSR_ERR_BAD_ARG, "group %d: xyz_gradient_accum and denom must both be set or both be null", g);
-        if (st.xyz_gradient_accum == nullptr && st.max_radii2D != nullptr)
-            return fail(B200GSR_ERR_BAD_ARG, "group %d: max_radii2D without xyz_gradient_accum and denom", g);
+        if ((rc = check_stats_dests("group", g, st.xyz_gradient_accum, st.denom, st.max_radii2D))) return rc;
         if (st.xyz_gradient_accum == nullptr) continue;
         if ((frozen >> g) & 1u)
             return fail(B200GSR_ERR_BAD_ARG, "group %d: statistics on a frozen group (its rows would count in denom with "
                         "a zero gradient)", g);
-        any = true;
+        rs.lo[rs.n] = row; rs.len[rs.n] = (uint32_t)groups[g].n;
+        rs.accum[rs.n] = st.xyz_gradient_accum; rs.denom[rs.n] = st.denom; rs.max_radii[rs.n] = st.max_radii2D;
+        ++rs.n;
     }
-    if (any && dyn && !dyn_stats_view)
+    if (rs.n > 0 && dyn && !dyn_stats_view)
         return fail(B200GSR_ERR_BAD_ARG, "stats_view must be a device pointer to an int32 when a group gathers statistics");
+    rs.view = rs.n > 0 ? stats_view : -1;
     return B200GSR_OK;
 }
 
+// The frozen group mask as frozen row ranges: each frozen group's packed rows, adjacent frozen groups merged and empty
+// ones merged away, so 24 groups give at most B200GSR_MAX_FROZEN_RANGES = 12 ranges.
+static GsrFrozenRanges group_ranges(int32_t num_groups, const b200gsr_group* groups, uint32_t frozen) {
+    GsrFrozenRanges fr{};
+    uint32_t row = 0;
+    for (int g = 0; g < num_groups; ++g) {
+        const uint32_t n = (uint32_t)groups[g].n;
+        if (n > 0 && ((frozen >> g) & 1u)) {
+            if (fr.n > 0 && fr.lo[fr.n - 1] + fr.len[fr.n - 1] == row) {
+                fr.len[fr.n - 1] += n;
+            } else {
+                fr.lo[fr.n] = row; fr.len[fr.n] = n;
+                ++fr.n;
+            }
+        }
+        row += n;
+    }
+    return fr;
+}
+
 // b200gsr_backward_scene, b200gsr_backward_scene_dyn (frozen = 0), their _frozen variants (include/b200gsr_frozen.h)
-// and their _stats variants (include/b200gsr_stats.h, `with_stats`: d_means2D may be null)
+// and their _stats variants (include/b200gsr_stats.h, `with_stats`: d_means2D may be null).  The frozen mask and the
+// group statistics reach the kernels as the frozen row ranges and statistics records of backward_views.
 static int backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_groups, const b200gsr_group* groups,
                           const b200gsr_group_grad* grads, GsrScene sc, bool dyn, const float* d_scales,
                           const int32_t* radii, const float* out_depth_alpha, const float* dL_dcolor,
@@ -1179,8 +1209,8 @@ static int backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_grou
     if (flags & ~B200GSR_BWD_DETERMINISTIC) return fail(B200GSR_ERR_BAD_ARG, "unknown flags 0x%x", flags);
     if (frozen >> num_groups)      // num_groups <= B200GSR_MAX_GROUPS < 32 (check_scene)
         return fail(B200GSR_ERR_BAD_ARG, "frozen mask 0x%x has bits at or above num_groups %d", frozen, num_groups);
-    bool gathers = false;
-    if (with_stats && (rc = check_stats(B, num_groups, frozen, stats, dyn, stats_view, dyn_stats_view, gathers)))
+    GsrRowStats rs;
+    if (with_stats && (rc = scene_stats(B, num_groups, groups, frozen, stats, dyn, stats_view, dyn_stats_view, rs)))
         return rc;
     if (num_groups > 0 && !grads) return fail(B200GSR_ERR_BAD_ARG, "grads is null");
     for (int g = 0; g < num_groups; ++g)
@@ -1195,15 +1225,12 @@ static int backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_grou
     if ((rc = setup_backward(true, B, prm, radii, out_depth_alpha, dL_dcolor, dL_ddepth_alpha, saved, saved_bytes,
                              max_pairs, (flags & B200GSR_BWD_DETERMINISTIC) != 0, stream, a)))
         return rc;
-    sc.num_groups = num_groups; sc.groups = groups; sc.grads = grads; sc.d_scales = d_scales; sc.frozen = frozen;
-    if (gathers) {
-        sc.stats = stats;
-        sc.stats_view = stats_view;
-        sc.dyn_stats_view = dyn_stats_view;
-    } else {
-        sc.stats_view = -1;
-    }
+    sc.num_groups = num_groups; sc.groups = groups; sc.grads = grads; sc.d_scales = d_scales;
+    const GsrFrozenRanges fr = group_ranges(num_groups, groups, frozen);
     a.scene = &sc;
+    a.frozen_rows = frozen ? &fr : nullptr;
+    a.row_stats = with_stats ? &rs : nullptr;
+    a.dyn_stats_view = with_stats && rs.n > 0 ? dyn_stats_view : nullptr;
     a.g_begin = 0; a.g_end = P;
     prof_mark_bwd(0, a.stream);
     GSR_RANGE_PUSH("b200gsr.scene.composite_bwd");
@@ -1215,9 +1242,6 @@ static int backward_scene(int32_t B, const b200gsr_params* prm, int32_t num_grou
     for (int v = 0; v < B && !rc; ++v) {      // in view order: view 0 writes the leaf gradients, later views add
         a.prm = prm[v]; a.view = v;
         a.d_means2D = d_means2D ? d_means2D + 3 * (size_t)P * v : nullptr;
-        // the STATS kernel where it has work: every view under _dyn (the view to gather is read on the device) or
-        // without d_means2D; by value, only the launch of the view that gathers.  The other launches are _frozen's.
-        sc.stats_mode = with_stats && (dyn || !d_means2D || (gathers && v == stats_view));
         rc = check_cuda(gsr_launch_project_bwd(a), "project_bwd");
     }
     GSR_RANGE_POP();

@@ -244,15 +244,6 @@ struct GsrScene {
     // shs_noise / scale_noise / seed and the views' tanfovx / tanfovy / sh_degree (both null otherwise)
     const b200gsr_step_view* dyn_views;
     const unsigned long long* dyn_seed;
-    // backward (b200gsr_backward_scene[_dyn]_frozen): bit g = group g is frozen; its leaves get no gradient and
-    // composite_bwd / project_bwd run their FROZEN instantiations.  0 = the default kernels.
-    uint32_t frozen;    // backward (b200gsr_backward_scene[_dyn]_stats): project_bwd runs its STATS instantiation, which takes a null
-    // d_means2D and gathers the densification statistics of `stats` (host array [num_groups], or null) in the launch
-    // of the view stats_view (by value) or *dyn_stats_view (the _dyn entry point).  false = the other kernels.
-    bool stats_mode;
-    const b200gsr_group_stats* stats;
-    int32_t stats_view;
-    const int32_t* dyn_stats_view;
     // b200gsr_*_scene_dyn_live: device [num_groups] live row counts (include/b200gsr_reserve.h); project_sh /
     // project_bwd run their LIVE instantiations.  Null otherwise.
     const int32_t* live;
@@ -283,18 +274,20 @@ struct GsrFwdArgs {
     const GsrScene* scene; // scene render: the raw leaves replace means3D .. cov3d (null otherwise)
 };
 
-// Frozen rows of a multi-view backward (b200gsr_backward_views_frozen): n sorted, merged, non-empty half-open ranges
-// [lo, lo + len) of one view's P rows, the same in every view.  composite_bwd and project_bwd run their FROZEN
-// instantiations over them.
+// Frozen rows of a multi-view backward: n sorted, merged, non-empty half-open ranges [lo, lo + len) of one view's P
+// rows, the same in every view.  b200gsr_backward_views_frozen / _stats take them from the caller; the scene
+// backwards' _frozen, _stats and _live variants form them from the frozen group mask, so a mask whose frozen groups
+// are all empty gives n = 0.  composite_bwd and project_bwd run their FROZEN instantiations over them.
 struct GsrFrozenRanges {
     int n;
     uint32_t lo[B200GSR_MAX_FROZEN_RANGES], len[B200GSR_MAX_FROZEN_RANGES];
 };
 
-// Densification statistics of a multi-view backward (b200gsr_backward_views_stats): n sorted, non-overlapping,
-// non-empty row ranges [lo, lo + len) of one view's P rows with their destinations (accum null = the record gathers
-// nothing; max_radii may be null), and the view whose launch gathers (-1 = none).  project_bwd runs its packed STATS
-// instantiation in that launch, and in every launch whose d_means2D is null.
+// Densification statistics of a multi-view backward: n sorted, non-overlapping row ranges [lo, lo + len) of one
+// view's P rows that gather, with their destinations (max_radii may be null), and the view whose launch gathers
+// (-1 = none).  b200gsr_backward_views_stats takes them from the caller's records; the scene backwards' _stats and
+// _live variants make one per group that gathers (the group's rows, possibly none), and their _dyn forms read the
+// gathering view from device memory instead (GsrBwdArgs::dyn_stats_view).
 struct GsrRowStats {
     int n;
     int32_t view;
@@ -323,8 +316,11 @@ struct GsrBwdArgs {
     unsigned long long* stats;   // optional device counters (b200gsr_debug_counters); selects the STATS kernels
     cudaStream_t stream;
     const GsrScene* scene;       // scene render: leaf gradients of the raw parameters (null otherwise)
-    const GsrFrozenRanges* frozen_rows;   // b200gsr_backward_views_frozen with ranges (null otherwise)
-    const GsrRowStats* row_stats;         // b200gsr_backward_views_stats (null otherwise)
+    const GsrFrozenRanges* frozen_rows;   // frozen rows (null: nothing frozen)
+    // Statistics (null: not gathered).  project_bwd runs its STATS instantiation in the launch of the gathering view,
+    // in every launch without d_means2D, and in every launch of a _dyn scene backward.
+    const GsrRowStats* row_stats;
+    const int32_t* dyn_stats_view;        // _dyn scene backwards: device int32, the view that gathers (null = none)
 };
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device) instead of on every

@@ -424,9 +424,9 @@ __device__ __forceinline__ void halve2(float (&v)[10], bool hi) {
     if (Hh & 1) v[Hh - 1] = keep[Hh - 1] + recv[Hh - 1];
 }
 
-// Frozen groups (b200gsr_backward_scene_frozen): the packed rows of the frozen groups as merged half-open intervals
-// [lo, lo + len).  Adjacent frozen groups merge, so 24 groups give at most 12 intervals.  The caller's frozen row
-// ranges of b200gsr_backward_views_frozen arrive in the same form.
+// Frozen rows (GsrFrozenRanges) as merged half-open intervals [lo, lo + len): the caller's ranges of
+// b200gsr_backward_views_frozen, or the packed rows of the scene backwards' frozen groups.  Adjacent frozen groups
+// merge, so 24 groups give at most 12 intervals.
 constexpr int kMaxFrozenIntervals = (B200GSR_MAX_GROUPS + 1) / 2;
 static_assert(kMaxFrozenIntervals == B200GSR_MAX_FROZEN_RANGES, "b200gsr_views_frozen.h states the interval limit");
 struct NoFrozen {};
@@ -822,27 +822,7 @@ static cudaError_t launch_bwd(const GsrBwdArgs& a, const CompPtrs& c, uint32_t* 
     return cudaGetLastError();
 }
 
-// The frozen groups' packed rows (bit g of sc.frozen: group g) as merged intervals; empty groups merge away.
-static FrozenRows frozen_rows(const GsrScene& sc, int P_view) {
-    FrozenRows f{};
-    f.P_view = (uint32_t)P_view;
-    uint32_t row = 0;
-    for (int g = 0; g < sc.num_groups; ++g) {
-        const uint32_t n = (uint32_t)sc.groups[g].n;
-        if (n > 0 && ((sc.frozen >> g) & 1u)) {
-            if (f.n > 0 && f.lo[f.n - 1] + f.len[f.n - 1] == row) {
-                f.len[f.n - 1] += n;
-            } else {
-                f.lo[f.n] = row; f.len[f.n] = n;
-                ++f.n;
-            }
-        }
-        row += n;
-    }
-    return f;
-}
-
-// The caller's frozen row ranges (b200gsr_backward_views_frozen, validated and merged by the entry point).
+// The frozen row ranges (validated and merged by the entry point).
 static FrozenRows frozen_rows(const GsrFrozenRanges& r, int P_view) {
     FrozenRows f{};
     f.P_view = (uint32_t)P_view;
@@ -856,11 +836,10 @@ cudaError_t gsr_launch_composite_bwd(const GsrBwdArgs& a) {
     if (c.grid.ntiles == 0) return cudaSuccess;
     uint32_t* queue = reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE;
     float* dgeom = reinterpret_cast<float*>(a.saved + a.vl.dgeom);
-    // Frozen groups: the FROZEN instantiations; the instrumented kernel has no such mode and the counters are left
+    // Frozen rows: the FROZEN instantiations; the instrumented kernel has no such mode and the counters are left
     // untouched, as in deterministic mode.
-    const bool frozen = (a.scene != nullptr && a.scene->frozen != 0u) || a.frozen_rows != nullptr;
-    const FrozenRows fz = a.frozen_rows ? frozen_rows(*a.frozen_rows, a.P_view)
-                                        : frozen ? frozen_rows(*a.scene, a.P_view) : FrozenRows{};
+    const bool frozen = a.frozen_rows != nullptr;
+    const FrozenRows fz = frozen ? frozen_rows(*a.frozen_rows, a.P_view) : FrozenRows{};
     if (a.det) {
         // Deterministic mode: the default kernel with integer commits, run twice (instrumentation does not apply).
         // Pass B pops its own work queue (header words, zero between calls like the first one): no memset.

@@ -268,32 +268,23 @@ struct SceneFwdDyn : SceneFwd { SceneDyn dyn; };
 struct SceneBwdDyn : SceneBwd { SceneDyn dyn; };
 template <bool RAW, bool DYN>
 using FwdScene = std::conditional_t<RAW, std::conditional_t<DYN, SceneFwdDyn, SceneFwd>, NoScene>;
-// FROZEN (with RAW): bit g of `frozen` = group g is frozen (b200gsr_backward_scene_frozen).  A derived type, so that
-// the other instantiations' kernel argument keeps its layout.
-template <typename S>
-struct SceneFrozen : S { uint32_t frozen; };
-// FROZEN without RAW, the packed-input backward with frozen rows (b200gsr_backward_views_frozen): the caller's frozen
-// row ranges of one view.  Derived from NoScene, whose fields (none) the default statements read.
-struct RowsFrozen : NoScene { GsrFrozenRanges rows; };
-// STATS without RAW, the packed-input backward with the densification statistics (b200gsr_backward_views_stats): the
-// records' row ranges and destinations, the view whose launch gathers (st.view), and this launch's view.  Derived from
-// RowsFrozen whatever FROZEN is (rows.n = 0 when nothing is frozen).
-struct RowsStats : RowsFrozen {
-    GsrRowStats st;
-    int32_t view;
-};
-// STATS (with RAW): the densification statistics of b200gsr_backward_scene[_dyn]_stats.  Per group the destinations
-// (accum null = the group gathers nothing; max_radii may be null), and the view whose launch gathers: `view` by value,
-// or *view_dev under DYN (null = none).  Derived from SceneFrozen whatever FROZEN is.
-struct StatsTable {
-    float* accum[kMaxGroups];
-    float* denom[kMaxGroups];
-    float* max_radii[kMaxGroups];
-    int32_t view;
-    const int32_t* view_dev;
-};
-template <bool DYN>
-struct SceneStats : SceneFrozen<std::conditional_t<DYN, SceneBwdDyn, SceneBwd>> { StatsTable st; };
+// project_bwd's base argument: NoScene for the packed inputs, SceneBwd / SceneBwdDyn under RAW.
+template <bool RAW, bool DYN>
+using BwdBase = std::conditional_t<RAW, std::conditional_t<DYN, SceneBwdDyn, SceneBwd>, NoScene>;
+// FROZEN: the frozen row ranges of one view (GsrFrozenRanges).  Derived types, so that the other instantiations'
+// kernel argument keeps its layout.
+template <typename B>
+struct RowsFrozen : B { GsrFrozenRanges rows; };
+// STATS: the statistics records and the view whose launch gathers (st.view).  Derived from RowsFrozen whatever FROZEN
+// is (rows.n = 0 when nothing is frozen).
+template <typename B>
+struct RowsStats : RowsFrozen<B> { GsrRowStats st; };
+// The packed inputs' STATS argument adds this launch's view, which SceneBwd carries under RAW.
+struct PackedStats : RowsStats<NoScene> { int32_t view; };
+// DYN's adds the device int32 read in place of st.view (null = none), so that a replayed graph can move the view.
+struct RowsStatsDyn : RowsStats<SceneBwdDyn> { const int32_t* view_dev; };
+template <bool RAW, bool DYN>
+using BwdStats = std::conditional_t<RAW, std::conditional_t<DYN, RowsStatsDyn, RowsStats<SceneBwd>>, PackedStats>;
 // LIVE (b200gsr_*_scene_dyn_live): the device live row count of each group (include/b200gsr_reserve.h).  A derived
 // type, so that the other instantiations' kernel argument keeps its layout.
 template <typename S>
@@ -302,12 +293,8 @@ template <bool RAW, bool DYN, bool LIVE>
 using FwdSceneLive = std::conditional_t<LIVE, SceneLive<SceneFwdDyn>, FwdScene<RAW, DYN>>;
 // project_bwd_kernel's argument type for each mode.
 template <bool RAW, bool DYN, bool FROZEN, bool STATS, bool LIVE>
-using BwdScene = std::conditional_t<
-    STATS, std::conditional_t<RAW, std::conditional_t<LIVE, SceneLive<SceneStats<DYN>>, SceneStats<DYN>>, RowsStats>,
-    std::conditional_t<
-        RAW, std::conditional_t<FROZEN, SceneFrozen<std::conditional_t<DYN, SceneBwdDyn, SceneBwd>>,
-                                std::conditional_t<DYN, SceneBwdDyn, SceneBwd>>,
-        std::conditional_t<FROZEN, RowsFrozen, NoScene>>>;
+using BwdScene = std::conditional_t<STATS, std::conditional_t<LIVE, SceneLive<BwdStats<RAW, DYN>>, BwdStats<RAW, DYN>>,
+                                    std::conditional_t<FROZEN, RowsFrozen<BwdBase<RAW, DYN>>, BwdBase<RAW, DYN>>>;
 
 // LIVE: row `loc` of group `grp` -> its row in the compact layout (sum_{h<grp} live[h] + loc), the counter of its
 // augmentation noise, or -1 when it is dead (loc >= live[grp]).  Live counts are clamped to the group's capacity.
@@ -346,20 +333,48 @@ __device__ __forceinline__ ViewNoise view_noise(const S& sc, b200gsr_params& p) 
 #define GSR_C_SHS (DYN ? nz.c_shs : sc.c_shs)
 #define GSR_C_SCALE (DYN ? nz.c_scale : sc.c_scale)
 
-// FROZEN: whether active row i belongs to a frozen group (RAW) or lies in one of the frozen row ranges (packed
-// inputs; a loop over the ranges in use, as composite_bwd's row_frozen).  A constant false otherwise.
+// FROZEN: whether active row i lies in one of the frozen row ranges (a loop over the ranges in use, as composite_bwd's
+// row_frozen).  A constant false otherwise.
 template <bool FROZEN, typename S>
 __device__ __forceinline__ bool frozen_row(const S& sc, bool active, int i) {
-    if constexpr (FROZEN && std::is_base_of_v<RowsFrozen, S>) {
+    if constexpr (FROZEN) {
         if (!active) return false;
 #pragma unroll 1
         for (int k = 0; k < sc.rows.n; ++k)
             if ((uint32_t)i - sc.rows.lo[k] < sc.rows.len[k]) return true;
         return false;
-    } else if constexpr (FROZEN) {
-        return active && ((sc.frozen >> find_group(sc.tab, i)) & 1u);
     } else {
         return false;
+    }
+}
+
+// STATS: the view whose launch gathers the statistics: st.view, or under DYN the device int32 (null = none).
+template <bool DYN, typename S>
+__device__ __forceinline__ int gathering_view(const S& sc) {
+    if constexpr (DYN) return sc.view_dev != nullptr ? __ldg(sc.view_dev) : -1;
+    else return sc.st.view;
+}
+// STATS: with `gathers` (a visible row in the launch of that view), row i adds its screen-space gradient's norm, 1 and
+// its radius to row i - lo of the record that holds it: the arithmetic of densify_stats_kernel on the d_means2D row this
+// thread computed, so no atomics.  The records are sorted and disjoint, so at most one holds row i, and none overlaps a
+// frozen row (refused on the host).  The caller evaluates `gathers`: the view test written inside this function made
+// the packed inputs' kernels test `vis` on its own branch.
+template <typename S>
+__device__ __forceinline__ void gather_stats(const S& sc, bool gathers, int i, const int32_t* __restrict__ radii,
+                                             int rec_base, const float (&dm2)[2]) {
+    if (gathers) {
+#pragma unroll 1
+        for (int k = 0; k < sc.st.n; ++k) {
+            const uint32_t loc = (uint32_t)i - sc.st.lo[k];
+            if (loc < sc.st.len[k]) {
+                const int r = __ldg(radii + rec_base + i);
+                sc.st.accum[k][loc] += gsr_screen_grad_norm(dm2[0], dm2[1]);
+                sc.st.denom[k][loc] += 1.0f;
+                float* pm = sc.st.max_radii[k];
+                if (pm != nullptr) pm[loc] = fmaxf(pm[loc], (float)r);
+                break;
+            }
+        }
     }
 }
 
@@ -691,18 +706,13 @@ project_sh_kernel(b200gsr_params p, const float* __restrict__ means3D,
 // the raw leaves of `sc.tab` and the view's parameter gradients are chained straight to the leaf gradients of
 // `sc.gtab`; view 0 writes every row (zeros on culled rows), later views add into the rows they touched only.  It
 // carries more live state (the leaf values and noise of the row), hence 5 CTAs/SM.  DYN (with RAW): the view's
-// per-step values come from device memory (view_noise).  FROZEN (with RAW): rows of the groups set in sc.frozen are
-// treated as culled - no SH staging, geometry, dgeom access, leaf load or store, or noise draw - except that their
-// d_means2D rows are written (zeros); composite_bwd's FROZEN mode left their dgeom rows at zero.  Every other row runs
-// the default statements.  FROZEN without RAW (b200gsr_backward_views_frozen): the rows in sc.rows are treated as
-// culled - no SH staging, geometry, dgeom read-and-clear or input load - and their gradient rows and d_means2D rows
-// are written as zeros (added to under `accumulate`), so every output row stays defined.  STATS (with RAW): d_means2D
-// may be null (nothing stored), and in the launch of the statistics view (sc.st) each visible row of a group with
-// statistics adds its screen-space gradient's norm, 1 and its radius to the group's accum / denom / max_radii row -
-// the arithmetic of densify_stats_kernel on the d_means2D row this launch computes.  One thread per row: no atomics.
-// STATS without RAW (b200gsr_backward_views_stats): d_means2D may be null, and in the launch of the statistics view
-// (sc.st.view == sc.view) each visible row inside one of the records adds the same three values to the record's row
-// (row - lo); the thread that computed the row's screen-space gradient does it, so again no atomics.
+// per-step values come from device memory (view_noise).  FROZEN: the rows in sc.rows are treated as culled - no SH
+// staging, geometry, dgeom access or input load.  Under RAW their leaf rows are neither loaded nor stored and no noise
+// is drawn for them; only their d_means2D rows are written (zeros), and composite_bwd's FROZEN mode left their dgeom
+// rows at zero.  With packed inputs their gradient rows and d_means2D rows are written as zeros (added to under
+// `accumulate`), so every output row stays defined.  Every other row runs the default statements.  STATS: d_means2D
+// may be null (nothing stored), and the launch of the statistics view gathers the statistics of the records in sc.st
+// (gather_stats).
 // LIVE (with STATS and DYN, b200gsr_backward_scene_dyn_live): dead rows get zero gradients and no statistics, and
 // read no leaf.
 // S is the mode's BwdScene: a template parameter, so that `sc` has a dependent type and the statements of the other
@@ -722,6 +732,8 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
                    float* __restrict__ d_rots, float* __restrict__ d_cov3d, const __grid_constant__ S sc) {
     extern __shared__ __align__(16) float sh_buf[];
     __shared__ uint8_t vis_s[kBlock];
+    // RAW FROZEN: the block's rows' fz, for view 0's SH drain (a range test there cost 4 % of the kernel on an H100)
+    __shared__ uint8_t frozen_s[RAW && FROZEN ? kBlock : 1];
     const ViewNoise nz = view_noise<DYN>(sc, p);
     // this launch covers Gaussians [g_base, g_end) (the whole range, or one chunk when the host
     // overlaps the gradient all-reduce of finished chunks with the remaining ones)
@@ -736,6 +748,7 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
     const int ncoef = (deg + 1) * (deg + 1);
     if (RAW || shs != nullptr) {
         vis_s[threadIdx.x] = vis;
+        if constexpr (RAW && FROZEN) frozen_s[threadIdx.x] = fz;
         __syncthreads();
         if constexpr (RAW) stage_raw_rows<false>(sc.tab, p.M, 3 * ncoef, g0, g_end, vis_s, sh_buf, stride);
         else stage_sh_rows<MT, false>(shs, p.M, 3 * ncoef, g0, g_end, vis_s, sh_buf, stride);   // issue only
@@ -981,18 +994,8 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
             if (!STATS || d_means2D != nullptr) {
                 d_means2D[3 * (size_t)i] = dm2[0]; d_means2D[3 * (size_t)i + 1] = dm2[1]; d_means2D[3 * (size_t)i + 2] = 0.f;
             }
-            if constexpr (STATS) {
-                // visible = radii > 0 (no row of a group with statistics is frozen: refused on the host)
-                const int sv = DYN ? (sc.st.view_dev != nullptr ? __ldg(sc.st.view_dev) : -1) : sc.st.view;
-                float* pa = sc.st.accum[grp];
-                if (vis && sv == (int)sc.view && pa != nullptr) {
-                    const int r = __ldg(radii + rec_base + i);
-                    pa[loc] += gsr_screen_grad_norm(dm2[0], dm2[1]);
-                    sc.st.denom[grp][loc] += 1.0f;
-                    float* pm = sc.st.max_radii[grp];
-                    if (pm != nullptr) pm[loc] = fmaxf(pm[loc], (float)r);
-                }
-            }
+            if constexpr (STATS)
+                gather_stats(sc, vis && gathering_view<DYN>(sc) == (int)sc.view, i, radii, rec_base, dm2);
             // this view's contribution to the row's 11 leaf floats; a later view loads all old values before it
             // stores any (the five leaf arrays may alias as far as the compiler knows: load/store pairs would
             // serialise on the load latency)
@@ -1055,9 +1058,9 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
                 const int gi = g0 + row;
                 const bool v = gi < g_end && vis_s[row];
                 bool on = gi < g_end && (first || v);
+                if constexpr (FROZEN) on = on && !frozen_s[row];
                 int gg = 0;
                 if (on) gg = find_group(sc.tab, gi);
-                if constexpr (FROZEN) on = on && !((sc.frozen >> gg) & 1u);
                 const size_t ll = on ? (size_t)(gi - sc.tab.start[gg]) : 0;
 #pragma unroll
                 for (int j = 0; j < 3; ++j) {
@@ -1096,24 +1099,7 @@ project_bwd_kernel(b200gsr_params p, const float* __restrict__ means3D,
         if (!STATS || d_means2D != nullptr) {
             d_means2D[3 * (size_t)i] = dm2[0]; d_means2D[3 * (size_t)i + 1] = dm2[1]; d_means2D[3 * (size_t)i + 2] = 0.f;
         }
-        if constexpr (STATS && !RAW) {
-            // visible = radii > 0 (no record overlaps a frozen range: refused on the host); the records are sorted
-            // and disjoint, so at most one holds row i
-            if (vis && sc.st.view == sc.view) {
-#pragma unroll 1
-                for (int k = 0; k < sc.st.n; ++k) {
-                    const uint32_t loc = (uint32_t)i - sc.st.lo[k];
-                    if (loc < sc.st.len[k]) {
-                        const int r = __ldg(radii + rec_base + i);
-                        sc.st.accum[k][loc] += gsr_screen_grad_norm(dm2[0], dm2[1]);
-                        sc.st.denom[k][loc] += 1.0f;
-                        float* pm = sc.st.max_radii[k];
-                        if (pm != nullptr) pm[loc] = fmaxf(pm[loc], (float)r);
-                        break;
-                    }
-                }
-            }
-        }
+        if constexpr (STATS) gather_stats(sc, vis && gathering_view<DYN>(sc) == (int)sc.view, i, radii, rec_base, dm2);
         GSR_OUT(d_opac + i, dop, 2);
         if (cov3d != nullptr) {
 #pragma unroll
@@ -1292,70 +1278,50 @@ static SceneBwd scene_bwd(const GsrBwdArgs& a) {
 }
 
 template <int MT, bool RAW = false, bool DYN = false, bool FROZEN = false, bool STATS = false, bool LIVE = false>
-static void launch_project_bwd(const GsrBwdArgs& a, int g_begin, int g_end, size_t smem) {
+static void launch_project_bwd(const GsrBwdArgs& a, size_t smem) {
     BwdScene<RAW, DYN, FROZEN, STATS, LIVE> sc{};
     if constexpr (RAW) static_cast<SceneBwd&>(sc) = scene_bwd(a);
     if constexpr (DYN) sc.dyn = SceneDyn{a.scene->dyn_views, a.scene->dyn_seed};
-    if constexpr (RAW && (FROZEN || STATS)) sc.frozen = a.scene->frozen;
-    if constexpr (!RAW && FROZEN) sc.rows = *a.frozen_rows;
-    if constexpr (!RAW && STATS) {
-        sc.st = *a.row_stats;
-        sc.view = a.view;
-    }
-    if constexpr (RAW && STATS) {
-        const GsrScene& s = *a.scene;
-        for (int g = 0; g < s.num_groups && s.stats; ++g) {
-            sc.st.accum[g] = s.stats[g].xyz_gradient_accum;
-            sc.st.denom[g] = s.stats[g].denom;
-            sc.st.max_radii[g] = s.stats[g].max_radii2D;
-        }
-        sc.st.view = s.stats_view;
-        sc.st.view_dev = s.dyn_stats_view;
-    }
+    if constexpr (FROZEN) sc.rows = *a.frozen_rows;
+    if constexpr (STATS) sc.st = *a.row_stats;
+    if constexpr (STATS && !RAW) sc.view = a.view;
+    if constexpr (STATS && DYN) sc.view_dev = a.dyn_stats_view;
     if constexpr (LIVE) sc.live = a.scene->live;
-    const int nblocks = (g_end - g_begin + kBlock - 1) / kBlock;
+    const int nblocks = (a.g_end - a.g_begin + kBlock - 1) / kBlock;
     project_bwd_kernel<MT, RAW, DYN, FROZEN, STATS, LIVE><<<nblocks, kBlock, smem, a.stream>>>(
         a.prm, a.means3D, a.shs, a.colors, a.scales, a.rots, a.cov3d, a.radii,
         reinterpret_cast<float*>(a.saved + a.vl.dgeom),
-        reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE, g_begin, g_end,
+        reinterpret_cast<uint32_t*>(a.saved + a.vl.header) + GSR_H_BWD_QUEUE, a.g_begin, a.g_end,
         a.dsh_coefs > 0 ? a.dsh_coefs : (a.dsh_coefs < 0 ? -1 : a.prm.M), a.view * a.P_view, a.accumulate, a.d_means3D,
         a.d_means2D, a.d_shs,
         a.d_colors, a.d_opac, a.d_scales, a.d_rots, a.d_cov3d, sc);
 }
 
+// The FROZEN and STATS instantiations of one (MT, RAW, DYN).
+template <int MT, bool RAW = false, bool DYN = false>
+static void launch_project_bwd_modes(const GsrBwdArgs& a, bool frozen, bool stats, size_t smem) {
+    if (frozen && stats) launch_project_bwd<MT, RAW, DYN, true, true>(a, smem);
+    else if (frozen) launch_project_bwd<MT, RAW, DYN, true>(a, smem);
+    else if (stats) launch_project_bwd<MT, RAW, DYN, false, true>(a, smem);
+    else launch_project_bwd<MT, RAW, DYN>(a, smem);
+}
+
 cudaError_t gsr_launch_project_bwd(const GsrBwdArgs& a) {
-    const int g_begin = a.g_begin, g_end = a.g_end;
-    if (g_end <= g_begin) return cudaSuccess;
+    if (a.g_end <= a.g_begin) return cudaSuccess;
     const size_t smem = (a.shs || a.scene) ? (size_t)kBlock * sh_row_stride(a.prm.M) * sizeof(float) : 0;
-    const bool frozen = a.scene && a.scene->frozen;
-    if (a.scene && a.scene->live) {     // b200gsr_backward_scene_dyn_live: every launch gathers the statistics
-        if (frozen) launch_project_bwd<0, true, true, true, true, true>(a, g_begin, g_end, smem);
-        else launch_project_bwd<0, true, true, false, true, true>(a, g_begin, g_end, smem);
-    } else if (a.scene && a.scene->stats_mode) {
-        const bool dyn = a.scene->dyn_views != nullptr;
-        if (dyn && frozen) launch_project_bwd<0, true, true, true, true>(a, g_begin, g_end, smem);
-        else if (dyn) launch_project_bwd<0, true, true, false, true>(a, g_begin, g_end, smem);
-        else if (frozen) launch_project_bwd<0, true, false, true, true>(a, g_begin, g_end, smem);
-        else launch_project_bwd<0, true, false, false, true>(a, g_begin, g_end, smem);
-    } else if (a.scene && a.scene->dyn_views && frozen) launch_project_bwd<0, true, true, true>(a, g_begin, g_end, smem);
-    else if (a.scene && frozen) launch_project_bwd<0, true, false, true>(a, g_begin, g_end, smem);
-    else if (a.scene && a.scene->dyn_views) launch_project_bwd<0, true, true>(a, g_begin, g_end, smem);
-    else if (a.scene) launch_project_bwd<0, true>(a, g_begin, g_end, smem);
-    else if (a.row_stats && (a.view == a.row_stats->view || !a.d_means2D)) {
-        // b200gsr_backward_views_stats: the launch that gathers, and every launch that stores no d_means2D
-        if (a.frozen_rows && a.shs && a.prm.M == 16) launch_project_bwd<16, false, false, true, true>(a, g_begin, g_end, smem);
-        else if (a.frozen_rows && a.shs && a.prm.M == 4) launch_project_bwd<4, false, false, true, true>(a, g_begin, g_end, smem);
-        else if (a.frozen_rows) launch_project_bwd<0, false, false, true, true>(a, g_begin, g_end, smem);
-        else if (a.shs && a.prm.M == 16) launch_project_bwd<16, false, false, false, true>(a, g_begin, g_end, smem);
-        else if (a.shs && a.prm.M == 4) launch_project_bwd<4, false, false, false, true>(a, g_begin, g_end, smem);
-        else launch_project_bwd<0, false, false, false, true>(a, g_begin, g_end, smem);
-    }
-    else if (a.frozen_rows && a.shs && a.prm.M == 16) launch_project_bwd<16, false, false, true>(a, g_begin, g_end, smem);
-    else if (a.frozen_rows && a.shs && a.prm.M == 4) launch_project_bwd<4, false, false, true>(a, g_begin, g_end, smem);
-    else if (a.frozen_rows) launch_project_bwd<0, false, false, true>(a, g_begin, g_end, smem);
-    else if (a.shs && a.prm.M == 16) launch_project_bwd<16>(a, g_begin, g_end, smem);
-    else if (a.shs && a.prm.M == 4) launch_project_bwd<4>(a, g_begin, g_end, smem);
-    else launch_project_bwd<0>(a, g_begin, g_end, smem);
+    const bool dyn = a.scene && a.scene->dyn_views;
+    const bool frozen = a.frozen_rows != nullptr;
+    // The STATS instantiation where it has work: the launch of the view that gathers, every launch that stores no
+    // d_means2D, and every launch under _dyn (and _live), whose kernels read the view to gather from device memory.
+    const bool stats = a.row_stats && (dyn || !a.d_means2D || a.view == a.row_stats->view);
+    // (the raw rows are staged with 4-byte copies whatever M is: no per-M instantiation under RAW)
+    if (a.scene && a.scene->live && frozen) launch_project_bwd<0, true, true, true, true, true>(a, smem);
+    else if (a.scene && a.scene->live) launch_project_bwd<0, true, true, false, true, true>(a, smem);
+    else if (dyn) launch_project_bwd_modes<0, true, true>(a, frozen, stats, smem);
+    else if (a.scene) launch_project_bwd_modes<0, true>(a, frozen, stats, smem);
+    else if (a.shs && a.prm.M == 16) launch_project_bwd_modes<16>(a, frozen, stats, smem);
+    else if (a.shs && a.prm.M == 4) launch_project_bwd_modes<4>(a, frozen, stats, smem);
+    else launch_project_bwd_modes<0>(a, frozen, stats, smem);
     return cudaGetLastError();
 }
 
