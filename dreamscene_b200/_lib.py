@@ -1,6 +1,7 @@
 """ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h,
 include/b200gsr_loss.h, include/b200gsr_frozen.h, include/b200gsr_stats.h,
-include/b200gsr_reserve.h, include/b200gsr_frames.h, include/b200gsr_views_frozen.h, include/b200gsr_views_stats.h).  Fails loudly if the library is missing:
+include/b200gsr_reserve.h, include/b200gsr_frames.h, include/b200gsr_views_frozen.h, include/b200gsr_views_stats.h,
+include/b200gsr_fields.h).  Fails loudly if the library is missing:
 there is NO CPU or PyTorch fallback in the product path."""
 from __future__ import annotations
 
@@ -218,6 +219,25 @@ VIEWS_STATS_SIGNATURES = {
                                      [sz, u64, _P(ViewGrads), u32, _P(RowRange), i32, _P(RowStats), i32, i32, vp]),
 }
 
+
+class FieldsLayout(C.Structure):    # == b200gsr_fields_layout (include/b200gsr_fields.h)
+    _fields_ = [("total", C.c_size_t), ("blocks_per_axis", C.c_int32), ("max_blocks_per_axis", C.c_int32),
+                ("max_pairs", C.c_int64)]
+
+
+class FieldsInfo(C.Structure):      # == b200gsr_fields_info (include/b200gsr_fields.h)
+    _fields_ = [("scale", C.c_double), ("center", C.c_float * 3), ("extent", C.c_float), ("kept", C.c_int32),
+                ("overflow", C.c_uint32), ("pairs", C.c_int64)]
+
+
+# The opacity-field entry points of include/b200gsr_fields.h (same library), in that header's order.
+FIELDS_SIGNATURES = {
+    "b200gsr_fields_layout_query": (C.c_int, [i32, i32, i32, C.c_double, vp, _P(FieldsLayout)]),
+    "b200gsr_fields": (C.c_int, [i32, vp, vp, vp, vp, i32, i32, C.c_double, vp, vp, vp, vp, sz, vp]),
+}
+FIELDS_MAX_R = 1024                 # B200GSR_FIELDS_MAX_R
+FIELDS_MAX_CHUNKS = 32              # B200GSR_FIELDS_MAX_CHUNKS
+
 _lib = None
 ABI_VERSION = 3
 ERR_BAD_ARG = -1
@@ -248,7 +268,8 @@ def load():
     lib = C.CDLL(LIB_PATH)
     for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES, **STEP_SIGNATURES, **LOSS_SIGNATURES,
                                       **FROZEN_SIGNATURES, **STATS_SIGNATURES, **RESERVE_SIGNATURES,
-                                      **FRAMES_SIGNATURES, **VIEWS_FROZEN_SIGNATURES, **VIEWS_STATS_SIGNATURES}.items():
+                                      **FRAMES_SIGNATURES, **VIEWS_FROZEN_SIGNATURES, **VIEWS_STATS_SIGNATURES,
+                                      **FIELDS_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:

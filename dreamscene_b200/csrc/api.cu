@@ -1,4 +1,4 @@
-// C ABI (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h, include/b200gsr_loss.h): argument
+// C ABI (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h, include/b200gsr_loss.h, ...): argument
 // validation, buffer layouts, launch sequencing.
 #include "common.cuh"
 #include "../../include/b200gsr_step.h"
@@ -9,7 +9,9 @@
 #include "../../include/b200gsr_frames.h"
 #include "../../include/b200gsr_views_frozen.h"
 #include "../../include/b200gsr_views_stats.h"
+#include "../../include/b200gsr_fields.h"
 
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -834,6 +836,62 @@ int b200gsr_frames(int32_t B, int32_t H, int32_t W, const float* color, const fl
     if (!ds) return fail(B200GSR_ERR_CUDA, "cannot query the current CUDA device");
     return check_cuda(gsr_launch_frames(B, H, W, (int)Hs, color, depth_alpha, focal, rgb8, depth8, stats, ds->num_sms,
                                         static_cast<cudaStream_t>(stream)), "frames");
+}
+
+// Opacity field (include/b200gsr_fields.h): every refusal before the plan reads coords, the plan's own limits after.
+static int fields_plan(int32_t P, int32_t R, int32_t num_blocks, double relax_ratio, const float* coords,
+                       GsrFieldsPlan* pl) {
+    if (P < 1) return fail(B200GSR_ERR_BAD_ARG, "fields: P = %d, need at least one row", P);
+    if (R < 1 || R > B200GSR_FIELDS_MAX_R)
+        return fail(B200GSR_ERR_BAD_ARG, "fields: resolution %d not in 1..%d", R, B200GSR_FIELDS_MAX_R);
+    if (num_blocks < 1 || num_blocks > R)
+        return fail(B200GSR_ERR_BAD_ARG, "fields: num_blocks %d not in 1..resolution %d", num_blocks, R);
+    if (std::fmod((double)R, 2.0 / num_blocks) != 0.0)
+        return fail(B200GSR_ERR_BAD_ARG, "fields: resolution %d is not a multiple of the block size 2 / %d", R, num_blocks);
+    const int split = R / num_blocks, C = (R + split - 1) / split;
+    if (C > B200GSR_FIELDS_MAX_CHUNKS)
+        return fail(B200GSR_ERR_BAD_ARG, "fields: %d chunks per axis, at most %d", C, B200GSR_FIELDS_MAX_CHUNKS);
+    if (!std::isfinite(relax_ratio)) return fail(B200GSR_ERR_BAD_ARG, "fields: relax_ratio must be finite");
+    if (!coords) return fail(B200GSR_ERR_BAD_ARG, "fields: coords is null");
+    for (int i = 0; i < R; ++i)
+        if (!std::isfinite(coords[i])) return fail(B200GSR_ERR_BAD_ARG, "fields: coords[%d] is not finite", i);
+    gsr_fields_plan(P, R, num_blocks, relax_ratio, coords, pl);
+    if (pl->max_pairs >= (1ll << 31))
+        return fail(B200GSR_ERR_BAD_ARG, "fields: %d rows x %d^3 blocks per row is too large", P, pl->max_per_axis);
+    if ((long long)pl->nblk * pl->nchunks >= (1ll << 31))
+        return fail(B200GSR_ERR_BAD_ARG, "fields: %d blocks x %d row chunks is too large", pl->nblk, pl->nchunks);
+    return B200GSR_OK;
+}
+
+int b200gsr_fields_layout_query(int32_t P, int32_t R, int32_t num_blocks, double relax_ratio, const float* coords,
+                                b200gsr_fields_layout* out) {
+    if (!out) return fail(B200GSR_ERR_BAD_ARG, "fields: out is null");
+    GsrFieldsPlan pl;
+    if (int rc = fields_plan(P, R, num_blocks, relax_ratio, coords, &pl)) return rc;
+    out->total = pl.total;
+    out->blocks_per_axis = pl.C;
+    out->max_blocks_per_axis = pl.max_per_axis;
+    out->max_pairs = pl.max_pairs;
+    return B200GSR_OK;
+}
+
+int b200gsr_fields(int32_t P, const float* xyz, const float* opacity, const float* scaling, const float* rotation,
+                   int32_t R, int32_t num_blocks, double relax_ratio, const float* coords, float* occ,
+                   b200gsr_fields_info* info, void* scratch, size_t scratch_bytes, void* stream) {
+    GsrFieldsPlan pl;
+    if (int rc = fields_plan(P, R, num_blocks, relax_ratio, coords, &pl)) return rc;
+    if (!xyz || !opacity || !scaling || !rotation || !occ || !info || !scratch)
+        return fail(B200GSR_ERR_BAD_ARG, "fields: null pointer");
+    if (reinterpret_cast<uintptr_t>(rotation) & 15u) return fail(B200GSR_ERR_BAD_ARG, "fields: rotation must be 16-byte aligned");
+    if (reinterpret_cast<uintptr_t>(info) & 7u) return fail(B200GSR_ERR_BAD_ARG, "fields: info must be 8-byte aligned");
+    if (reinterpret_cast<uintptr_t>(scratch) & 255u) return fail(B200GSR_ERR_BAD_ARG, "fields: scratch must be 256-byte aligned");
+    if (scratch_bytes < pl.total)
+        return fail(B200GSR_ERR_BAD_ARG, "fields: scratch holds %zu bytes, need %zu", scratch_bytes, pl.total);
+    DeviceState* ds = device_state();
+    if (!ds) return fail(B200GSR_ERR_CUDA, "cannot query the current CUDA device");
+    return check_cuda(gsr_launch_fields(pl, coords, xyz, opacity, scaling, rotation, occ, info,
+                                        static_cast<uint8_t*>(scratch), ds->num_sms, static_cast<cudaStream_t>(stream)),
+                      "fields");
 }
 
 #define GSR_ST(x) static_cast<cudaStream_t>(x)

@@ -7,6 +7,7 @@
 #include "../../include/b200gsr_reserve.h"
 #include "../../include/b200gsr_views_frozen.h"
 #include "../../include/b200gsr_views_stats.h"
+#include "../../include/b200gsr_fields.h"
 
 #define GSR_TILE 16
 #define GSR_NEAR_Z 0.2f
@@ -222,6 +223,9 @@ __device__ __forceinline__ float gsr_screen_grad_norm(float gx, float gy) {
     return __fsqrt_rn(s);
 }
 
+// torch's float32 sigmoid on CUDA, 1 / (1 + exp(-x)) with every step rounded to nearest (densify.cu, fields.cu)
+__device__ __forceinline__ float gsr_sigmoid_rn(float x) { return __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-x))); }
+
 // ---- shared-memory address helper (cp.async destinations) ----------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return (uint32_t)__cvta_generic_to_shared(p);
@@ -388,6 +392,25 @@ cudaError_t gsr_split_children(int n_out, int first_child, float child_div, cons
                                const float* xyz, const float* scaling, const float* rotation, const float* z,
                                float* xyz_out, float* scaling_out, cudaStream_t s);
 cudaError_t gsr_kth_smallest(int n, const float* v, uint32_t k, void* scratch, float* out, int num_sms, cudaStream_t s);
+
+// exclusive prefix sum of n uint32 (densify.cu): out may be in; bsums holds (n + 4095) / 4096 words; *total = the sum
+void gsr_scan_u32(int n, const uint32_t* in, uint32_t* out, uint32_t* bsums, uint32_t* total, cudaStream_t s);
+
+// ---- opacity field on a voxel grid (fields.cu; b200gsr_fields) -------------------------------------------------
+// Everything the host decides from (P, R, num_blocks, relax_ratio, coords): the chunking, the block boxes on one axis
+// (the same on all three) and the scratch layout.
+struct GsrFieldsPlan {
+    int P, R, split, C, nblk, nchunks, max_per_axis;
+    float r;
+    float lo[B200GSR_FIELDS_MAX_CHUNKS], hi[B200GSR_FIELDS_MAX_CHUNKS];
+    long long max_pairs;
+    size_t off_state, off_grid, off_rec, off_mask, off_hist, off_bsums, off_members, total;
+};
+// Host only; the arguments must already be valid (b200gsr_fields_layout_query checks them).
+void gsr_fields_plan(int P, int R, int num_blocks, double relax_ratio, const float* coords, GsrFieldsPlan* plan);
+cudaError_t gsr_launch_fields(const GsrFieldsPlan& p, const float* coords, const float* xyz, const float* opacity,
+                              const float* scaling, const float* rotation, float* occ, b200gsr_fields_info* info,
+                              uint8_t* scratch, int num_sms, cudaStream_t s);
 
 // simple_knn replacement (knn.cu)
 size_t gsr_knn_scratch_bytes(int P, int* max_cells_out);

@@ -8,7 +8,7 @@
 //   densify_classify  per-Gaussian decisions of densify_and_prune, in the reference's order
 //                     (clone -> split -> prune, including that the stats arrays are reset in between,
 //                     so the screen-size criterion never fires inside densify_and_prune)
-//   scan_u32          exclusive prefix sum (two-level)
+//   gsr_scan_u32      exclusive prefix sum (two-level; fields.cu uses it too)
 //   densify_map       decisions + scans -> source map of the NEW point set, in the reference's
 //                     output order [kept originals | clones | split children (N blocks)]
 //   gather_rows       out[p,:] = in[src[p],:]  (or zeros for appended rows: Adam moments, stats)
@@ -31,8 +31,6 @@ __global__ void densify_stats_kernel(int P, const float* __restrict__ vs_grad, c
     denom[i] += 1.0f;
     if (max_radii != nullptr) max_radii[i] = fmaxf(max_radii[i], (float)r);
 }
-
-__device__ __forceinline__ float sigmoidf_rn(float x) { return __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-x))); }
 
 // A split child's log-scale, log(exp(s) / (0.8 N)) (gs_renderer.py:984-992).  torch divides a CUDA tensor by a CPU
 // scalar as a multiply by the fp32 reciprocal, inv = fp32(1 / fp32(0.8 N)); a true division differs in the last bit
@@ -59,7 +57,7 @@ __global__ void densify_classify_kernel(int P, const float* __restrict__ accum, 
     const float s = fmaxf(fmaxf(e0, e1), e2);
     const bool clone = (fabsf(g) >= max_grad) && (s <= dense_extent);
     const bool split = (g >= max_grad) && (s > dense_extent);
-    const bool low = sigmoidf_rn(opacity[i]) < min_opacity;
+    const bool low = gsr_sigmoid_rn(opacity[i]) < min_opacity;
     const bool pruned = low || (big_ws > 0.0f && s > big_ws);
     // the final prune sees the children's stored log-scales: max over the components of exp(child_log_scale(e_k))
     const float inv = __fdiv_rn(1.0f, child_div);
@@ -271,7 +269,7 @@ cudaError_t gsr_densify_stats(int P, const float* vs_grad, const int32_t* radii,
     return cudaGetLastError();
 }
 
-static void scan_u32(int n, const uint32_t* in, uint32_t* out, uint32_t* bsums, uint32_t* total, cudaStream_t s) {
+void gsr_scan_u32(int n, const uint32_t* in, uint32_t* out, uint32_t* bsums, uint32_t* total, cudaStream_t s) {
     const int nb = (n + 4095) / 4096;
     scan_blocks_kernel<<<nb, 1024, 0, s>>>(n, in, out, bsums);
     scan_sums_kernel<<<1, 1024, 0, s>>>(nb, bsums, total);
@@ -293,7 +291,7 @@ cudaError_t gsr_densify_plan(int P, const float* accum, const float* denom, cons
     uint32_t* bsums = offs + 4 * (size_t)P;
     densify_classify_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, accum, denom, scaling, opacity, max_grad, dense_extent,
                                                              min_opacity, big_ws, child_div, flags);
-    scan_u32(4 * P, flags, offs, bsums, totals5 + 4, s);
+    gsr_scan_u32(4 * P, flags, offs, bsums, totals5 + 4, s);
     plane_totals_kernel<<<1, 32, 0, s>>>(P, flags, offs, totals5);
     return cudaGetLastError();
 }
@@ -328,7 +326,7 @@ cudaError_t gsr_compact_plan(int P, const uint8_t* keep, void* scratch, int32_t*
     uint32_t* offs = flags + 4 * (size_t)P;
     uint32_t* bsums = offs + 4 * (size_t)P;
     mask_to_u32_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, keep, flags);
-    scan_u32(P, flags, offs, bsums, count, s);
+    gsr_scan_u32(P, flags, offs, bsums, count, s);
     compact_map_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, flags, offs, src_map);
     return cudaGetLastError();
 }
