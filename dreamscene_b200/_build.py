@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200gsr.so")
 SOURCES = ["api.cu", "project.cu", "binning.cu", "composite.cu", "knn.cu", "assemble.cu", "postprocess.cu", "densify.cu",
-           "optim.cu", "loss.cu", "fields.cu"]
+           "optim.cu", "loss.cu", "fields.cu", "mesh.cu"]
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "scene_math.cuh"),
            os.path.join(HERE, "..", "include", "b200gsr.h"), os.path.join(HERE, "..", "include", "b200gsr_scene.h"),
            os.path.join(HERE, "..", "include", "b200gsr_step.h"), os.path.join(HERE, "..", "include", "b200gsr_loss.h"),
@@ -19,7 +19,8 @@ HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "scene_math.cuh"
            os.path.join(HERE, "..", "include", "b200gsr_frames.h"),
            os.path.join(HERE, "..", "include", "b200gsr_views_frozen.h"),
            os.path.join(HERE, "..", "include", "b200gsr_views_stats.h"),
-           os.path.join(HERE, "..", "include", "b200gsr_fields.h")]
+           os.path.join(HERE, "..", "include", "b200gsr_fields.h"),
+           os.path.join(HERE, "..", "include", "b200gsr_mesh.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

@@ -1,7 +1,7 @@
 """ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h,
 include/b200gsr_loss.h, include/b200gsr_frozen.h, include/b200gsr_stats.h,
 include/b200gsr_reserve.h, include/b200gsr_frames.h, include/b200gsr_views_frozen.h, include/b200gsr_views_stats.h,
-include/b200gsr_fields.h).  Fails loudly if the library is missing:
+include/b200gsr_fields.h, include/b200gsr_mesh.h).  Fails loudly if the library is missing:
 there is NO CPU or PyTorch fallback in the product path."""
 from __future__ import annotations
 
@@ -238,6 +238,21 @@ FIELDS_SIGNATURES = {
 FIELDS_MAX_R = 1024                 # B200GSR_FIELDS_MAX_R
 FIELDS_MAX_CHUNKS = 32              # B200GSR_FIELDS_MAX_CHUNKS
 
+
+class MeshLayout(C.Structure):      # == b200gsr_mesh_layout (include/b200gsr_mesh.h)
+    _fields_ = [("total", C.c_size_t), ("points", C.c_int64), ("cells", C.c_int64)]
+
+
+# The marching-cubes entry points of include/b200gsr_mesh.h (same library), in that header's order.
+MESH_SIGNATURES = {
+    "b200gsr_mesh_table": (C.c_int, [_P(C.c_uint8), _P(C.c_int8)]),
+    "b200gsr_mesh_layout_query": (C.c_int, [i32, i32, i32, _P(MeshLayout)]),
+    "b200gsr_mesh_count": (C.c_int, [i32, i32, i32, vp, f32, vp, vp, sz, vp]),
+    "b200gsr_mesh_emit": (C.c_int, [i32, i32, i32, vp, f32, vp, sz, vp, i32, vp, i32, vp]),
+}
+MESH_MAX_TRIANGLES = 5              # B200GSR_MESH_MAX_TRIANGLES
+MESH_TABLE_WIDTH = 15               # B200GSR_MESH_TABLE_WIDTH
+
 _lib = None
 ABI_VERSION = 3
 ERR_BAD_ARG = -1
@@ -269,7 +284,7 @@ def load():
     for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES, **STEP_SIGNATURES, **LOSS_SIGNATURES,
                                       **FROZEN_SIGNATURES, **STATS_SIGNATURES, **RESERVE_SIGNATURES,
                                       **FRAMES_SIGNATURES, **VIEWS_FROZEN_SIGNATURES, **VIEWS_STATS_SIGNATURES,
-                                      **FIELDS_SIGNATURES}.items():
+                                      **FIELDS_SIGNATURES, **MESH_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:

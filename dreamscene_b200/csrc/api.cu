@@ -10,6 +10,7 @@
 #include "../../include/b200gsr_views_frozen.h"
 #include "../../include/b200gsr_views_stats.h"
 #include "../../include/b200gsr_fields.h"
+#include "../../include/b200gsr_mesh.h"
 
 #include <cmath>
 #include <cstdarg>
@@ -892,6 +893,71 @@ int b200gsr_fields(int32_t P, const float* xyz, const float* opacity, const floa
     return check_cuda(gsr_launch_fields(pl, coords, xyz, opacity, scaling, rotation, occ, info,
                                         static_cast<uint8_t*>(scratch), ds->num_sms, static_cast<cudaStream_t>(stream)),
                       "fields");
+}
+
+// Marching cubes (include/b200gsr_mesh.h): the grid's limits first, then the call's own arguments.
+int b200gsr_mesh_table(uint8_t* counts, int8_t* edges) {
+    if (!counts || !edges) return fail(B200GSR_ERR_BAD_ARG, "mesh: null pointer");
+    gsr_mesh_table(counts, edges);
+    return B200GSR_OK;
+}
+
+static int mesh_plan(int32_t X, int32_t Y, int32_t Z, GsrMeshPlan* pl) {
+    for (int32_t d : {X, Y, Z})
+        if (d < 1 || d > B200GSR_FIELDS_MAX_R)
+            return fail(B200GSR_ERR_BAD_ARG, "mesh: dimension %d not in 1..%d", d, B200GSR_FIELDS_MAX_R);
+    gsr_mesh_plan(X, Y, Z, pl);
+    if (3 * pl->points >= (1ll << 31))
+        return fail(B200GSR_ERR_BAD_ARG, "mesh: %d x %d x %d points is too large (3 X Y Z must be below 2^31)", X, Y, Z);
+    if (B200GSR_MESH_MAX_TRIANGLES * pl->cells >= (1ll << 31))
+        return fail(B200GSR_ERR_BAD_ARG, "mesh: %lld cells is too large (%d per cell must stay below 2^31)", pl->cells,
+                    B200GSR_MESH_MAX_TRIANGLES);
+    return B200GSR_OK;
+}
+
+int b200gsr_mesh_layout_query(int32_t X, int32_t Y, int32_t Z, b200gsr_mesh_layout* out) {
+    if (!out) return fail(B200GSR_ERR_BAD_ARG, "mesh: out is null");
+    GsrMeshPlan pl;
+    if (int rc = mesh_plan(X, Y, Z, &pl)) return rc;
+    out->total = pl.total;
+    out->points = pl.points;
+    out->cells = pl.cells;
+    return B200GSR_OK;
+}
+
+static int mesh_check(int32_t X, int32_t Y, int32_t Z, const float* volume, float iso, const void* scratch,
+                      size_t scratch_bytes, GsrMeshPlan* pl) {
+    if (int rc = mesh_plan(X, Y, Z, pl)) return rc;
+    if (!std::isfinite(iso)) return fail(B200GSR_ERR_BAD_ARG, "mesh: iso must be finite");
+    if (!volume || !scratch) return fail(B200GSR_ERR_BAD_ARG, "mesh: null pointer");
+    if (reinterpret_cast<uintptr_t>(volume) & 3u) return fail(B200GSR_ERR_BAD_ARG, "mesh: volume must be 4-byte aligned");
+    if (reinterpret_cast<uintptr_t>(scratch) & 255u) return fail(B200GSR_ERR_BAD_ARG, "mesh: scratch must be 256-byte aligned");
+    if (scratch_bytes < pl->total)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh: scratch holds %zu bytes, need %zu", scratch_bytes, pl->total);
+    return B200GSR_OK;
+}
+
+int b200gsr_mesh_count(int32_t X, int32_t Y, int32_t Z, const float* volume, float iso, int32_t* totals, void* scratch,
+                       size_t scratch_bytes, void* stream) {
+    GsrMeshPlan pl;
+    if (int rc = mesh_check(X, Y, Z, volume, iso, scratch, scratch_bytes, &pl)) return rc;
+    if (!totals) return fail(B200GSR_ERR_BAD_ARG, "mesh: null pointer");
+    if (reinterpret_cast<uintptr_t>(totals) & 3u) return fail(B200GSR_ERR_BAD_ARG, "mesh: totals must be 4-byte aligned");
+    return check_cuda(gsr_launch_mesh_count(pl, volume, iso, totals, static_cast<uint8_t*>(scratch), static_cast<cudaStream_t>(stream)),
+                      "mesh_count");
+}
+
+int b200gsr_mesh_emit(int32_t X, int32_t Y, int32_t Z, const float* volume, float iso, const void* scratch,
+                      size_t scratch_bytes, float* vertices, int32_t V, int32_t* faces, int32_t F, void* stream) {
+    GsrMeshPlan pl;
+    if (int rc = mesh_check(X, Y, Z, volume, iso, scratch, scratch_bytes, &pl)) return rc;
+    if (!vertices || !faces) return fail(B200GSR_ERR_BAD_ARG, "mesh: null pointer");
+    if ((reinterpret_cast<uintptr_t>(vertices) | reinterpret_cast<uintptr_t>(faces)) & 3u)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh: vertices and faces must be 4-byte aligned");
+    if (V < 0 || F < 0) return fail(B200GSR_ERR_BAD_ARG, "mesh: V = %d, F = %d, need V, F >= 0", V, F);
+    return check_cuda(gsr_launch_mesh_emit(pl, volume, iso, static_cast<const uint8_t*>(scratch), vertices, V, faces, F,
+                                           static_cast<cudaStream_t>(stream)),
+                      "mesh_emit");
 }
 
 #define GSR_ST(x) static_cast<cudaStream_t>(x)

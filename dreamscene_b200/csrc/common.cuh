@@ -412,6 +412,22 @@ cudaError_t gsr_launch_fields(const GsrFieldsPlan& p, const float* coords, const
                               const float* scaling, const float* rotation, float* occ, b200gsr_fields_info* info,
                               uint8_t* scratch, int num_sms, cudaStream_t s);
 
+// ---- marching cubes (mesh.cu; b200gsr_mesh_*) ------------------------------------------------------------------
+// The scratch layout of an X x Y x Z volume.
+struct GsrMeshPlan {
+    int X, Y, Z;
+    long long points, cells;
+    size_t off_emask, off_cube, off_vstart, off_fstart, off_bsums, total;
+};
+// Host only: the cube table the kernels use (counts[256], edges[256 * B200GSR_MESH_TABLE_WIDTH]) and the plan of
+// already valid dimensions (b200gsr_mesh_layout_query checks them).
+void gsr_mesh_table(uint8_t* counts, int8_t* edges);
+void gsr_mesh_plan(int X, int Y, int Z, GsrMeshPlan* plan);
+cudaError_t gsr_launch_mesh_count(const GsrMeshPlan& p, const float* vol, float iso, int32_t* totals, uint8_t* scratch,
+                                  cudaStream_t s);
+cudaError_t gsr_launch_mesh_emit(const GsrMeshPlan& p, const float* vol, float iso, const uint8_t* scratch,
+                                 float* vertices, int32_t V, int32_t* faces, int32_t F, cudaStream_t s);
+
 // simple_knn replacement (knn.cu)
 size_t gsr_knn_scratch_bytes(int P, int* max_cells_out);
 cudaError_t gsr_launch_knn(int P, const float* pts, float* out, uint8_t* scratch, cudaStream_t s);

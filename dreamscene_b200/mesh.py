@@ -1,0 +1,76 @@
+"""Triangle meshes from volumes on the device: marching cubes (include/b200gsr_mesh.h), and the mesh of a Gaussian
+group's opacity field.
+
+``marching_cubes(volume, iso)`` puts a vertex on every grid edge the iso-surface crosses, at the same position as
+``mcubes.marching_cubes(volume, iso)`` does, and triangulates each cell from a cube table generated from one face rule,
+so the surface is crack-free and consistently oriented (counter-clockwise seen from outside, the OBJ / PLY convention).
+The triangulation is not mcubes' table, so the faces differ from mcubes' faces.  ``extract_mesh(group)`` evaluates the
+group's opacity field with ``fields.extract_fields`` and marches it, without the field leaving the device.
+"""
+from __future__ import annotations
+
+import ctypes as C
+from typing import Tuple
+
+import torch
+
+from . import _lib
+from .fields import extract_fields
+
+
+def marching_cubes(volume: torch.Tensor, iso: float) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The iso-surface of a float32 CUDA volume [X,Y,Z] at `iso`.
+
+    -> (vertices float32 CUDA [V,3], faces int32 CUDA [F,3]).  Vertices are in index space: the vertex on the edge
+    from grid point p along axis a is p with coordinate a replaced by p_a + (iso - v[p]) / (v[p + e_a] - v[p]), each
+    operation rounded to float32.  There is one vertex per crossing edge, shared by the cells around it, ordered by
+    the grid point's linear index and then the axis; faces come cell by cell in linear order.  A point is inside when
+    its value is > iso (NaN is outside); iso is rounded to float32.  A dimension below 2, or an iso nothing crosses,
+    gives V = F = 0.  Two calls give the same bits.
+
+    Refused with ValueError: a CPU tensor, a volume that is not 3-D or not float32, a dimension above 1024 or a grid
+    too large to index with int32 (3 X Y Z >= 2^31), and a non-finite iso.  The call reads the two totals back to
+    allocate the outputs, so it waits for the device and cannot be captured into a CUDA graph (RuntimeError)."""
+    if not isinstance(volume, torch.Tensor):
+        raise ValueError(f"marching_cubes: volume must be a torch tensor, got {type(volume).__name__}")
+    if volume.dim() != 3:
+        raise ValueError(f"marching_cubes: volume must be 3-D [X,Y,Z], got shape {tuple(volume.shape)}")
+    if volume.dtype != torch.float32:
+        raise ValueError(f"marching_cubes: volume must be float32, got {volume.dtype}")
+    if volume.device.type != "cuda":
+        raise ValueError("marching_cubes (b200gsr): volume must be a CUDA tensor; there is no CPU fallback")
+    if torch.cuda.is_current_stream_capturing():
+        raise RuntimeError("marching_cubes reads its totals back to the host, so it cannot be captured into a CUDA graph")
+    X, Y, Z = (int(d) for d in volume.shape)
+    dev = volume.device
+    lib = _lib.load()
+    layout = _lib.MeshLayout()
+    _lib.check(lib.b200gsr_mesh_layout_query(X, Y, Z, C.byref(layout)), "b200gsr_mesh_layout_query", ValueError)
+    with torch.no_grad(), torch.cuda.device(dev):
+        vol = volume.detach().contiguous()
+        totals = torch.empty(2, dtype=torch.int32, device=dev)
+        scratch = torch.empty(layout.total, dtype=torch.uint8, device=dev)
+        ptr, st = _lib.ptr, _lib.stream(dev)
+        _lib.check(lib.b200gsr_mesh_count(X, Y, Z, ptr(vol), iso, ptr(totals), ptr(scratch), scratch.numel(), st),
+                   "b200gsr_mesh_count", ValueError)
+        V, F = (int(n) for n in totals.tolist())          # the call's one host sync
+        vertices = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        faces = torch.empty((F, 3), dtype=torch.int32, device=dev)
+        if V:
+            _lib.check(lib.b200gsr_mesh_emit(X, Y, Z, ptr(vol), iso, ptr(scratch), scratch.numel(), ptr(vertices), V,
+                                             ptr(faces), F, st), "b200gsr_mesh_emit", ValueError)
+    return vertices, faces
+
+
+def extract_mesh(group, resolution: int = 128, iso: float = 1.0, num_blocks: int = 16,
+                 relax_ratio: float = 1.5) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The mesh of a Gaussian group's opacity field: extract_fields(group, resolution, num_blocks, relax_ratio), then
+    marching_cubes(occ, iso), as DreamGaussian's extract_mesh does with mcubes on the host.
+
+    group accepts what extract_fields accepts (a plain group or ReservedGroup.rows()) and is refused as it refuses.
+    -> (vertices float32 CUDA [V,3] in world space, faces int32 CUDA [F,3]): the index-space vertices v mapped with
+    torch float32 operations as (v / (R - 1) * 2 - 1) / scale + center, the normalisation extract_fields returns.
+    Same faces and orientation as marching_cubes.  Waits for the device; no gradients."""
+    occ, center, scale = extract_fields(group, resolution, num_blocks, relax_ratio)
+    vertices, faces = marching_cubes(occ, iso)
+    return (vertices / (int(resolution) - 1) * 2 - 1) / scale + center, faces
