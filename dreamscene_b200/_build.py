@@ -20,7 +20,8 @@ HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "scene_math.cuh"
            os.path.join(HERE, "..", "include", "b200gsr_views_frozen.h"),
            os.path.join(HERE, "..", "include", "b200gsr_views_stats.h"),
            os.path.join(HERE, "..", "include", "b200gsr_fields.h"),
-           os.path.join(HERE, "..", "include", "b200gsr_mesh.h")]
+           os.path.join(HERE, "..", "include", "b200gsr_mesh.h"),
+           os.path.join(HERE, "..", "include", "b200gsr_mesh_colour.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

@@ -1,8 +1,8 @@
 """ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h,
 include/b200gsr_loss.h, include/b200gsr_frozen.h, include/b200gsr_stats.h,
 include/b200gsr_reserve.h, include/b200gsr_frames.h, include/b200gsr_views_frozen.h, include/b200gsr_views_stats.h,
-include/b200gsr_fields.h, include/b200gsr_mesh.h).  Fails loudly if the library is missing:
-there is NO CPU or PyTorch fallback in the product path."""
+include/b200gsr_fields.h, include/b200gsr_mesh.h, include/b200gsr_mesh_colour.h).  Fails loudly if the library is
+missing: there is NO CPU or PyTorch fallback in the product path."""
 from __future__ import annotations
 
 import ctypes as C
@@ -253,6 +253,14 @@ MESH_SIGNATURES = {
 MESH_MAX_TRIANGLES = 5              # B200GSR_MESH_MAX_TRIANGLES
 MESH_TABLE_WIDTH = 15               # B200GSR_MESH_TABLE_WIDTH
 
+# The colour-field and vertex-attribute entry points of include/b200gsr_mesh_colour.h (same library), in that header's
+# order.
+MESH_COLOUR_SIGNATURES = {
+    "b200gsr_fields_rgb_layout_query": (C.c_int, [i32, i32, i32, C.c_double, vp, _P(FieldsLayout)]),
+    "b200gsr_fields_rgb": (C.c_int, [i32, vp, vp, vp, vp, vp, i32, i32, C.c_double, vp, vp, vp, vp, vp, sz, vp]),
+    "b200gsr_mesh_attributes": (C.c_int, [i32, i32, i32, vp, f32, vp, sz, vp, vp, i32, vp]),
+}
+
 _lib = None
 ABI_VERSION = 3
 ERR_BAD_ARG = -1
@@ -284,7 +292,7 @@ def load():
     for name, (restype, argtypes) in {**SIGNATURES, **SCENE_SIGNATURES, **STEP_SIGNATURES, **LOSS_SIGNATURES,
                                       **FROZEN_SIGNATURES, **STATS_SIGNATURES, **RESERVE_SIGNATURES,
                                       **FRAMES_SIGNATURES, **VIEWS_FROZEN_SIGNATURES, **VIEWS_STATS_SIGNATURES,
-                                      **FIELDS_SIGNATURES, **MESH_SIGNATURES}.items():
+                                      **FIELDS_SIGNATURES, **MESH_SIGNATURES, **MESH_COLOUR_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:

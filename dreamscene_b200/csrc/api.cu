@@ -11,6 +11,7 @@
 #include "../../include/b200gsr_views_stats.h"
 #include "../../include/b200gsr_fields.h"
 #include "../../include/b200gsr_mesh.h"
+#include "../../include/b200gsr_mesh_colour.h"
 
 #include <cmath>
 #include <cstdarg>
@@ -876,11 +877,10 @@ int b200gsr_fields_layout_query(int32_t P, int32_t R, int32_t num_blocks, double
     return B200GSR_OK;
 }
 
-int b200gsr_fields(int32_t P, const float* xyz, const float* opacity, const float* scaling, const float* rotation,
-                   int32_t R, int32_t num_blocks, double relax_ratio, const float* coords, float* occ,
-                   b200gsr_fields_info* info, void* scratch, size_t scratch_bytes, void* stream) {
-    GsrFieldsPlan pl;
-    if (int rc = fields_plan(P, R, num_blocks, relax_ratio, coords, &pl)) return rc;
+// The call's own arguments, after the plan: features_dc and rgb are both null for the opacity field alone.
+static int fields_run(const GsrFieldsPlan& pl, const float* coords, const float* xyz, const float* opacity,
+                      const float* scaling, const float* rotation, const float* features_dc, float* occ, float* rgb,
+                      b200gsr_fields_info* info, void* scratch, size_t scratch_bytes, void* stream) {
     if (!xyz || !opacity || !scaling || !rotation || !occ || !info || !scratch)
         return fail(B200GSR_ERR_BAD_ARG, "fields: null pointer");
     if (reinterpret_cast<uintptr_t>(rotation) & 15u) return fail(B200GSR_ERR_BAD_ARG, "fields: rotation must be 16-byte aligned");
@@ -890,9 +890,53 @@ int b200gsr_fields(int32_t P, const float* xyz, const float* opacity, const floa
         return fail(B200GSR_ERR_BAD_ARG, "fields: scratch holds %zu bytes, need %zu", scratch_bytes, pl.total);
     DeviceState* ds = device_state();
     if (!ds) return fail(B200GSR_ERR_CUDA, "cannot query the current CUDA device");
-    return check_cuda(gsr_launch_fields(pl, coords, xyz, opacity, scaling, rotation, occ, info,
+    return check_cuda(gsr_launch_fields(pl, coords, xyz, opacity, scaling, rotation, features_dc, occ, rgb, info,
                                         static_cast<uint8_t*>(scratch), ds->num_sms, static_cast<cudaStream_t>(stream)),
-                      "fields");
+                      rgb ? "fields_rgb" : "fields");
+}
+
+int b200gsr_fields(int32_t P, const float* xyz, const float* opacity, const float* scaling, const float* rotation,
+                   int32_t R, int32_t num_blocks, double relax_ratio, const float* coords, float* occ,
+                   b200gsr_fields_info* info, void* scratch, size_t scratch_bytes, void* stream) {
+    GsrFieldsPlan pl;
+    if (int rc = fields_plan(P, R, num_blocks, relax_ratio, coords, &pl)) return rc;
+    return fields_run(pl, coords, xyz, opacity, scaling, rotation, nullptr, occ, nullptr, info, scratch, scratch_bytes,
+                      stream);
+}
+
+// Colour field and vertex attributes (include/b200gsr_mesh_colour.h): the opacity field's plan and its refusals,
+// then the colour field's own limit; the attribute pass takes marching cubes' checks.
+static int fields_rgb_plan(int32_t P, int32_t R, int32_t num_blocks, double relax_ratio, const float* coords,
+                           GsrFieldsPlan* pl) {
+    if (int rc = fields_plan(P, R, num_blocks, relax_ratio, coords, pl)) return rc;
+    if (3 * (long long)R * R * R >= (1ll << 31))
+        return fail(B200GSR_ERR_BAD_ARG, "fields_rgb: resolution %d is too large (3 R^3 must be below 2^31)", R);
+    return B200GSR_OK;
+}
+
+int b200gsr_fields_rgb_layout_query(int32_t P, int32_t R, int32_t num_blocks, double relax_ratio, const float* coords,
+                                    b200gsr_fields_layout* out) {
+    if (!out) return fail(B200GSR_ERR_BAD_ARG, "fields: out is null");
+    GsrFieldsPlan pl;
+    if (int rc = fields_rgb_plan(P, R, num_blocks, relax_ratio, coords, &pl)) return rc;
+    out->total = pl.total;
+    out->blocks_per_axis = pl.C;
+    out->max_blocks_per_axis = pl.max_per_axis;
+    out->max_pairs = pl.max_pairs;
+    return B200GSR_OK;
+}
+
+int b200gsr_fields_rgb(int32_t P, const float* xyz, const float* opacity, const float* scaling, const float* rotation,
+                       const float* features_dc, int32_t R, int32_t num_blocks, double relax_ratio, const float* coords,
+                       float* occ, float* rgb, b200gsr_fields_info* info, void* scratch, size_t scratch_bytes,
+                       void* stream) {
+    GsrFieldsPlan pl;
+    if (int rc = fields_rgb_plan(P, R, num_blocks, relax_ratio, coords, &pl)) return rc;
+    if (!features_dc || !rgb) return fail(B200GSR_ERR_BAD_ARG, "fields: null pointer");
+    if ((reinterpret_cast<uintptr_t>(features_dc) | reinterpret_cast<uintptr_t>(rgb)) & 3u)
+        return fail(B200GSR_ERR_BAD_ARG, "fields: features_dc and rgb must be 4-byte aligned");
+    return fields_run(pl, coords, xyz, opacity, scaling, rotation, features_dc, occ, rgb, info, scratch, scratch_bytes,
+                      stream);
 }
 
 // Marching cubes (include/b200gsr_mesh.h): the grid's limits first, then the call's own arguments.
@@ -958,6 +1002,19 @@ int b200gsr_mesh_emit(int32_t X, int32_t Y, int32_t Z, const float* volume, floa
     return check_cuda(gsr_launch_mesh_emit(pl, volume, iso, static_cast<const uint8_t*>(scratch), vertices, V, faces, F,
                                            static_cast<cudaStream_t>(stream)),
                       "mesh_emit");
+}
+
+int b200gsr_mesh_attributes(int32_t X, int32_t Y, int32_t Z, const float* volume, float iso, const void* scratch,
+                            size_t scratch_bytes, const float* attributes, float* out, int32_t V, void* stream) {
+    GsrMeshPlan pl;
+    if (int rc = mesh_check(X, Y, Z, volume, iso, scratch, scratch_bytes, &pl)) return rc;
+    if (!attributes || !out) return fail(B200GSR_ERR_BAD_ARG, "mesh: null pointer");
+    if ((reinterpret_cast<uintptr_t>(attributes) | reinterpret_cast<uintptr_t>(out)) & 3u)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh: attributes and out must be 4-byte aligned");
+    if (V < 0) return fail(B200GSR_ERR_BAD_ARG, "mesh: V = %d, need V >= 0", V);
+    return check_cuda(gsr_launch_mesh_attributes(pl, volume, iso, static_cast<const uint8_t*>(scratch), attributes, out,
+                                                 V, static_cast<cudaStream_t>(stream)),
+                      "mesh_attributes");
 }
 
 #define GSR_ST(x) static_cast<cudaStream_t>(x)

@@ -406,11 +406,13 @@ struct GsrFieldsPlan {
     long long max_pairs;
     size_t off_state, off_grid, off_rec, off_mask, off_hist, off_bsums, off_members, total;
 };
-// Host only; the arguments must already be valid (b200gsr_fields_layout_query checks them).
+// Host only; the arguments must already be valid (b200gsr_fields_layout_query checks them).  With rgb set the
+// launch also writes the colour field of include/b200gsr_mesh_colour.h from features_dc; with rgb null it reads
+// neither.
 void gsr_fields_plan(int P, int R, int num_blocks, double relax_ratio, const float* coords, GsrFieldsPlan* plan);
 cudaError_t gsr_launch_fields(const GsrFieldsPlan& p, const float* coords, const float* xyz, const float* opacity,
-                              const float* scaling, const float* rotation, float* occ, b200gsr_fields_info* info,
-                              uint8_t* scratch, int num_sms, cudaStream_t s);
+                              const float* scaling, const float* rotation, const float* features_dc, float* occ,
+                              float* rgb, b200gsr_fields_info* info, uint8_t* scratch, int num_sms, cudaStream_t s);
 
 // ---- marching cubes (mesh.cu; b200gsr_mesh_*) ------------------------------------------------------------------
 // The scratch layout of an X x Y x Z volume.
@@ -427,6 +429,9 @@ cudaError_t gsr_launch_mesh_count(const GsrMeshPlan& p, const float* vol, float 
                                   cudaStream_t s);
 cudaError_t gsr_launch_mesh_emit(const GsrMeshPlan& p, const float* vol, float iso, const uint8_t* scratch,
                                  float* vertices, int32_t V, int32_t* faces, int32_t F, cudaStream_t s);
+// After gsr_launch_mesh_count: attributes [N,3] interpolated onto the vertices (include/b200gsr_mesh_colour.h)
+cudaError_t gsr_launch_mesh_attributes(const GsrMeshPlan& p, const float* vol, float iso, const uint8_t* scratch,
+                                       const float* attributes, float* out, int32_t V, cudaStream_t s);
 
 // simple_knn replacement (knn.cu)
 size_t gsr_knn_scratch_bytes(int P, int* max_cells_out);

@@ -10,6 +10,8 @@
 //   fields_scatter   one warp per row chunk walks its rows in order, so every block lists its members in row order
 //   fields_eval      one CTA per block: members staged through shared memory, each thread sums its grid points in
 //                    registers in list order, so the field is the same on every call
+//   fields_eval_rgb  the same, also summing the members' opacity-weighted colours beside occ and dividing them by it
+//                    (include/b200gsr_mesh_colour.h); each member's colour is made as it is staged
 #include "common.cuh"
 #include "../../include/b200gsr_fields.h"
 
@@ -209,10 +211,25 @@ __global__ void __launch_bounds__(32) fields_scatter_kernel(FieldsArgs a) {
     }
 }
 
-// One CTA per block; PT grid points per thread per pass, kEvalThreads * PT points per pass.
-template <int PT>
-__global__ void __launch_bounds__(kEvalThreads) fields_eval_kernel(FieldsArgs a) {
+// op * clamp_min(SH2RGB(dc), 0) per channel: torch's float32 dc * SH_C0 + 0.5 (two roundings), then the clamp, which
+// keeps NaN
+__device__ __forceinline__ float4 weighted_colour(float op, const float* __restrict__ dc) {
+    constexpr float kShC0 = 0.28209479177387814f;
+    float c[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const float v = __fadd_rn(__fmul_rn(dc[k], kShC0), 0.5f);
+        c[k] = __fmul_rn(op, v < 0.0f ? 0.0f : v);
+    }
+    return make_float4(c[0], c[1], c[2], 0.0f);
+}
+
+// One CTA per block; PT grid points per thread per pass, kEvalThreads * PT points per pass.  RGB adds three sums per
+// point beside acc, whose fmaf sequence it leaves as it is, so occ is the same bits with and without them.
+template <int PT, bool RGB>
+__device__ __forceinline__ void fields_eval(const FieldsArgs& a, const float* dc, float* rgb) {
     __shared__ float4 s0[kEvalThreads], s1[kEvalThreads], s2[kEvalThreads];
+    __shared__ float4 s3[kEvalThreads];      // RGB: op * colour of the staged members
     const int b = blockIdx.x, C = a.C, R = a.R, tid = threadIdx.x;
     const int bz = b % C, by = (b / C) % C, bx = b / (C * C);
     const int x0 = bx * a.split, y0 = by * a.split, z0 = bz * a.split;
@@ -222,7 +239,7 @@ __global__ void __launch_bounds__(kEvalThreads) fields_eval_kernel(FieldsArgs a)
     uint32_t end = b + 1 < a.nblk ? a.hist[(size_t)(b + 1) * a.nchunks] : a.state->total;
     if (a.state->overflow) end = start;
     for (int pbase = 0; pbase < npts; pbase += kEvalThreads * PT) {
-        float px[PT], py[PT], pz[PT], acc[PT];
+        float px[PT], py[PT], pz[PT], acc[PT], cr[RGB ? PT : 1], cg[RGB ? PT : 1], cb[RGB ? PT : 1];
         size_t out[PT];
 #pragma unroll
         for (int k = 0; k < PT; ++k) {
@@ -234,6 +251,7 @@ __global__ void __launch_bounds__(kEvalThreads) fields_eval_kernel(FieldsArgs a)
             pz[k] = valid ? a.grid[z0 + l] : 0.0f;
             out[k] = valid ? ((size_t)(x0 + i) * R + (y0 + j)) * R + (z0 + l) : ~(size_t)0;
             acc[k] = 0.0f;
+            if constexpr (RGB) cr[k] = cg[k] = cb[k] = 0.0f;
         }
         for (uint32_t m0 = start; m0 < end; m0 += kEvalThreads) {
             __syncthreads();
@@ -242,6 +260,7 @@ __global__ void __launch_bounds__(kEvalThreads) fields_eval_kernel(FieldsArgs a)
                 s0[tid] = a.rec[3 * r];
                 s1[tid] = a.rec[3 * r + 1];
                 s2[tid] = a.rec[3 * r + 2];
+                if constexpr (RGB) s3[tid] = weighted_colour(a.rec[3 * r].w, dc + 3 * r);
             }
             __syncthreads();
             const int n = (int)min((uint32_t)kEvalThreads, end - m0);
@@ -253,12 +272,27 @@ __global__ void __launch_bounds__(kEvalThreads) fields_eval_kernel(FieldsArgs a)
                     const float e = x * fmaf(g1.x, x, fmaf(g1.y, y, g1.z * z)) + y * fmaf(g1.w, y, g2.x * z) + g2.y * z * z;
                     const float w = e > 0.0f ? 0.0f : exp2f(e);          // power > 0: the reference's weight 0
                     acc[k] = fmaf(g0.w, w, acc[k]);
+                    if constexpr (RGB) {
+                        const float4 c = s3[j];
+                        cr[k] = fmaf(w, c.x, cr[k]);
+                        cg[k] = fmaf(w, c.y, cg[k]);
+                        cb[k] = fmaf(w, c.z, cb[k]);
+                    }
                 }
             }
         }
 #pragma unroll
         for (int k = 0; k < PT; ++k)
-            if (out[k] != ~(size_t)0) a.occ[out[k]] = acc[k];
+            if (out[k] != ~(size_t)0) {
+                a.occ[out[k]] = acc[k];
+                if constexpr (RGB) {
+                    const bool empty = acc[k] == 0.0f;
+                    float* o = rgb + 3 * out[k];
+                    o[0] = empty ? 0.0f : __fdiv_rn(cr[k], acc[k]);
+                    o[1] = empty ? 0.0f : __fdiv_rn(cg[k], acc[k]);
+                    o[2] = empty ? 0.0f : __fdiv_rn(cb[k], acc[k]);
+                }
+            }
     }
     if (b == 0 && tid == 0) {
         a.info->pairs = (int64_t)a.state->total;
@@ -267,8 +301,20 @@ __global__ void __launch_bounds__(kEvalThreads) fields_eval_kernel(FieldsArgs a)
 }
 
 template <int PT>
-void launch_eval(const FieldsArgs& a, cudaStream_t s) {
-    fields_eval_kernel<PT><<<a.nblk, kEvalThreads, 0, s>>>(a);
+__global__ void __launch_bounds__(kEvalThreads) fields_eval_kernel(FieldsArgs a) {
+    fields_eval<PT, false>(a, nullptr, nullptr);
+}
+
+template <int PT>
+__global__ void __launch_bounds__(kEvalThreads) fields_eval_rgb_kernel(FieldsArgs a, const float* __restrict__ dc,
+                                                                       float* __restrict__ rgb) {
+    fields_eval<PT, true>(a, dc, rgb);
+}
+
+template <int PT>
+void launch_eval(const FieldsArgs& a, const float* dc, float* rgb, cudaStream_t s) {
+    if (rgb) fields_eval_rgb_kernel<PT><<<a.nblk, kEvalThreads, 0, s>>>(a, dc, rgb);
+    else fields_eval_kernel<PT><<<a.nblk, kEvalThreads, 0, s>>>(a);
 }
 
 size_t align256(size_t v) { return (v + 255) / 256 * 256; }
@@ -316,8 +362,8 @@ void gsr_fields_plan(int P, int R, int num_blocks, double relax_ratio, const flo
 }
 
 cudaError_t gsr_launch_fields(const GsrFieldsPlan& p, const float* coords, const float* xyz, const float* opacity,
-                              const float* scaling, const float* rotation, float* occ, b200gsr_fields_info* info,
-                              uint8_t* scratch, int num_sms, cudaStream_t s) {
+                              const float* scaling, const float* rotation, const float* features_dc, float* occ,
+                              float* rgb, b200gsr_fields_info* info, uint8_t* scratch, int num_sms, cudaStream_t s) {
     static_assert(sizeof(FieldsState) <= 16 * sizeof(uint32_t), "state must fit its slot");
     static std::atomic<unsigned long long> smem_count{0}, smem_scatter{0};
     FieldsArgs a;
@@ -363,10 +409,10 @@ cudaError_t gsr_launch_fields(const GsrFieldsPlan& p, const float* coords, const
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     // points per block: the first block is the largest
     const int pts = p.split * p.split * p.split, cover = pts < 16 * kEvalThreads ? pts : 16 * kEvalThreads;
-    if (cover <= kEvalThreads) launch_eval<1>(a, s);
-    else if (cover <= 2 * kEvalThreads) launch_eval<2>(a, s);
-    else if (cover <= 4 * kEvalThreads) launch_eval<4>(a, s);
-    else if (cover <= 8 * kEvalThreads) launch_eval<8>(a, s);
-    else launch_eval<16>(a, s);
+    if (cover <= kEvalThreads) launch_eval<1>(a, features_dc, rgb, s);
+    else if (cover <= 2 * kEvalThreads) launch_eval<2>(a, features_dc, rgb, s);
+    else if (cover <= 4 * kEvalThreads) launch_eval<4>(a, features_dc, rgb, s);
+    else if (cover <= 8 * kEvalThreads) launch_eval<8>(a, features_dc, rgb, s);
+    else launch_eval<16>(a, features_dc, rgb, s);
     return cudaGetLastError();
 }

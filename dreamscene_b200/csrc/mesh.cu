@@ -7,6 +7,8 @@
 //   mesh_vertices   per grid point: its vertices, in axis order, at its vertex offset
 //   mesh_faces      per cell: its triangles in table order at its face offset, each corner the vertex offset of the
 //                   edge's grid point plus the rank of the edge's axis among that point's crossing edges
+//   mesh_attributes per grid point: its vertices' attributes, interpolated with the vertices' t, at the same offsets
+//                   (include/b200gsr_mesh_colour.h)
 //
 // Built without fast-math: the interpolation is __fsub_rn / __fdiv_rn / __fadd_rn, one float32 rounding each.
 #include "common.cuh"
@@ -179,6 +181,31 @@ __global__ void __launch_bounds__(kThreads) mesh_faces_kernel(MeshArgs a, int32_
     }
 }
 
+// a + t (b - a) per channel, three roundings; t is mesh_vertices_kernel's, so each attribute sits where its vertex does
+__global__ void __launch_bounds__(kThreads) mesh_attributes_kernel(MeshArgs a, const float* __restrict__ attr,
+                                                                   float* __restrict__ out, uint32_t V) {
+    const int p = blockIdx.x * kThreads + threadIdx.x;
+    if (p >= a.N) return;
+    const uint32_t m = a.emask[p];
+    if (!m) return;
+    const int step[3] = {a.Y * a.Z, a.Z, 1};
+    const float f0 = a.vol[p], d0 = __fsub_rn(a.iso, f0);
+    const float* a0 = attr + 3 * (size_t)p;
+    uint32_t v = a.vstart[p];
+#pragma unroll
+    for (int ax = 0; ax < 3; ++ax) {
+        if (!(m >> ax & 1u)) continue;
+        const float t = __fdiv_rn(d0, __fsub_rn(a.vol[p + step[ax]], f0));
+        const float* a1 = a0 + 3 * (size_t)step[ax];
+        if (v < V) {
+            float* o = out + 3 * (size_t)v;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) o[c] = __fadd_rn(a0[c], __fmul_rn(t, __fsub_rn(a1[c], a0[c])));
+        }
+        ++v;
+    }
+}
+
 size_t align256(size_t v) { return (v + 255) / 256 * 256; }
 
 MeshArgs mesh_args(const GsrMeshPlan& p, const float* vol, float iso, uint8_t* scratch) {
@@ -235,5 +262,12 @@ cudaError_t gsr_launch_mesh_emit(const GsrMeshPlan& p, const float* vol, float i
     const int blocks = (a.N + kThreads - 1) / kThreads;
     mesh_vertices_kernel<<<blocks, kThreads, 0, s>>>(a, vertices, (uint32_t)V);
     mesh_faces_kernel<<<blocks, kThreads, 0, s>>>(a, faces, (uint32_t)F);
+    return cudaGetLastError();
+}
+
+cudaError_t gsr_launch_mesh_attributes(const GsrMeshPlan& p, const float* vol, float iso, const uint8_t* scratch,
+                                       const float* attributes, float* out, int32_t V, cudaStream_t s) {
+    MeshArgs a = mesh_args(p, vol, iso, const_cast<uint8_t*>(scratch));
+    mesh_attributes_kernel<<<(a.N + kThreads - 1) / kThreads, kThreads, 0, s>>>(a, attributes, out, (uint32_t)V);
     return cudaGetLastError();
 }

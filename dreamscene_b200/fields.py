@@ -4,7 +4,8 @@ DreamScene's extract_fields (gs_renderer.py) loops over num_blocks^3 grid blocks
 [points, Gaussians, 3] and [points, Gaussians, 6] tensors of every Gaussian near the block.  ``extract_fields(group)``
 computes the same field with one pass of kernels (include/b200gsr_fields.h): a filter and normalisation pass, a
 binning pass that lists every block's Gaussians in row order, and one CTA per block summing its grid points in
-registers.
+registers.  ``extract_fields_rgb(group)`` evaluates the group's colour field in the same pass: the opacity-weighted
+mean of the Gaussians' view-independent colours, which mesh.extract_coloured_mesh carries onto a mesh.
 """
 from __future__ import annotations
 
@@ -64,6 +65,43 @@ def extract_fields(group, resolution: int = 128, num_blocks: int = 16,
     Refused with ValueError: CPU tensors, bad sizes, no row passing the opacity filter, and kept centres that all
     coincide (the reference divides by zero).  The call waits for the device to read the normalisation back, so it
     cannot be captured into a CUDA graph.  No gradients."""
+    return _evaluate(group, resolution, num_blocks, relax_ratio, None)
+
+
+def extract_fields_rgb(group, resolution: int = 128, num_blocks: int = 16,
+                       relax_ratio: float = 1.5) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, float]:
+    """extract_fields(group, resolution, num_blocks, relax_ratio) and the group's colour field on the same grid.
+
+    group also needs _features_dc [P,1,3], the degree-0 SH coefficients, as a CUDA tensor on the leaves' device.
+    -> (occ [R,R,R], rgb float32 CUDA [R,R,R,3], center [3], scale): occ, center and scale are bit for bit what
+       extract_fields returns.  Each Gaussian's colour is c = clamp_min(_features_dc * SH_C0 + 0.5, 0), the reference's
+       SH2RGB clamped at 0 as the renderer clamps it, in float32: the mean of its SH colour over all view directions,
+       so the colour is view-independent.  rgb[i,j,k] = (sum of opacity * weight * c over the members occ sums, in
+       the same order) / occ[i,j,k], 0 where occ is 0: a weighted mean of the member colours, so every value lies
+       between the smallest and largest of them, up to rounding, where occ is not a tiny (subnormal-range) value.
+       It is not clamped above 1.  The sums are float32 in row order, the same bits on every call
+       (include/b200gsr_mesh_colour.h).
+
+    Refused with ValueError: what extract_fields refuses, a missing or misshapen _features_dc, and grids with
+    3 R^3 >= 2^31 (R above 894).  Waits for the device, as extract_fields does; no gradients."""
+    return _evaluate(group, resolution, num_blocks, relax_ratio, "extract_fields_rgb")
+
+
+def _features_dc(group, P, dev, what):
+    try:
+        dc = S._get(group, "_features_dc")
+    except (KeyError, AttributeError):
+        raise ValueError(f"{what}: the group has no _features_dc") from None
+    if not isinstance(dc, torch.Tensor) or tuple(dc.shape) != (P, 1, 3):
+        shape = tuple(dc.shape) if isinstance(dc, torch.Tensor) else type(dc).__name__
+        raise ValueError(f"{what}: _features_dc has shape {shape}, expected {(P, 1, 3)}")
+    if dc.device != dev:
+        raise ValueError(f"{what}: _features_dc must live on the leaves' device {dev}")
+    return dc
+
+
+def _evaluate(group, resolution, num_blocks, relax_ratio, rgb_of):
+    """The field of extract_fields and, when rgb_of names the caller, the colour field beside it."""
     resolution, num_blocks, relax_ratio = int(resolution), int(num_blocks), float(relax_ratio)
     if not 1 <= num_blocks <= resolution:
         raise ValueError(f"extract_fields: num_blocks must be in 1..resolution, got {num_blocks} for {resolution}")
@@ -72,21 +110,30 @@ def extract_fields(group, resolution: int = 128, num_blocks: int = 16,
                          f"{num_blocks} (the reference asserts resolution % block_size == 0)")
     leaves, P = _check_group(group)
     dev = leaves[0].device
+    dc = None if rgb_of is None else _features_dc(group, P, dev, rgb_of)
     coords = torch.linspace(-1, 1, resolution)          # torch's float32 coordinates, on the host
     lib = _lib.load()
     layout = _lib.FieldsLayout()
     cptr = C.c_void_p(coords.data_ptr())
-    _lib.check(lib.b200gsr_fields_layout_query(P, resolution, num_blocks, relax_ratio, cptr, C.byref(layout)),
-               "b200gsr_fields_layout_query", ValueError)
+    query = "b200gsr_fields_layout_query" if dc is None else "b200gsr_fields_rgb_layout_query"
+    _lib.check(getattr(lib, query)(P, resolution, num_blocks, relax_ratio, cptr, C.byref(layout)), query, ValueError)
     with torch.no_grad(), torch.cuda.device(dev):
         xyz, opacity, scaling, rotation = [_lib.prepare(t.detach()) for t in leaves]
         occ = torch.empty((resolution,) * 3, dtype=torch.float32, device=dev)
         info = torch.empty(C.sizeof(_lib.FieldsInfo), dtype=torch.uint8, device=dev)
         scratch = torch.empty(layout.total, dtype=torch.uint8, device=dev)
         ptr = _lib.ptr
-        _lib.check(lib.b200gsr_fields(P, ptr(xyz), ptr(opacity), ptr(scaling), ptr(rotation), resolution, num_blocks,
-                                      relax_ratio, cptr, ptr(occ), ptr(info), ptr(scratch), scratch.numel(),
-                                      _lib.stream(dev)), "b200gsr_fields", ValueError)
+        if dc is None:
+            _lib.check(lib.b200gsr_fields(P, ptr(xyz), ptr(opacity), ptr(scaling), ptr(rotation), resolution,
+                                          num_blocks, relax_ratio, cptr, ptr(occ), ptr(info), ptr(scratch),
+                                          scratch.numel(), _lib.stream(dev)), "b200gsr_fields", ValueError)
+        else:
+            dc = _lib.prepare(dc.detach())
+            rgb = torch.empty((resolution,) * 3 + (3,), dtype=torch.float32, device=dev)
+            _lib.check(lib.b200gsr_fields_rgb(P, ptr(xyz), ptr(opacity), ptr(scaling), ptr(rotation), ptr(dc),
+                                              resolution, num_blocks, relax_ratio, cptr, ptr(occ), ptr(rgb), ptr(info),
+                                              ptr(scratch), scratch.numel(), _lib.stream(dev)), "b200gsr_fields_rgb",
+                       ValueError)
         res = _lib.FieldsInfo.from_buffer_copy(bytes(info.cpu().numpy()))
     if res.kept == 0:
         raise ValueError("extract_fields: no Gaussian has opacity above 0.005")
@@ -94,4 +141,5 @@ def extract_fields(group, resolution: int = 128, num_blocks: int = 16,
         raise ValueError("extract_fields: every kept Gaussian has the same centre, so the field has no scale")
     if res.overflow:
         raise RuntimeError("extract_fields: the member lists overflowed their capacity")
-    return occ, torch.tensor(list(res.center), dtype=torch.float32, device=dev), float(res.scale)
+    center = torch.tensor(list(res.center), dtype=torch.float32, device=dev)
+    return (occ, center, float(res.scale)) if dc is None else (occ, rgb, center, float(res.scale))

@@ -6,19 +6,21 @@ group's opacity field.
 so the surface is crack-free and consistently oriented (counter-clockwise seen from outside, the OBJ / PLY convention).
 The triangulation is not mcubes' table, so the faces differ from mcubes' faces.  ``extract_mesh(group)`` evaluates the
 group's opacity field with ``fields.extract_fields`` and marches it, without the field leaving the device.
+``marching_cubes(volume, iso, attributes)`` also interpolates a per-point attribute volume onto the vertices, and
+``extract_coloured_mesh(group)`` uses it to colour the mesh with ``fields.extract_fields_rgb``'s colour field.
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Tuple
+from typing import Optional, Tuple
 
 import torch
 
 from . import _lib
-from .fields import extract_fields
+from .fields import extract_fields, extract_fields_rgb
 
 
-def marching_cubes(volume: torch.Tensor, iso: float) -> Tuple[torch.Tensor, torch.Tensor]:
+def marching_cubes(volume: torch.Tensor, iso: float, attributes: Optional[torch.Tensor] = None):
     """The iso-surface of a float32 CUDA volume [X,Y,Z] at `iso`.
 
     -> (vertices float32 CUDA [V,3], faces int32 CUDA [F,3]).  Vertices are in index space: the vertex on the edge
@@ -30,7 +32,13 @@ def marching_cubes(volume: torch.Tensor, iso: float) -> Tuple[torch.Tensor, torc
 
     Refused with ValueError: a CPU tensor, a volume that is not 3-D or not float32, a dimension above 1024 or a grid
     too large to index with int32 (3 X Y Z >= 2^31), and a non-finite iso.  The call reads the two totals back to
-    allocate the outputs, so it waits for the device and cannot be captured into a CUDA graph (RuntimeError)."""
+    allocate the outputs, so it waits for the device and cannot be captured into a CUDA graph (RuntimeError).
+
+    attributes: None, or a float32 CUDA tensor [X,Y,Z,3] on the volume's device, a value per grid point (a colour,
+    say).  Then the call returns (vertices, faces, vertex_attributes float32 CUDA [V,3]): the vertex on the edge from p
+    along axis a gets attributes[p] + t * (attributes[p + e_a] - attributes[p]) per channel, with the vertex's t and
+    each operation rounded to float32; a NaN t gives a NaN attribute.  It makes no further host sync.  A wrong shape,
+    dtype or device of attributes is refused with ValueError before any device work."""
     if not isinstance(volume, torch.Tensor):
         raise ValueError(f"marching_cubes: volume must be a torch tensor, got {type(volume).__name__}")
     if volume.dim() != 3:
@@ -43,6 +51,17 @@ def marching_cubes(volume: torch.Tensor, iso: float) -> Tuple[torch.Tensor, torc
         raise RuntimeError("marching_cubes reads its totals back to the host, so it cannot be captured into a CUDA graph")
     X, Y, Z = (int(d) for d in volume.shape)
     dev = volume.device
+    if attributes is not None:
+        if not isinstance(attributes, torch.Tensor):
+            raise ValueError(f"marching_cubes: attributes must be a torch tensor, got {type(attributes).__name__}")
+        if tuple(attributes.shape) != (X, Y, Z, 3):
+            raise ValueError(f"marching_cubes: attributes have shape {tuple(attributes.shape)}, "
+                             f"expected {(X, Y, Z, 3)}")
+        if attributes.dtype != torch.float32:
+            raise ValueError(f"marching_cubes: attributes must be float32, got {attributes.dtype}")
+        if attributes.device != dev:
+            raise ValueError(f"marching_cubes (b200gsr): attributes must be a CUDA tensor on the volume's device "
+                             f"{dev}; there is no CPU fallback")
     lib = _lib.load()
     layout = _lib.MeshLayout()
     _lib.check(lib.b200gsr_mesh_layout_query(X, Y, Z, C.byref(layout)), "b200gsr_mesh_layout_query", ValueError)
@@ -59,7 +78,14 @@ def marching_cubes(volume: torch.Tensor, iso: float) -> Tuple[torch.Tensor, torc
         if V:
             _lib.check(lib.b200gsr_mesh_emit(X, Y, Z, ptr(vol), iso, ptr(scratch), scratch.numel(), ptr(vertices), V,
                                              ptr(faces), F, st), "b200gsr_mesh_emit", ValueError)
-    return vertices, faces
+        if attributes is None:
+            return vertices, faces
+        attr = attributes.detach().contiguous()
+        out = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        if V:
+            _lib.check(lib.b200gsr_mesh_attributes(X, Y, Z, ptr(vol), iso, ptr(scratch), scratch.numel(), ptr(attr),
+                                                   ptr(out), V, st), "b200gsr_mesh_attributes", ValueError)
+    return vertices, faces, out
 
 
 def extract_mesh(group, resolution: int = 128, iso: float = 1.0, num_blocks: int = 16,
@@ -74,3 +100,18 @@ def extract_mesh(group, resolution: int = 128, iso: float = 1.0, num_blocks: int
     occ, center, scale = extract_fields(group, resolution, num_blocks, relax_ratio)
     vertices, faces = marching_cubes(occ, iso)
     return (vertices / (int(resolution) - 1) * 2 - 1) / scale + center, faces
+
+
+def extract_coloured_mesh(group, resolution: int = 128, iso: float = 1.0, num_blocks: int = 16,
+                          relax_ratio: float = 1.5) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """The mesh of extract_mesh(group, resolution, iso, num_blocks, relax_ratio), coloured.
+
+    extract_fields_rgb evaluates the opacity field and the colour field in one pass, and marching_cubes(occ, iso, rgb)
+    interpolates the colour field onto the vertices.  group accepts what extract_fields_rgb accepts (it needs
+    _features_dc [P,1,3]) and is refused as it refuses.
+    -> (vertices float32 CUDA [V,3] in world space, faces int32 CUDA [F,3], colours float32 CUDA [V,3]): vertices and
+    faces bit for bit extract_mesh's.  The colours are view-independent (each Gaussian's degree-0 SH colour, clamped
+    at 0 as the renderer clamps it) and not clamped above 1.  Waits for the device; no gradients."""
+    occ, rgb, center, scale = extract_fields_rgb(group, resolution, num_blocks, relax_ratio)
+    vertices, faces, colours = marching_cubes(occ, iso, rgb)
+    return (vertices / (int(resolution) - 1) * 2 - 1) / scale + center, faces, colours

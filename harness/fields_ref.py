@@ -152,3 +152,55 @@ def extract_fields(group, resolution=128, num_blocks=16, relax_ratio=1.5, dtype=
             val += (m_opa[:, start:end] * w.reshape(pts.shape[0], -1)).sum(-1)
         occ[x0:x0 + len(xs), y0:y0 + len(ys), z0:z0 + len(zs)] = val.reshape(len(xs), len(ys), len(zs))
     return occ, n["center"], n["scale"]
+
+
+# ---- the colour field of include/b200gsr_mesh_colour.h (dreamscene_b200.fields.extract_fields_rgb) ----------------
+SH_C0 = 0.28209479177387814          # the reference's utils/sh_utils.C0
+
+
+def sh2rgb(features_dc):
+    """Step 1: clamp_min(SH2RGB(_features_dc), 0) of [P,1,3] -> [P,3] float32, torch's float32 multiply by the Python
+    scalar, then its add, then the clamp (which keeps NaN)."""
+    return torch.clamp_min(features_dc.float()[:, 0] * SH_C0 + 0.5, 0)
+
+
+def extract_fields_rgb(group, resolution=128, num_blocks=16, relax_ratio=1.5, dtype=torch.float32, blocks=None):
+    """Step 2 beside extract_fields: -> (occ [R,R,R], rgb [R,R,R,3], both of `dtype`, center float32 [3], scale).
+
+    The same members, boxes and weights as extract_fields; rgb = (sum of opacity * weight * colour) / occ, 0 where
+    occ is 0.  The colours are step 1's float32 values in either dtype; with float64 the products and sums are float64.
+    blocks: an iterable of (xi, yi, zi) to evaluate (the others stay 0), or None for all."""
+    n = normalise(group)
+    mask, xyzs, opacities = n["mask"], n["xyz"], n["opacity"]
+    device = xyzs.device
+    rotation = _leaf(group, "_rotation")[mask]
+    colours = sh2rgb(_leaf(group, "_features_dc"))[mask].to(dtype)
+    if dtype == torch.float32:
+        stds = torch.exp(_leaf(group, "_scaling"))[mask] * n["scale"]
+        gxyz, opas = xyzs, opacities
+    else:
+        gxyz = (_leaf(group, "_xyz")[mask].to(dtype) - n["center"].to(dtype)) * n["scale"]
+        stds = torch.exp(_leaf(group, "_scaling")[mask].to(dtype)) * n["scale"]
+        opas = torch.sigmoid(_leaf(group, "_opacity")[mask].to(dtype))
+        rotation = rotation.to(dtype)
+    covs = covariance(stds, rotation)
+    occ = torch.zeros([resolution] * 3, dtype=dtype, device=device)
+    num = torch.zeros([resolution] * 3 + [3], dtype=dtype, device=device)
+    X = chunks(resolution, num_blocks)
+    wanted = None if blocks is None else set(map(tuple, blocks))
+    for (xi, yi, zi), (vmin, vmax) in block_boxes(resolution, num_blocks, relax_ratio, device).items():
+        if wanted is not None and (xi, yi, zi) not in wanted:
+            continue
+        (x0, xs), (y0, ys), (z0, zs) = X[xi], X[yi], X[zi]
+        member = (xyzs < vmax).all(-1) & (xyzs > vmin).all(-1)
+        if not member.any():
+            continue
+        pts = _points(xs, ys, zs).to(device=device, dtype=dtype)
+        d = pts.unsqueeze(1) - gxyz[member].unsqueeze(0)                                  # [points, members, 3]
+        w = gaussian_3d_coeff(d.reshape(-1, 3), covs[member].repeat(len(pts), 1)).view(len(pts), -1)
+        ow = opas[member].view(1, -1) * w
+        sl = (slice(x0, x0 + len(xs)), slice(y0, y0 + len(ys)), slice(z0, z0 + len(zs)))
+        occ[sl] = ow.sum(-1).view(len(xs), len(ys), len(zs))
+        num[sl] = (ow @ colours[member]).view(len(xs), len(ys), len(zs), 3)
+    rgb = torch.where(occ.unsqueeze(-1) > 0, num / occ.unsqueeze(-1), torch.zeros_like(num))
+    return occ, rgb, n["center"], n["scale"]

@@ -143,3 +143,26 @@ def marching_cubes(volume, iso):
     rank = np.bitwise_count((mask.reshape(-1)[q] & ((1 << ax) - 1)).astype(np.uint8)).astype(np.int64)
     faces = (vstart[q] + rank).astype(np.int32)
     return verts, faces.reshape(-1, 3)
+
+
+def vertex_attributes(volume, iso, attributes):
+    """-> [V,3] float32: step 4 of include/b200gsr_mesh_colour.h, the attributes [X,Y,Z,3] of a float32 volume's grid
+    points carried onto marching_cubes(volume, iso)'s vertices, in their order: a[p] + t * (a[p + e_a] - a[p]) per
+    channel with the vertex's t, each operation rounded to float32."""
+    vol = np.ascontiguousarray(volume, dtype=np.float32)
+    attr = np.ascontiguousarray(attributes, dtype=np.float32).reshape(-1, 3)
+    iso = np.float32(iso)
+    X, Y, Z = vol.shape
+    if min(X, Y, Z) < 2:
+        return np.zeros((0, 3), np.float32)
+    inside = vol > iso
+    mask = np.zeros((X, Y, Z), np.int64)
+    mask[:-1] |= (inside[:-1] != inside[1:]) * 1
+    mask[:, :-1] |= (inside[:, :-1] != inside[:, 1:]) * 2
+    mask[:, :, :-1] |= (inside[:, :, :-1] != inside[:, :, 1:]) * 4
+    pts, axes = np.nonzero(((mask.reshape(-1, 1) >> np.arange(3)) & 1).astype(bool))
+    q = pts + np.array([Y * Z, Z, 1])[axes]
+    f0 = vol.reshape(-1)[pts]
+    t = ((iso - f0) / (vol.reshape(-1)[q] - f0))[:, None]
+    a0, a1 = attr[pts], attr[q]
+    return a0 + t * (a1 - a0)
