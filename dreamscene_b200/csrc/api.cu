@@ -12,6 +12,7 @@
 #include "../../include/b200gsr_fields.h"
 #include "../../include/b200gsr_mesh.h"
 #include "../../include/b200gsr_mesh_colour.h"
+#include "../../include/b200gsr_mesh_clean.h"
 
 #include <cmath>
 #include <cstdarg>
@@ -1015,6 +1016,91 @@ int b200gsr_mesh_attributes(int32_t X, int32_t Y, int32_t Z, const float* volume
     return check_cuda(gsr_launch_mesh_attributes(pl, volume, iso, static_cast<const uint8_t*>(scratch), attributes, out,
                                                  V, static_cast<cudaStream_t>(stream)),
                       "mesh_attributes");
+}
+
+// Mesh components and cleaning (include/b200gsr_mesh_clean.h): the sizes first, then the pointers, then the
+// thresholds.
+static int mesh_clean_plan(int32_t V, int32_t F, GsrMeshCleanPlan* pl) {
+    if (V < 1) return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: V = %d, need 1 <= V < 2^31", V);
+    if (F < 0 || 3 * (long long)F >= (1ll << 31))
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: F = %d, need 0 <= F and 3 F < 2^31", F);
+    gsr_mesh_clean_plan(V, F, pl);
+    return B200GSR_OK;
+}
+
+int b200gsr_mesh_clean_layout_query(int32_t V, int32_t F, size_t* scratch_bytes) {
+    if (!scratch_bytes) return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: scratch_bytes is null");
+    GsrMeshCleanPlan pl;
+    if (int rc = mesh_clean_plan(V, F, &pl)) return rc;
+    *scratch_bytes = pl.total;
+    return B200GSR_OK;
+}
+
+static int mesh_clean_check(int32_t V, int32_t F, const int32_t* faces, const void* scratch, size_t scratch_bytes,
+                            GsrMeshCleanPlan* pl) {
+    if (int rc = mesh_clean_plan(V, F, pl)) return rc;
+    if ((!faces && F > 0) || !scratch) return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: null pointer");
+    if (reinterpret_cast<uintptr_t>(faces) & 3u) return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: faces must be 4-byte aligned");
+    if (reinterpret_cast<uintptr_t>(scratch) & 255u)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: scratch must be 256-byte aligned");
+    if (scratch_bytes < pl->total)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: scratch holds %zu bytes, need %zu", scratch_bytes, pl->total);
+    return B200GSR_OK;
+}
+
+static int mesh_clean_thresholds(const float* vertices, int32_t min_faces, double min_diameter) {
+    if (!vertices) return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: null pointer");
+    if (reinterpret_cast<uintptr_t>(vertices) & 3u)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: vertices must be 4-byte aligned");
+    if (min_faces < 0) return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: min_faces = %d, need min_faces >= 0", min_faces);
+    if (!std::isfinite(min_diameter) || min_diameter < 0)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: min_diameter = %g, need a finite min_diameter >= 0", min_diameter);
+    return B200GSR_OK;
+}
+
+int b200gsr_mesh_components(int32_t V, int32_t F, const int32_t* faces, int32_t* labels, int32_t* bad, void* scratch,
+                            size_t scratch_bytes, void* stream) {
+    GsrMeshCleanPlan pl;
+    if (int rc = mesh_clean_check(V, F, faces, scratch, scratch_bytes, &pl)) return rc;
+    if (!labels || !bad) return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: null pointer");
+    if ((reinterpret_cast<uintptr_t>(labels) | reinterpret_cast<uintptr_t>(bad)) & 3u)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: labels and bad must be 4-byte aligned");
+    return check_cuda(gsr_launch_mesh_components(pl, faces, labels, bad, static_cast<uint8_t*>(scratch),
+                                                 static_cast<cudaStream_t>(stream)),
+                      "mesh_components");
+}
+
+int b200gsr_mesh_clean_count(int32_t V, int32_t F, const float* vertices, const int32_t* faces, int32_t min_faces,
+                             double min_diameter, int32_t keep_largest, int32_t* totals, void* scratch,
+                             size_t scratch_bytes, void* stream) {
+    GsrMeshCleanPlan pl;
+    if (int rc = mesh_clean_check(V, F, faces, scratch, scratch_bytes, &pl)) return rc;
+    if (int rc = mesh_clean_thresholds(vertices, min_faces, min_diameter)) return rc;
+    if (!totals) return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: null pointer");
+    if (reinterpret_cast<uintptr_t>(totals) & 3u) return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: totals must be 4-byte aligned");
+    return check_cuda(gsr_launch_mesh_clean_count(pl, vertices, faces, min_faces, min_diameter, keep_largest != 0,
+                                                  totals, static_cast<uint8_t*>(scratch),
+                                                  static_cast<cudaStream_t>(stream)),
+                      "mesh_clean_count");
+}
+
+int b200gsr_mesh_clean_emit(int32_t V, int32_t F, const float* vertices, const int32_t* faces, int32_t min_faces,
+                            double min_diameter, int32_t keep_largest, const void* scratch, size_t scratch_bytes,
+                            float* out_vertices, int32_t* out_faces, int32_t* kept, int32_t V_out, int32_t F_out,
+                            void* stream) {
+    GsrMeshCleanPlan pl;
+    if (int rc = mesh_clean_check(V, F, faces, scratch, scratch_bytes, &pl)) return rc;
+    if (int rc = mesh_clean_thresholds(vertices, min_faces, min_diameter)) return rc;
+    if (!out_vertices || !out_faces || !kept) return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: null pointer");
+    if ((reinterpret_cast<uintptr_t>(out_vertices) | reinterpret_cast<uintptr_t>(out_faces) |
+         reinterpret_cast<uintptr_t>(kept)) & 3u)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: out_vertices, out_faces and kept must be 4-byte aligned");
+    if (V_out < 0 || F_out < 0)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_clean: V_out = %d, F_out = %d, need V_out, F_out >= 0", V_out, F_out);
+    return check_cuda(gsr_launch_mesh_clean_emit(pl, vertices, faces, keep_largest != 0,
+                                                 static_cast<const uint8_t*>(scratch), out_vertices, out_faces, kept,
+                                                 V_out, F_out, static_cast<cudaStream_t>(stream)),
+                      "mesh_clean_emit");
 }
 
 #define GSR_ST(x) static_cast<cudaStream_t>(x)

@@ -433,6 +433,26 @@ cudaError_t gsr_launch_mesh_emit(const GsrMeshPlan& p, const float* vol, float i
 cudaError_t gsr_launch_mesh_attributes(const GsrMeshPlan& p, const float* vol, float iso, const uint8_t* scratch,
                                        const float* attributes, float* out, int32_t V, cudaStream_t s);
 
+// ---- mesh components and cleaning (mesh_clean.cu; b200gsr_mesh_components / _clean_*) ---------------------------
+// The scratch layout for V vertices and F faces.
+struct GsrMeshCleanPlan {
+    int V, F;
+    size_t off_parent, off_label, off_ref, off_pass, off_fcount, off_box, off_vstart, off_fstart, off_misc, off_bsums,
+        total;
+};
+// Host only; V and F must already be valid (b200gsr_mesh_clean_layout_query checks them).
+void gsr_mesh_clean_plan(int V, int F, GsrMeshCleanPlan* plan);
+cudaError_t gsr_launch_mesh_components(const GsrMeshCleanPlan& p, const int32_t* faces, int32_t* labels, int32_t* bad,
+                                       uint8_t* scratch, cudaStream_t s);
+cudaError_t gsr_launch_mesh_clean_count(const GsrMeshCleanPlan& p, const float* vertices, const int32_t* faces,
+                                        int min_faces, double min_diameter, bool keep_largest, int32_t* totals,
+                                        uint8_t* scratch, cudaStream_t s);
+// After gsr_launch_mesh_clean_count with the same inputs and scratch: its decisions, gathered
+cudaError_t gsr_launch_mesh_clean_emit(const GsrMeshCleanPlan& p, const float* vertices, const int32_t* faces,
+                                       bool keep_largest, const uint8_t* scratch, float* out_vertices,
+                                       int32_t* out_faces, int32_t* kept, int32_t V_out, int32_t F_out,
+                                       cudaStream_t s);
+
 // simple_knn replacement (knn.cu)
 size_t gsr_knn_scratch_bytes(int P, int* max_cells_out);
 cudaError_t gsr_launch_knn(int P, const float* pts, float* out, uint8_t* scratch, cudaStream_t s);

@@ -8,10 +8,14 @@ The triangulation is not mcubes' table, so the faces differ from mcubes' faces. 
 group's opacity field with ``fields.extract_fields`` and marches it, without the field leaving the device.
 ``marching_cubes(volume, iso, attributes)`` also interpolates a per-point attribute volume onto the vertices, and
 ``extract_coloured_mesh(group)`` uses it to colour the mesh with ``fields.extract_fields_rgb``'s colour field.
+``mesh_components(faces, V)`` labels a mesh's connected components and ``clean_mesh(vertices, faces)`` removes the
+small ones (include/b200gsr_mesh_clean.h), the floaters low-opacity Gaussians leave around an object.
 """
 from __future__ import annotations
 
 import ctypes as C
+import math
+from numbers import Integral, Real
 from typing import Optional, Tuple
 
 import torch
@@ -115,3 +119,132 @@ def extract_coloured_mesh(group, resolution: int = 128, iso: float = 1.0, num_bl
     occ, rgb, center, scale = extract_fields_rgb(group, resolution, num_blocks, relax_ratio)
     vertices, faces, colours = marching_cubes(occ, iso, rgb)
     return (vertices / (int(resolution) - 1) * 2 - 1) / scale + center, faces, colours
+
+
+def _faces_arg(faces, what: str) -> None:
+    if not isinstance(faces, torch.Tensor):
+        raise ValueError(f"{what}: faces must be a torch tensor, got {type(faces).__name__}")
+    if faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError(f"{what}: faces must be [F,3], got shape {tuple(faces.shape)}")
+    if faces.dtype != torch.int32:
+        raise ValueError(f"{what}: faces must be int32, got {faces.dtype}")
+
+
+def _on_cuda(t: torch.Tensor, name: str, what: str) -> None:
+    if t.device.type != "cuda":
+        raise ValueError(f"{what} (b200gsr): {name} must be a CUDA tensor; there is no CPU fallback")
+
+
+def _no_capture(what: str) -> None:
+    if torch.cuda.is_current_stream_capturing():
+        raise RuntimeError(f"{what} reads its totals back to the host, so it cannot be captured into a CUDA graph")
+
+
+def _bad_faces(what: str, bad: int, V: int) -> None:
+    if bad:
+        raise ValueError(f"{what}: {bad} face(s) have a vertex index outside [0, {V})")
+
+
+def _scratch_bytes(lib, V: int, F: int, what: str) -> int:
+    n = C.c_size_t(0)
+    _lib.check(lib.b200gsr_mesh_clean_layout_query(V, F, C.byref(n)), what, ValueError)
+    return int(n.value)
+
+
+def mesh_components(faces: torch.Tensor, num_vertices: int) -> torch.Tensor:
+    """The connected components of a triangle mesh with `num_vertices` vertices: int32 CUDA labels [V].
+
+    Two vertices are connected when some face contains both; a vertex's label is the smallest vertex index in its
+    component, so a vertex no face references is labelled with its own index.  faces: int32 CUDA [F,3] (marching_cubes'
+    faces, say).  Two calls give the same labels.
+
+    Refused with ValueError: faces that are not an int32 CUDA tensor [F,3], num_vertices not an integer in
+    [0, 2^31), 3 F >= 2^31, and a face index outside [0, V) (checked on the device and read back: the call's one host
+    sync, so it cannot be captured into a CUDA graph, RuntimeError)."""
+    if isinstance(num_vertices, bool) or not isinstance(num_vertices, Integral) or not 0 <= num_vertices < 2**31:
+        raise ValueError(f"mesh_components: num_vertices must be an integer in [0, 2^31), got {num_vertices!r}")
+    _faces_arg(faces, "mesh_components")
+    _on_cuda(faces, "faces", "mesh_components")
+    _no_capture("mesh_components")
+    V, F, dev = int(num_vertices), int(faces.shape[0]), faces.device
+    if V == 0:
+        _bad_faces("mesh_components", F, V)
+        return torch.empty(0, dtype=torch.int32, device=dev)
+    lib = _lib.load()
+    nbytes = _scratch_bytes(lib, V, F, "b200gsr_mesh_clean_layout_query")
+    with torch.no_grad(), torch.cuda.device(dev):
+        f = faces.detach().contiguous()
+        labels = torch.empty(V, dtype=torch.int32, device=dev)
+        bad = torch.empty(1, dtype=torch.int32, device=dev)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        ptr = _lib.ptr
+        _lib.check(lib.b200gsr_mesh_components(V, F, ptr(f), ptr(labels), ptr(bad), ptr(scratch), nbytes,
+                                               _lib.stream(dev)), "b200gsr_mesh_components", ValueError)
+        _bad_faces("mesh_components", int(bad.item()), V)   # the call's one host sync
+    return labels
+
+
+def clean_mesh(vertices: torch.Tensor, faces: torch.Tensor, *, min_faces: int = 1, min_diameter: float = 0.0,
+               keep_largest: bool = False) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Remove a mesh's small connected components (the floaters), as DreamGaussian's clean_mesh does with pymeshlab's
+    "remove connected components by face count / by diameter" filters.
+
+    vertices float32 CUDA [V,3], faces int32 CUDA [F,3] on the same device.  Components are mesh_components'.  A
+    component with a face is kept when it has at least `min_faces` faces, when min_diameter is 0 or its box diagonal is
+    at least min_diameter times the diagonal of all referenced vertices (float64, see include/b200gsr_mesh_clean.h;
+    NaN coordinates are skipped), and, with keep_largest, when it also has the most faces of those passing (ties to the
+    smallest label).
+    -> (vertices float32 CUDA [V',3], faces int32 CUDA [F',3], kept int32 CUDA [V']): the referenced vertices of the
+    kept components in input order, their bits unchanged, kept their input indices, and the kept components' faces in
+    input order renumbered into them.  Carry per-vertex data with data[kept].  Unreferenced vertices are always
+    dropped, so the defaults return a mesh whose vertices are all referenced unchanged, kept = arange(V).  Two calls
+    give the same bits; no gradients.
+
+    Refused with ValueError: wrong types, shapes, dtypes or devices; min_faces not an integer in [0, 2^31);
+    min_diameter negative or not finite; 3 F >= 2^31; a face index outside [0, V) (found on the device: the call reads
+    its totals back once, before the outputs are allocated, so it cannot be captured into a CUDA graph, RuntimeError)."""
+    if isinstance(min_faces, bool) or not isinstance(min_faces, Integral) or not 0 <= min_faces < 2**31:
+        raise ValueError(f"clean_mesh: min_faces must be an integer in [0, 2^31), got {min_faces!r}")
+    if isinstance(min_diameter, bool) or not isinstance(min_diameter, Real) or not math.isfinite(min_diameter) \
+            or min_diameter < 0:
+        raise ValueError(f"clean_mesh: min_diameter must be a finite number >= 0, got {min_diameter!r}")
+    if not isinstance(keep_largest, bool):
+        raise ValueError(f"clean_mesh: keep_largest must be a bool, got {keep_largest!r}")
+    if not isinstance(vertices, torch.Tensor):
+        raise ValueError(f"clean_mesh: vertices must be a torch tensor, got {type(vertices).__name__}")
+    if vertices.dim() != 2 or vertices.shape[1] != 3:
+        raise ValueError(f"clean_mesh: vertices must be [V,3], got shape {tuple(vertices.shape)}")
+    if vertices.dtype != torch.float32:
+        raise ValueError(f"clean_mesh: vertices must be float32, got {vertices.dtype}")
+    _faces_arg(faces, "clean_mesh")
+    _on_cuda(vertices, "vertices", "clean_mesh")
+    _on_cuda(faces, "faces", "clean_mesh")
+    if faces.device != vertices.device:
+        raise ValueError(f"clean_mesh: faces are on {faces.device}, vertices on {vertices.device}")
+    _no_capture("clean_mesh")
+    V, F, dev = int(vertices.shape[0]), int(faces.shape[0]), vertices.device
+    if V == 0:
+        _bad_faces("clean_mesh", F, V)
+        return (torch.empty((0, 3), dtype=torch.float32, device=dev), torch.empty((0, 3), dtype=torch.int32, device=dev),
+                torch.empty(0, dtype=torch.int32, device=dev))
+    lib = _lib.load()
+    nbytes = _scratch_bytes(lib, V, F, "b200gsr_mesh_clean_layout_query")
+    args = (int(min_faces), float(min_diameter), int(keep_largest))
+    with torch.no_grad(), torch.cuda.device(dev):
+        v = vertices.detach().contiguous()
+        f = faces.detach().contiguous()
+        totals = torch.empty(3, dtype=torch.int32, device=dev)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        ptr, st = _lib.ptr, _lib.stream(dev)
+        _lib.check(lib.b200gsr_mesh_clean_count(V, F, ptr(v), ptr(f), *args, ptr(totals), ptr(scratch), nbytes, st),
+                   "b200gsr_mesh_clean_count", ValueError)
+        V_out, F_out, bad = (int(n) for n in totals.tolist())      # the call's one host sync
+        _bad_faces("clean_mesh", bad, V)
+        out_v = torch.empty((V_out, 3), dtype=torch.float32, device=dev)
+        out_f = torch.empty((F_out, 3), dtype=torch.int32, device=dev)
+        kept = torch.empty(V_out, dtype=torch.int32, device=dev)
+        if V_out:
+            _lib.check(lib.b200gsr_mesh_clean_emit(V, F, ptr(v), ptr(f), *args, ptr(scratch), nbytes, ptr(out_v),
+                                                   ptr(out_f), ptr(kept), V_out, F_out, st),
+                       "b200gsr_mesh_clean_emit", ValueError)
+    return out_v, out_f, kept

@@ -1,6 +1,7 @@
 """Marching cubes restated in numpy from the rule of include/b200gsr_mesh.h: the cube table generated from the face rule,
 and the surface of a volume with the same vertices, in the same order, with the same float32 rounding.  The checker of
-dreamscene_b200.mesh.marching_cubes; not product code.
+dreamscene_b200.mesh.marching_cubes; not product code.  Also the components and the cleaning of include/b200gsr_mesh_clean.h
+(components, clean_mesh), with scipy's connected_components, the checker of mesh_components and clean_mesh.
 
 Corner c = dx | dy << 1 | dz << 2.  Edge (axis a, corner b), bit a of b clear, runs from b to b | 1 << a; the twelve
 edges are numbered axis by axis, and within an axis by b: x 0..3 (b = 0, 2, 4, 6), y 4..7 (b = 0, 1, 4, 5), z 8..11
@@ -22,6 +23,8 @@ reversed, so the surface would not be a manifold.  Every loop of the 256 cases h
 from __future__ import annotations
 
 import numpy as np
+import scipy.sparse
+from scipy.sparse.csgraph import connected_components
 
 MAX_TRIANGLES = 5
 
@@ -166,3 +169,68 @@ def vertex_attributes(volume, iso, attributes):
     t = ((iso - f0) / (vol.reshape(-1)[q] - f0))[:, None]
     a0, a1 = attr[pts], attr[q]
     return a0 + t * (a1 - a0)
+
+
+def _faces(faces, V):
+    f = np.asarray(faces, dtype=np.int64).reshape(-1, 3)
+    if f.size and (f.min() < 0 or f.max() >= V):
+        raise ValueError("a face index is outside [0, V)")
+    return f
+
+
+def components(faces, V):
+    """-> int64 [V]: each vertex's label, the smallest vertex index of its component.  Two vertices are connected when
+    some face contains both; an unreferenced vertex is its own component."""
+    f = _faces(faces, V)
+    rows = np.concatenate([f[:, 0], f[:, 0]])
+    cols = np.concatenate([f[:, 1], f[:, 2]])
+    graph = scipy.sparse.coo_matrix((np.ones(len(rows), np.int8), (rows, cols)), shape=(V, V))
+    _, lab = connected_components(graph, directed=False)
+    first = np.full(lab.max() + 1, V, np.int64)
+    np.minimum.at(first, lab, np.arange(V))
+    return first[lab]
+
+
+def _diagonal(lo, hi):
+    """Box diagonals in float64 from per-axis float32 min / max [..., 3] (NaN: an empty axis, extent 0), each operation
+    rounded on its own: sqrt((dx*dx + dy*dy) + dz*dz)."""
+    d = np.where(np.isnan(lo), 0.0, hi.astype(np.float64) - lo.astype(np.float64))
+    return np.sqrt((d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]) + d[..., 2] * d[..., 2])
+
+
+def clean_mesh(vertices, faces, min_faces=1, min_diameter=0.0, keep_largest=False):
+    """-> (vertices float32 [V',3], faces int32 [F',3], kept int32 [V']) of include/b200gsr_mesh_clean.h: the kept
+    components' referenced vertices in input order (their bits), their input indices, and their faces in input order
+    renumbered into them."""
+    v = np.ascontiguousarray(vertices, dtype=np.float32).reshape(-1, 3)
+    V = len(v)
+    f = _faces(faces, V)
+    label = components(f, V)
+    ref = np.zeros(V, bool)
+    ref[f.reshape(-1)] = True
+    nfaces = np.bincount(label[f[:, 0]], minlength=V) if len(f) else np.zeros(V, np.int64)
+    # per-root boxes over the referenced vertices, NaN skipped (fmin / fmax); an axis with no value stays NaN
+    lo = np.full((V, 3), np.nan, np.float32)
+    hi = np.full((V, 3), np.nan, np.float32)
+    np.fmin.at(lo, label[ref], v[ref])
+    np.fmax.at(hi, label[ref], v[ref])
+    with np.errstate(all="ignore"):
+        mesh_lo = np.fmin.reduce(v[ref], axis=0, initial=np.nan) if ref.any() else np.full(3, np.nan, np.float32)
+        mesh_hi = np.fmax.reduce(v[ref], axis=0, initial=np.nan) if ref.any() else np.full(3, np.nan, np.float32)
+        d_all = float(_diagonal(mesh_lo, mesh_hi))
+        roots = np.flatnonzero(ref & (label == np.arange(V)))
+        ok = nfaces[roots] >= min_faces
+        if min_diameter != 0:
+            ok &= _diagonal(lo[roots], hi[roots]) >= float(min_diameter) * d_all
+    keep_root = np.zeros(V, bool)
+    passing = roots[ok]
+    if keep_largest:
+        if len(passing):
+            keep_root[passing[np.argmax(nfaces[passing])]] = True        # argmax: the first, the smallest label
+    else:
+        keep_root[passing] = True
+    vkeep = ref & keep_root[label]
+    fkeep = keep_root[label[f[:, 0]]] if len(f) else np.zeros(0, bool)
+    kept = np.flatnonzero(vkeep)
+    new_index = np.cumsum(vkeep) - 1
+    return v[kept], new_index[f[fkeep]].astype(np.int32).reshape(-1, 3), kept.astype(np.int32)
