@@ -10,7 +10,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200gsr.so")
 SOURCES = ["api.cu", "project.cu", "binning.cu", "composite.cu", "knn.cu", "assemble.cu", "postprocess.cu", "densify.cu",
-           "optim.cu", "loss.cu", "fields.cu", "mesh.cu", "mesh_clean.cu"]
+           "optim.cu", "loss.cu", "fields.cu", "mesh.cu", "mesh_clean.cu",
+           "mesh_decimate.cu"]
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "scene_math.cuh"),
            os.path.join(HERE, "..", "include", "b200gsr.h"), os.path.join(HERE, "..", "include", "b200gsr_scene.h"),
            os.path.join(HERE, "..", "include", "b200gsr_step.h"), os.path.join(HERE, "..", "include", "b200gsr_loss.h"),
@@ -22,7 +23,8 @@ HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "scene_math.cuh"
            os.path.join(HERE, "..", "include", "b200gsr_fields.h"),
            os.path.join(HERE, "..", "include", "b200gsr_mesh.h"),
            os.path.join(HERE, "..", "include", "b200gsr_mesh_colour.h"),
-           os.path.join(HERE, "..", "include", "b200gsr_mesh_clean.h")]
+           os.path.join(HERE, "..", "include", "b200gsr_mesh_clean.h"),
+           os.path.join(HERE, "..", "include", "b200gsr_mesh_decimate.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

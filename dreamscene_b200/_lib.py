@@ -1,8 +1,8 @@
 """ctypes binding of libb200gsr.so (include/b200gsr.h, include/b200gsr_scene.h, include/b200gsr_step.h,
 include/b200gsr_loss.h, include/b200gsr_frozen.h, include/b200gsr_stats.h,
 include/b200gsr_reserve.h, include/b200gsr_frames.h, include/b200gsr_views_frozen.h, include/b200gsr_views_stats.h,
-include/b200gsr_fields.h, include/b200gsr_mesh.h, include/b200gsr_mesh_colour.h, include/b200gsr_mesh_clean.h).  Fails
-loudly if the library is missing: there is NO CPU or PyTorch fallback in the product path."""
+include/b200gsr_fields.h, include/b200gsr_mesh.h, include/b200gsr_mesh_colour.h, include/b200gsr_mesh_clean.h,
+include/b200gsr_mesh_decimate.h).  Fails loudly if the library is missing: there is NO CPU or PyTorch fallback in the product path."""
 from __future__ import annotations
 
 import ctypes as C
@@ -269,6 +269,16 @@ MESH_CLEAN_SIGNATURES = {
     "b200gsr_mesh_clean_emit": (C.c_int, [i32, i32, vp, vp, i32, C.c_double, i32, vp, sz, vp, vp, vp, i32, i32, vp]),
 }
 
+# The decimation entry points of include/b200gsr_mesh_decimate.h (same library), in that header's order.
+MESH_DECIMATE_SIGNATURES = {
+    "b200gsr_mesh_decimate_layout_query": (C.c_int, [i32, i32, _P(sz)]),
+    "b200gsr_mesh_decimate_begin": (C.c_int, [i32, i32, vp, vp, i32, i32, vp, vp, sz, vp]),
+    "b200gsr_mesh_decimate_rounds": (C.c_int, [i32, i32, i32, vp, vp, sz, vp]),
+    "b200gsr_mesh_decimate_emit": (C.c_int, [i32, i32, vp, vp, sz, vp, vp, vp, i32, i32, vp]),
+}
+DECIMATE_MAX_VALENCE = 32           # B200GSR_DECIMATE_MAX_VALENCE
+DECIMATE_STATUS_WORDS = 6           # B200GSR_DECIMATE_STATUS_WORDS
+
 _lib = None
 ABI_VERSION = 3
 ERR_BAD_ARG = -1
@@ -301,7 +311,7 @@ def load():
                                       **FROZEN_SIGNATURES, **STATS_SIGNATURES, **RESERVE_SIGNATURES,
                                       **FRAMES_SIGNATURES, **VIEWS_FROZEN_SIGNATURES, **VIEWS_STATS_SIGNATURES,
                                       **FIELDS_SIGNATURES, **MESH_SIGNATURES, **MESH_COLOUR_SIGNATURES,
-                                      **MESH_CLEAN_SIGNATURES}.items():
+                                      **MESH_CLEAN_SIGNATURES, **MESH_DECIMATE_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.b200gsr_version() != ABI_VERSION:

@@ -13,6 +13,7 @@
 #include "../../include/b200gsr_mesh.h"
 #include "../../include/b200gsr_mesh_colour.h"
 #include "../../include/b200gsr_mesh_clean.h"
+#include "../../include/b200gsr_mesh_decimate.h"
 
 #include <cmath>
 #include <cstdarg>
@@ -1101,6 +1102,82 @@ int b200gsr_mesh_clean_emit(int32_t V, int32_t F, const float* vertices, const i
                                                  static_cast<const uint8_t*>(scratch), out_vertices, out_faces, kept,
                                                  V_out, F_out, static_cast<cudaStream_t>(stream)),
                       "mesh_clean_emit");
+}
+
+// Mesh decimation (include/b200gsr_mesh_decimate.h): the sizes first, then the pointers, then the other values.
+static int mesh_decimate_plan(int32_t V, int32_t F, GsrMeshDecimatePlan* pl) {
+    if (V < 1) return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: V = %d, need 1 <= V < 2^31", V);
+    if (F < 0 || 3 * (long long)F >= (1ll << 31))
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: F = %d, need 0 <= F and 3 F < 2^31", F);
+    gsr_mesh_decimate_plan(V, F, pl);
+    return B200GSR_OK;
+}
+
+int b200gsr_mesh_decimate_layout_query(int32_t V, int32_t F, size_t* scratch_bytes) {
+    if (!scratch_bytes) return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: scratch_bytes is null");
+    GsrMeshDecimatePlan pl;
+    if (int rc = mesh_decimate_plan(V, F, &pl)) return rc;
+    *scratch_bytes = pl.total;
+    return B200GSR_OK;
+}
+
+static int mesh_decimate_check(int32_t V, int32_t F, const int32_t* status, const void* scratch, size_t scratch_bytes,
+                               GsrMeshDecimatePlan* pl) {
+    if (int rc = mesh_decimate_plan(V, F, pl)) return rc;
+    if (!status || !scratch) return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: null pointer");
+    if (reinterpret_cast<uintptr_t>(status) & 3u)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: status must be 4-byte aligned");
+    if (reinterpret_cast<uintptr_t>(scratch) & 255u)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: scratch must be 256-byte aligned");
+    if (scratch_bytes < pl->total)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: scratch holds %zu bytes, need %zu", scratch_bytes, pl->total);
+    return B200GSR_OK;
+}
+
+int b200gsr_mesh_decimate_begin(int32_t V, int32_t F, const float* vertices, const int32_t* faces, int32_t target_faces,
+                                int32_t optimal_placement, int32_t* status, void* scratch, size_t scratch_bytes,
+                                void* stream) {
+    GsrMeshDecimatePlan pl;
+    if (int rc = mesh_decimate_check(V, F, status, scratch, scratch_bytes, &pl)) return rc;
+    if (!vertices || (!faces && F > 0)) return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: null pointer");
+    if ((reinterpret_cast<uintptr_t>(vertices) | reinterpret_cast<uintptr_t>(faces)) & 3u)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: vertices and faces must be 4-byte aligned");
+    if (target_faces < 0)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: target_faces = %d, need target_faces >= 0", target_faces);
+    return check_cuda(gsr_launch_mesh_decimate_begin(pl, vertices, faces, target_faces, optimal_placement != 0, status,
+                                                     static_cast<uint8_t*>(scratch), static_cast<cudaStream_t>(stream)),
+                      "mesh_decimate_begin");
+}
+
+int b200gsr_mesh_decimate_rounds(int32_t V, int32_t F, int32_t rounds, int32_t* status, void* scratch,
+                                 size_t scratch_bytes, void* stream) {
+    GsrMeshDecimatePlan pl;
+    if (int rc = mesh_decimate_check(V, F, status, scratch, scratch_bytes, &pl)) return rc;
+    if (rounds < 0) return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: rounds = %d, need rounds >= 0", rounds);
+    return check_cuda(gsr_launch_mesh_decimate_rounds(pl, rounds, status, static_cast<uint8_t*>(scratch),
+                                                      static_cast<cudaStream_t>(stream)),
+                      "mesh_decimate_rounds");
+}
+
+int b200gsr_mesh_decimate_emit(int32_t V, int32_t F, const float* vertices, const void* scratch, size_t scratch_bytes,
+                               float* out_vertices, int32_t* out_faces, int32_t* kept, int32_t V_out, int32_t F_out,
+                               void* stream) {
+    GsrMeshDecimatePlan pl;
+    if (int rc = mesh_decimate_plan(V, F, &pl)) return rc;
+    if (!vertices || !scratch || !out_vertices || !out_faces || !kept)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: null pointer");
+    if ((reinterpret_cast<uintptr_t>(vertices) | reinterpret_cast<uintptr_t>(out_vertices) |
+         reinterpret_cast<uintptr_t>(out_faces) | reinterpret_cast<uintptr_t>(kept)) & 3u)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: vertices, out_vertices, out_faces and kept must be 4-byte aligned");
+    if (reinterpret_cast<uintptr_t>(scratch) & 255u)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: scratch must be 256-byte aligned");
+    if (scratch_bytes < pl.total)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: scratch holds %zu bytes, need %zu", scratch_bytes, pl.total);
+    if (V_out < 0 || F_out < 0)
+        return fail(B200GSR_ERR_BAD_ARG, "mesh_decimate: V_out = %d, F_out = %d, need V_out, F_out >= 0", V_out, F_out);
+    return check_cuda(gsr_launch_mesh_decimate_emit(pl, vertices, static_cast<const uint8_t*>(scratch), out_vertices,
+                                                    out_faces, kept, V_out, F_out, static_cast<cudaStream_t>(stream)),
+                      "mesh_decimate_emit");
 }
 
 #define GSR_ST(x) static_cast<cudaStream_t>(x)

@@ -453,6 +453,27 @@ cudaError_t gsr_launch_mesh_clean_emit(const GsrMeshCleanPlan& p, const float* v
                                        int32_t* out_faces, int32_t* kept, int32_t V_out, int32_t F_out,
                                        cudaStream_t s);
 
+// ---- mesh decimation (mesh_decimate.cu; b200gsr_mesh_decimate_*) -------------------------------------------------
+// The scratch layout for V vertices and F faces; cub_bytes is the room reserved for cub's radix-sort storage.
+struct GsrMeshDecimatePlan {
+    int V, F;
+    size_t cub_bytes;
+    size_t off_state, off_faces, off_keys, off_vals, off_cub, off_start, off_ep, off_eq, off_pos, off_Q, off_xb,
+        off_m_hi, off_M_hi, off_sel, off_m_lo, off_M_lo, off_kreg, off_moved, off_ref, off_vstart, off_fstart,
+        off_bsums, total;
+};
+// Host only; V and F must already be valid (b200gsr_mesh_decimate_layout_query checks them).
+void gsr_mesh_decimate_plan(int V, int F, GsrMeshDecimatePlan* plan);
+cudaError_t gsr_launch_mesh_decimate_begin(const GsrMeshDecimatePlan& p, const float* vertices, const int32_t* faces,
+                                           int target_faces, bool optimal_placement, int32_t* status, uint8_t* scratch,
+                                           cudaStream_t s);
+cudaError_t gsr_launch_mesh_decimate_rounds(const GsrMeshDecimatePlan& p, int rounds, int32_t* status,
+                                            uint8_t* scratch, cudaStream_t s);
+// After the rounds report done: the last count's offsets, gathered
+cudaError_t gsr_launch_mesh_decimate_emit(const GsrMeshDecimatePlan& p, const float* vertices, const uint8_t* scratch,
+                                          float* out_vertices, int32_t* out_faces, int32_t* kept, int32_t V_out,
+                                          int32_t F_out, cudaStream_t s);
+
 // simple_knn replacement (knn.cu)
 size_t gsr_knn_scratch_bytes(int P, int* max_cells_out);
 cudaError_t gsr_launch_knn(int P, const float* pts, float* out, uint8_t* scratch, cudaStream_t s);

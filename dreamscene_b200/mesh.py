@@ -10,6 +10,8 @@ group's opacity field with ``fields.extract_fields`` and marches it, without the
 ``extract_coloured_mesh(group)`` uses it to colour the mesh with ``fields.extract_fields_rgb``'s colour field.
 ``mesh_components(faces, V)`` labels a mesh's connected components and ``clean_mesh(vertices, faces)`` removes the
 small ones (include/b200gsr_mesh_clean.h), the floaters low-opacity Gaussians leave around an object.
+``decimate_mesh(vertices, faces, target_faces)`` reduces a mesh to a target face count by quadric edge collapse
+(include/b200gsr_mesh_decimate.h), as DreamGaussian's export does with pymeshlab before writing the mesh.
 """
 from __future__ import annotations
 
@@ -247,4 +249,82 @@ def clean_mesh(vertices: torch.Tensor, faces: torch.Tensor, *, min_faces: int = 
             _lib.check(lib.b200gsr_mesh_clean_emit(V, F, ptr(v), ptr(f), *args, ptr(scratch), nbytes, ptr(out_v),
                                                    ptr(out_f), ptr(kept), V_out, F_out, st),
                        "b200gsr_mesh_clean_emit", ValueError)
+    return out_v, out_f, kept
+
+
+DECIMATE_BATCH = 8          # rounds per b200gsr_mesh_decimate_rounds call: one status read-back each
+
+
+def decimate_mesh(vertices: torch.Tensor, faces: torch.Tensor, target_faces: int, *,
+                  optimal_placement: bool = True) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Reduce a mesh to `target_faces` faces by quadric edge collapse, as DreamGaussian's decimate_mesh does with
+    pymeshlab's meshing_decimation_quadric_edge_collapse (include/b200gsr_mesh_decimate.h states every rule).
+
+    vertices float32 CUDA [V,3], faces int32 CUDA [F,3] on the same device.  Each face's plane quadric, weighted by its
+    area, is summed per vertex in float64; edges are collapsed in rounds of independent edges, each round's cheapest
+    edges first.  An edge collapses only between two vertices whose faces form one closed, consistently oriented fan,
+    when the two share exactly two neighbours, when the result keeps valence >= 3 and when no surviving face turns
+    over, so boundaries, non-manifold parts and each component's topology stay as they are.  With optimal_placement the
+    survivor moves to the quadric's minimum (Cramer's rule, falling back to the best of the two ends and the midpoint
+    when the system is near singular), without it to that best of three.  Rounds run while F > target_faces and an
+    edge can collapse; the last round applies only the cheapest of its edges, so F' is target_faces or
+    target_faces - 1 unless the mesh runs out of collapsible edges first.
+    -> (vertices float32 CUDA [V',3], faces int32 CUDA [F',3], kept int32 CUDA [V']): the surviving referenced
+    vertices in input order, kept their input indices (carry per-vertex data with data[kept]; a vertex that absorbed
+    others carries its own index), and the surviving faces in input order, renumbered.  With F <= target_faces, or no
+    collapsible edge, this is clean_mesh(vertices, faces).  Two calls give the same bits; no gradients.
+
+    The rounds run DECIMATE_BATCH (8) at a time on the device; after each batch the call reads back one status record,
+    so it waits for the device 1 + ceil(rounds / 8) times (a tenfold reduction of the object meshes in
+    BASELINE.md takes about 30 rounds), and it cannot be captured into a CUDA graph (RuntimeError).
+    Refused with ValueError: what clean_mesh refuses; target_faces not an integer in [0, 2^31); optimal_placement not
+    a bool; a face index outside [0, V) (found on the device)."""
+    if isinstance(target_faces, bool) or not isinstance(target_faces, Integral) or not 0 <= target_faces < 2**31:
+        raise ValueError(f"decimate_mesh: target_faces must be an integer in [0, 2^31), got {target_faces!r}")
+    if not isinstance(optimal_placement, bool):
+        raise ValueError(f"decimate_mesh: optimal_placement must be a bool, got {optimal_placement!r}")
+    if not isinstance(vertices, torch.Tensor):
+        raise ValueError(f"decimate_mesh: vertices must be a torch tensor, got {type(vertices).__name__}")
+    if vertices.dim() != 2 or vertices.shape[1] != 3:
+        raise ValueError(f"decimate_mesh: vertices must be [V,3], got shape {tuple(vertices.shape)}")
+    if vertices.dtype != torch.float32:
+        raise ValueError(f"decimate_mesh: vertices must be float32, got {vertices.dtype}")
+    _faces_arg(faces, "decimate_mesh")
+    _on_cuda(vertices, "vertices", "decimate_mesh")
+    _on_cuda(faces, "faces", "decimate_mesh")
+    if faces.device != vertices.device:
+        raise ValueError(f"decimate_mesh: faces are on {faces.device}, vertices on {vertices.device}")
+    _no_capture("decimate_mesh")
+    V, F, dev = int(vertices.shape[0]), int(faces.shape[0]), vertices.device
+    if V == 0:
+        _bad_faces("decimate_mesh", F, V)
+        return (torch.empty((0, 3), dtype=torch.float32, device=dev), torch.empty((0, 3), dtype=torch.int32, device=dev),
+                torch.empty(0, dtype=torch.int32, device=dev))
+    lib = _lib.load()
+    n = C.c_size_t(0)
+    _lib.check(lib.b200gsr_mesh_decimate_layout_query(V, F, C.byref(n)), "b200gsr_mesh_decimate_layout_query",
+               ValueError)
+    nbytes = int(n.value)
+    with torch.no_grad(), torch.cuda.device(dev):
+        v = vertices.detach().contiguous()
+        f = faces.detach().contiguous()
+        status = torch.empty(_lib.DECIMATE_STATUS_WORDS, dtype=torch.int32, device=dev)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        ptr, st = _lib.ptr, _lib.stream(dev)
+        _lib.check(lib.b200gsr_mesh_decimate_begin(V, F, ptr(v), ptr(f), int(target_faces), int(optimal_placement),
+                                                   ptr(status), ptr(scratch), nbytes, st),
+                   "b200gsr_mesh_decimate_begin", ValueError)
+        _, _, done, bad, V_out, F_out = status.tolist()
+        _bad_faces("decimate_mesh", bad, V)
+        while not done:
+            _lib.check(lib.b200gsr_mesh_decimate_rounds(V, F, DECIMATE_BATCH, ptr(status), ptr(scratch), nbytes, st),
+                       "b200gsr_mesh_decimate_rounds", ValueError)
+            _, _, done, _, V_out, F_out = status.tolist()
+        out_v = torch.empty((V_out, 3), dtype=torch.float32, device=dev)
+        out_f = torch.empty((F_out, 3), dtype=torch.int32, device=dev)
+        kept = torch.empty(V_out, dtype=torch.int32, device=dev)
+        if V_out:
+            _lib.check(lib.b200gsr_mesh_decimate_emit(V, F, ptr(v), ptr(scratch), nbytes, ptr(out_v), ptr(out_f),
+                                                      ptr(kept), V_out, F_out, st),
+                       "b200gsr_mesh_decimate_emit", ValueError)
     return out_v, out_f, kept
